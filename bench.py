@@ -1,7 +1,7 @@
 # coding=utf-8
-"""Benchmark of the Multiverse ConvRNN hot path on B200 (contract: see the task statement).
+"""Benchmark of the Multiverse ConvRNN hot path on the H100.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c4|c3] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c4|c3|c5] [--impl reference] [--dump-outputs DIR]
   (N>1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...)
 
 A "step" is one pass of the hot path over one batch of synthetic trajectories
@@ -44,6 +44,33 @@ WORKLOADS = {
                desc="train.py step: fwd + CE/Huber/wd loss + BPTT + clip + Adadelta, two scales, "
                     "data-parallel (one NCCL all-reduce of the 85 MB gradient bucket)"),
 }
+
+
+DUMP_BUDGET = 60_000_000    # bytes of --dump-outputs in all, .npy headers included (under 64 MB)
+
+
+def dump_sample(named):
+  """Host copies of the named arrays (torch tensors or numpy) for --dump-outputs: floating point as float32, integers
+  as float64 (exact).  An array larger than its equal share of DUMP_BUDGET is replaced by a fixed sample of its
+  flattened elements - evenly spaced indices, taken on the device - so two builds fed the same arguments write
+  comparable files."""
+  share = DUMP_BUDGET // max(1, len(named)) - 256          # room for the .npy header
+  out = {}
+  for name, a in named.items():
+    t = a.detach() if torch.is_tensor(a) else torch.from_numpy(np.ascontiguousarray(a))
+    t = t.to(torch.float32 if t.is_floating_point() else torch.float64)
+    if t.numel() * t.element_size() > share:
+      k = share // t.element_size()
+      idx = torch.linspace(0, t.numel() - 1, k, dtype=torch.float64, device=t.device).round().long()
+      t = t.reshape(-1)[idx]
+    out[name] = t.cpu().numpy()
+  return out
+
+
+def write_dump(dirname, arrays):
+  os.makedirs(dirname, exist_ok=True)
+  for name, a in arrays.items():
+    np.save(os.path.join(dirname, name + ".npy"), a)
 
 
 def cell_flops(h, w, cx):
@@ -111,7 +138,7 @@ def load_peaks():
     d = json.load(open(p))
     return dict(bf16=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 hbm=d["hbm_gbs"], source="measured (MEASURED_PEAKS.json)")
-  return dict(bf16=1590.0, bf16_sustained=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+  return dict(bf16=989.0, bf16_sustained=989.0, hbm=3350.0, source="H100 SXM data sheet (dense, 700 W), not measured")
 
 
 def cpu_reference_run(cfg_over, n_sample, seed, repeats=1):
@@ -120,8 +147,8 @@ def cpu_reference_run(cfg_over, n_sample, seed, repeats=1):
   (trajectories/sec, seconds, threads)."""
   from multiverse_b200 import synthetic
   from oracle import multiverse_ref_torch as RT
-  # all host threads up to 32: on the 128-thread GPU boxes more threads make the oneDNN convolutions of
-  # this small-batch recurrent model SLOWER (profiles/r01_bench.json: 16-32 threads are the optimum)
+  # all host threads up to 32: beyond that, more threads make the oneDNN convolutions of this small-batch recurrent
+  # model slower
   threads = int(os.environ.get("MVB_CPU_THREADS", "0")) or min(32, os.cpu_count() or 1)
   torch.set_num_threads(threads)
   cfg = synthetic.make_config(batch_size=n_sample, **cfg_over)
@@ -152,7 +179,7 @@ def run_reference(args, wl):
               higher_is_better=True, scaling="strong", vs_baseline=None, dtype="f32", data="synthetic",
               config=dict(workload=args.workload + ": " + wl["desc"], global_batch=wl["global_batch"],
                           sample_per_step=n_sample, obs_len=8, pred_len=12,
-                          note="same workload as the b200 arm; each CPU step is a bounded sample of %d trajectories of "
+                          note="same workload as the GPU arm; each CPU step is a bounded sample of %d trajectories of "
                                "the %d-trajectory batch (the CPU rate does not depend on the batch size)"
                                % (n_sample, wl["global_batch"])),
               cpu_baseline=dict(value=value, unit="trajectories/s", cores=threads, kind="port",
@@ -211,7 +238,7 @@ def ddp_equivalence(ctx):
   return res
 
 
-def run_train(args, name, ctx, steps, warmup, cpu_baseline=True):
+def run_train(args, name, ctx, steps, warmup, cpu_baseline=True, dump=True):
   """Workload c5: one Trainer.step (code/pred_models.py:1719-1742) per timed step.  Returns the record on rank 0."""
   from multiverse_b200 import ops, synthetic
   from multiverse_b200.train_engine import TrainEngine
@@ -240,8 +267,8 @@ def run_train(args, name, ctx, steps, warmup, cpu_baseline=True):
       dist.barrier()
     torch.cuda.synchronize()
 
-  # L2 rule of the timing contract: the state one step streams through (c, h, operand planes of every launch) is
-  # far larger than the 126 MB L2 at the default sizes; when a shard is small enough to fit (greedy rollouts at
+  # The state one step streams through (c, h, operand planes of every launch) is far larger than the 50 MB L2 at the
+  # default sizes; when a shard is small enough to fit (greedy rollouts at
   # 32 trajectories per GPU), a 256 MB buffer is overwritten between the timed iterations and each iteration is
   # timed by its own pair of events (the flush is outside every pair).
   h0_, w0_ = [g for g, u in zip(cfg.scene_grids, cfg.use_grids) if u][0]
@@ -281,16 +308,28 @@ def run_train(args, name, ctx, steps, warmup, cpu_baseline=True):
     sampler.start()
   ops.reset_launch_count()
   eng.allreduce_events = []
-  ms_total = timed(lambda: eng.train_step(feeds, lr, dist, mb), steps)
+  last = {}
+
+  def train_step():
+    last["losses"] = eng.train_step(feeds, lr, dist, mb)[0]
+  ms_total = timed(train_step, steps)
   launches = ops.launch_count()
+  dumped = None
+  if dump and args.dump_outputs and rank == 0:
+    # the caller of a training step receives its losses and the updated weights
+    named = dict(losses=last["losses"])
+    named.update(("weight_" + k.replace("/", "_"), eng.params[k]) for k in eng.names)
+    dumped = dump_sample(named)
   ar_events, eng.allreduce_events = eng.allreduce_events, None
   clocks = sampler.stop() if rank == 0 else None
+  if dumped is not None:
+    write_dump(args.dump_outputs, dumped)
   ar = None
   if ar_events:
     # the one collective of the path (85 MB fp32 gradient bucket), device time per step.  A rank that arrives early
     # waits inside the collective for its peers (the ranks' fwd+bwd times differ by 1-2 % under the power cap), so
     # the MAX over ranks measures skew + transfer and the MIN - the last arriver's - the transfer itself: bus
-    # bandwidth 2 (G-1)/G * bytes / min time (the NCCL convention; 725 GB/s measured at 1 GiB on this pool).
+    # bandwidth 2 (G-1)/G * bytes / min time (the NCCL convention).
     mine = float(np.mean([a.elapsed_time(b) for a, b in ar_events]))
     ar_max = torch.tensor([mine], device=dev, dtype=torch.float64)
     ar_min = torch.tensor([mine], device=dev, dtype=torch.float64)
@@ -338,7 +377,7 @@ def run_train(args, name, ctx, steps, warmup, cpu_baseline=True):
                           micro_batch=mb, arithmetic="fp32-grade: bf16x%d operand planes, fp32 accumulate" % args.planes,
                           parallelism="data-parallel x%d, NCCL all-reduce of %.1f MB fp32 grads"
                           % (world, grad_mb),
-                          l2="activation store >> 126 MB L2, no flush needed"),
+                          l2="activation store >> 50 MB L2, no flush needed"),
               clocks=clocks,
               e2e=dict(value=gb * steps / (ms_e2e * 1e-3), unit="trajectories/s", ms_per_step=ms_e2e / steps,
                        h2d_bytes_per_step=h2d_bytes * world, d2h_bytes_per_step=host_loss.numel() * 4),
@@ -362,6 +401,9 @@ def main():
   ap.add_argument("--planes", type=int, default=2)
   ap.add_argument("--no-cpu-baseline", action="store_true")
   ap.add_argument("--no-extras", action="store_true", help="default run: skip the c3 / c5 sub-records")
+  ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                  help="write what the last timed step of the main workload computed to DIR/<name>.npy "
+                       "(with --gpus N > 1: rank 0's shard of the batch)")
   args = ap.parse_args()
   extras = args.workload is None and not args.no_extras and not args.global_batch
   args.workload = args.workload or "c4"
@@ -376,8 +418,8 @@ def main():
   if extras:
     # the other two north_star workloads in the same invocation, at the same N and in the same process group
     sub = {}
-    sub["c3"] = run_infer(args, "c3", ctx, max(args.steps, 10), args.warmup, cpu_baseline=False)
-    sub["c5"] = run_train(args, "c5", ctx, max(2, min(args.steps, 3)), args.warmup, cpu_baseline=False)
+    sub["c3"] = run_infer(args, "c3", ctx, args.steps, args.warmup, cpu_baseline=False, dump=False)
+    sub["c5"] = run_train(args, "c5", ctx, args.steps, args.warmup, cpu_baseline=False, dump=False)
     chk = ddp_equivalence(ctx) if world > 1 else None
     if rank == 0:
       sub["c5"]["ddp_equivalence"] = chk if chk is not None else "n/a at N=1 (tests/test_ddp_gpu.py runs it on 2 GPUs)"
@@ -388,7 +430,7 @@ def main():
     dist.destroy_process_group()
 
 
-def run_infer(args, name, ctx, steps, warmup, cpu_baseline=True):
+def run_infer(args, name, ctx, steps, warmup, cpu_baseline=True, dump=True):
   """Workloads c4 / c3: one forward (all decoders) per timed step.  Returns the record on rank 0."""
   from multiverse_b200 import ops, synthetic
   from multiverse_b200.engine import ConvRNNEngine
@@ -437,8 +479,8 @@ def run_infer(args, name, ctx, steps, warmup, cpu_baseline=True):
       dist.barrier()
     torch.cuda.synchronize()
 
-  # L2 rule of the timing contract: the state one step streams through (c, h, operand planes of every launch) is
-  # far larger than the 126 MB L2 at the default sizes; when a shard is small enough to fit (greedy rollouts at
+  # The state one step streams through (c, h, operand planes of every launch) is far larger than the 50 MB L2 at the
+  # default sizes; when a shard is small enough to fit (greedy rollouts at
   # 32 trajectories per GPU), a 256 MB buffer is overwritten between the timed iterations and each iteration is
   # timed by its own pair of events (the flush is outside every pair).
   h0_, w0_ = [g for g, u in zip(cfg.scene_grids, cfg.use_grids) if u][0]
@@ -480,7 +522,10 @@ def run_infer(args, name, ctx, steps, warmup, cpu_baseline=True):
   graph_mode = os.environ.get("MVB_CUDA_GRAPH", "")
   use_graph = (graph_mode == "1") if graph_mode in ("0", "1") else \
       rows_all <= int(os.environ.get("MVB_GRAPH_MAX_ROWS", "2000"))
-  step_fn = (lambda: eng.forward_graph(dev_feeds)) if use_graph else (lambda: eng.forward(dev_feeds))
+  last = {}
+
+  def step_fn():
+    last["out"] = eng.forward_graph(dev_feeds) if use_graph else eng.forward(dev_feeds)
   for _ in range(max(warmup, 3 if use_graph else 0)):     # a signature is captured at its second sight
     step_fn()
   sampler = ClockSampler(local)
@@ -491,6 +536,16 @@ def run_infer(args, name, ctx, steps, warmup, cpu_baseline=True):
     eng.cell_events = []
   ms_total = timed(step_fn, steps)
   launches = ops.launch_count()
+  dumped = None
+  if dump and args.dump_outputs and rank == 0:
+    out = last["out"]
+    named = {}
+    for key in ("grid_pred_decoded", "grid_pred_reg_decoded"):
+      named.update(("%s_%d" % (key, i), t) for i, t in enumerate(out[key]) if torch.is_tensor(t))
+    if out["beam_outputs"] is not None:
+      named.update(zip(("beam_logits", "beam_ids", "beam_logprobs"), out["beam_outputs"]))
+    dumped = dump_sample(named)
+  last.clear()
   if use_graph:
     # graph replays do not pass through the C ABI's launch counter: count one launch-by-launch forward
     ops.reset_launch_count()
@@ -501,6 +556,8 @@ def run_infer(args, name, ctx, steps, warmup, cpu_baseline=True):
   events = eng.cell_events
   eng.cell_events = None
   clocks = sampler.stop() if rank == 0 else None
+  if dumped is not None:
+    write_dump(args.dump_outputs, dumped)
   value = gb * steps / (ms_total * 1e-3)
 
   # ---- end to end through the reference-facing call (`e2e`) --------------------------------------
@@ -578,25 +635,19 @@ def run_infer(args, name, ctx, steps, warmup, cpu_baseline=True):
   fl = cell_flops(h0, w0, cfg.emb_size) * rows
   achieved = fl / (avg_ms * 1e-3) / 1e12
   traffic = None
-  tp = os.path.join(ROOT, "profiles", "cell_traffic.json")
-  if os.path.exists(tp):
-    try:
-      traffic = json.load(open(tp)).get("%s_rows%d" % (name, rows))
-    except Exception:
-      traffic = None
   passes = args.planes * (args.planes + 1) // 2
   if f16f8:
     arith = ("fp32-grade: operands as one fp16 + two e4m3 planes (f16f8), per product one fp16 tensor pass + two "
-             "e4m3 passes at twice the rate into one fp32 TMEM accumulator (2 bf16-pass equivalents), fp32 gates/state; "
+             "e4m3 passes at twice the rate into one fp32 accumulator (2 bf16-pass equivalents), fp32 gates/state; "
              "the regression encoder (raw pixel offsets) keeps 2 bf16 planes / 3 passes")
     ceil_note = ("fp32 parity costs one fp16 + two e4m3 tensor passes per product = 2 bf16-pass equivalents, so the "
                  "ceiling of this fraction against the bf16 peak is 0.5")
   else:
-    arith = ("fp32-grade: operands split into %d bf16 planes, %d tcgen05 passes per product, fp32 TMEM accumulate, "
+    arith = ("fp32-grade: operands split into %d bf16 planes, %d wgmma passes per product, fp32 accumulate, "
              "fp32 gates/state" % (args.planes, passes))
     ceil_note = ("fp32 parity needs %d bf16 tensor passes per product, so the ceiling of this fraction is %.3f"
                  % (passes, 1.0 / passes))
-  roofline = dict(bound="tensor", kernel="cell_fwd_kernel<%s, CTA pair cta_group::2> (%s step, %d sample rows of %dx%d)" % (
+  roofline = dict(bound="tensor", kernel="cell_fwd_kernel<%s, cluster pair, weight multicast> (%s step, %d sample rows of %dx%d)" % (
                       "f16f8" if f16f8 else "P=%d" % args.planes, dom_tag, rows, h0, w0),
                   achieved=achieved, peak=peaks["bf16_sustained"], unit="TFLOP/s",
                   frac=achieved / peaks["bf16_sustained"], traffic=traffic,
@@ -629,7 +680,7 @@ def run_infer(args, name, ctx, steps, warmup, cpu_baseline=True):
                                      "concurrent streams (forwards of <= MVB_GRAPH_MAX_ROWS rows x beams, the rule of "
                                      "the public call); roofline events from a launch-by-launch region of the same "
                                      "length right after" if use_graph else "launch by launch on one stream"),
-                          l2=("working set per step (%.2f GB of state) >> 126 MB L2, no flush needed"
+                          l2=("working set per step (%.2f GB of state) >> 50 MB L2, no flush needed"
                               % (state_bytes / 1e9) if flush_buf is None else
                               "working set per step %.0f MB: a 256 MB buffer is overwritten between the timed "
                               "iterations, each iteration timed by its own event pair" % (state_bytes / 1e6)),

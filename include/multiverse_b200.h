@@ -1,4 +1,4 @@
-/* libmultiverse_b200 - C ABI of the B200-native Multiverse ConvRNN hot path.
+/* libmultiverse_b200 - C ABI of the H100-native Multiverse ConvRNN hot path.
  *
  * The reference (JunweiLiang/Multiverse, code/pred_models.py) has no FFI: its device work is
  * TensorFlow-1.15 op dispatch behind `sess.run` (pred_models.py:1732 train, :1779 test,

@@ -5,23 +5,22 @@
 // and raw_rnn :455/:678):  concat([x,h]) -> conv3x3 SAME -> +biases -> split i,j,f,o ->
 // c' = sigmoid(f+forget_bias)*c + sigmoid(i)*tanh(j);  h' = tanh(c')*sigmoid(o).
 //
-// Formulation: one persistent warp-specialised tcgen05 GEMM
+// Formulation: one persistent warp-specialised wgmma GEMM
 //     G[R, 1024] = A[R, 9*Cpad] * Bt[1024, 9*Cpad]^T
 // over the halo layout (mvb_common.cuh): the A k-block for tap t / channel chunk q is
-// the TMA box  rows [m0+shift(t), +128) x channels [32q, +32)  of the activation matrix,
-// so the 3x3 im2col never exists in memory.  fp32 parity on bf16 tensor cores comes
+// the rows [m0+shift(t), +128) x channels [64q, +64) of the activation matrix, read in place from one TMA-loaded
+// stage per chunk, so the 3x3 im2col never exists in memory.  fp32 parity on bf16 tensor cores comes
 // from operand planes: x = x0+x1(+x2) with every plane bf16 (mvb::split_planes), and
-// the products a_i*b_j with i+j < P are all accumulated into the same fp32 TMEM tile
+// the products a_i*b_j with i+j < P are all accumulated into the same fp32 accumulator
 // (P=2 -> 3 MMAs, error ~2^-17; P=3 -> 6 MMAs, ~2^-24; P=1 -> plain bf16).
-// Output columns are gate-interleaved (tile of 256 = 4 gates x 64 channels) so the
-// epilogue warps own i,j,f,o of a channel and emit (c', h') directly - the gate
+// Output columns are gate-interleaved (tile of 256 = 4 gates x 64 channels) so every
+// thread holds i,j,f,o of its channels in its accumulator registers and emits (c', h') directly - the gate
 // pre-activations never reach HBM.
 //
 // Warp roles (384 threads, 1 CTA/SM, persistent over tiles):
-//   warp 0   TMA producer      warp 1   MMA issuer (one thread)
-//   warp 2   TMEM allocator    warp 3   idle
-//   warps 4-11  epilogue: two warpgroups split the 64 channels of a tile; TMEM holds
-//               two 256-column accumulators so tile i+1's MMAs overlap tile i's epilogue.
+//   warpgroup 0      TMA producer (one thread), registers handed to the others (setmaxnreg)
+//   warpgroups 1, 2  MMA + epilogue: each owns 64 rows of the 128-row tile, all 256 columns (128 fp32
+//                    accumulators per thread)
 #include "mvb_common.cuh"
 #include "mvb_kernels.h"
 #include <stdlib.h>
@@ -33,27 +32,21 @@ constexpr int BLOCK_N = 256;
 constexpr int XPAD = 32;      // the x block is zero-padded to a multiple of 32 channels (cpad = roundup(cx,32) + 256)
 constexpr int CHUNK = 64;     // channels per K chunk: 64 16-bit elements = 128 B = one SWIZZLE_128B row
 constexpr int ROW_BYTES = 128;
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;       // K of one 16-bit wgmma
 constexpr int TILE_CH = 64;   // hidden channels per N tile
 constexpr int N_TILES = kGates / BLOCK_N;  // 4
-constexpr int NUM_EPI_WARPS = 8;
-constexpr int NUM_THREADS = 128 + 32 * NUM_EPI_WARPS;
+constexpr int NUM_THREADS = 384;
 constexpr int B_SLOT_BYTES = BLOCK_N * ROW_BYTES;  // 32 KB: 256 weight rows x 128 B
-constexpr uint32_t SW128_LAYOUT = 2;
+constexpr uint32_t SW128_LAYOUT = kSwizzle128B;
 constexpr uint32_t SW128_SBO = 8 * ROW_BYTES;      // 1024 B between 8-row groups
 
-// Shared-memory rings.  What bounded the round-1 kernel was not the tensor pipe but the operand feed: the TMA unit
-// writes about ONE BOX ROW PER CLOCK into shared memory whatever the row's width (measured with the MMAs and the
-// epilogue switched off: 275 / 549 / 824 rows per k-block -> 3.2 / 6.0 / 8.6 ms, 32- and 64-byte rows alike), and
-// the round-1 stages were made of 32- and 64-byte rows, nine shifted copies of every activation row among them.
+// Shared-memory rings.  The TMA unit writes about one box row per clock into shared memory whatever the row's width,
+// so the stages are made of full 128-byte rows and no activation row is loaded once per tap:
 //   B ring: slots of 256 rows x 128 B = 64 channels of ONE plane of the weight tile (SWIZZLE_128B): per (chunk,
 //           tap) P slots (bf16 planes) or 2 (f16f8: the fp16 plane, then both e4m3 planes interleaved in one row).
 //   A ring: one stage per 64-channel chunk: rows [m0 - (Wp+1), m0 + 128 + (Wp+1)) of every activation plane,
-//           rounded up to a multiple of 8 rows (RA8).  The nine taps of the chunk read THE SAME stage through UMMA
-//           descriptors that start (dy Wp + dx) rows into it: tcgen05 applies the swizzle to absolute shared-memory
-//           address bits, so a K-major operand may start at any row of a TMA-written swizzled tile (probed on B200
-//           for SWIZZLE_32B / 64B / 128B: tools/umma_rowshift_probe.cu).
-// Rows written per 32 channels and tap: 147 (round 1: 768 bf16 x 2, 1152 f16f8); L2 -> SM bytes 18.4 KB (48 KB).
+//           rounded up to a multiple of 8 rows (RA8).  The nine taps of the chunk read THE SAME stage through wgmma
+//           descriptors that start (dy Wp + dx) rows into it (see make_smem_desc).
 template <int P> struct CellCfg {
   static constexpr int A_STAGES = 2;
   static constexpr int MAX_RA8 = 256;           // TMA box limit: 128 + 2 (W + 2) <= 256  ->  W <= 62
@@ -124,49 +117,165 @@ __device__ __forceinline__ float preact(float acc, float scale, float q) {
   return FMT ? __fmaf_rn(acc, scale, q) : __fadd_rn(acc, q);
 }
 
-// UMMA instruction descriptor: D=f32, A=B=bf16, both K-major, M=128, N=256.
-constexpr uint32_t kIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((BLOCK_N >> 3) << 17) |
-                            ((BLOCK_M >> 4) << 24);
-// same with A=B=fp16 for kind::f16 (format code 0), which is also A=B=e4m3 for kind::f8f6f4 (format code 0)
-constexpr uint32_t kIdescF16 = (1u << 4) | ((BLOCK_N >> 3) << 17) | ((BLOCK_M >> 4) << 24);
+// Per-row context of the epilogue: where the row's state comes from and which input tables apply to it.
+struct EpiRow {
+  long long row, src_row, psmp;
+  int py, px;
+  bool valid;
+  const float* xfb;     // x-fold: table row of this cell's border class (bias included), else nullptr
+  const float* xft;     // x-fold / sparse-x table row of this cell for its sample row, else nullptr
+};
+
+__device__ __forceinline__ EpiRow epi_row(const CellParams& prm, const Grid& g, long long row) {
+  EpiRow r;
+  r.row = row; r.src_row = row; r.psmp = 0; r.py = 0; r.px = 0; r.xfb = nullptr; r.xft = nullptr;
+  r.valid = row < prm.R && !(prm.abl & 4);
+  if (!r.valid) return r;
+  const long long smp = row / g.S;
+  const int rem = (int)(row - smp * g.S);
+  const int y = rem / g.Wp, x = rem - y * g.Wp;
+  r.valid = (x < g.W) && (y < g.H);
+  if (!r.valid) return r;
+  if (prm.row_map) r.src_row = (long long)prm.row_map[smp] * g.S + rem;
+  r.py = y; r.px = x; r.psmp = smp;
+  if (prm.xf_B) {
+    const int cy = y == 0 ? 0 : (y == g.H - 1 ? 2 : 1), cx = x == 0 ? 0 : (x == g.W - 1 ? 2 : 1);
+    r.xfb = prm.xf_B + (cy * 3 + cx) * kGates;
+    // x-fold table row of this cell for the sample row whose arg-max cell is `a` (nullptr outside its 5x5)
+    const int a = prm.xf_ids[smp];
+    const int ay = a / g.W, ax = a - ay * g.W;
+    const int ry = y - ay, rx = x - ax;
+    if (ry >= -2 && ry <= 2 && rx >= -2 && rx <= 2) {
+      const int acy = ay == 0 ? 0 : (ay == g.H - 1 ? 2 : 1), acx = ax == 0 ? 0 : (ax == g.W - 1 ? 2 : 1);
+      r.xft = prm.xf_T2 + ((long long)(acy * 3 + acx) * 25 + (ry + 2) * 5 + (rx + 2)) * kGates;
+    }
+  }
+  if (prm.xs_tab) {          // out[p] += in[p + off(tap)] . W[tap] with the input at the label cell only
+    const int l = prm.xs_label[smp];
+    if (l >= 0 && l < g.H * g.W) {
+      const int ly = l / g.W, dy = ly - y, dx = (l - ly * g.W) - x;
+      if (dy >= -1 && dy <= 1 && dx >= -1 && dx <= 1)
+        r.xft = prm.xs_tab + ((long long)smp * 9 + (dy + 1) * 3 + (dx + 1)) * kGates;
+    }
+  }
+  return r;
+}
+
+// The epilogue of one row and two adjacent packed columns j, j + 1 of every gate (a[gate][e] = accumulators of
+// column gate * 64 + j + e of N tile nt): state update and every requested output.
+template <int P, int FMT>
+__device__ __forceinline__ void epi_pair(const CellParams& prm, const Grid& g, const EpiRow& r, int nt, int j,
+                                         const float (&a)[4][2]) {
+  const int col = nt * BLOCK_N + j;             // packed column of gate 0
+  const int ch = nt * TILE_CH + j;              // hidden channel
+  if (prm.preact_out) {
+    float* gp = prm.preact_out + r.row * kGates + col;
+#pragma unroll
+    for (int gt = 0; gt < 4; ++gt) *reinterpret_cast<float2*>(gp + gt * TILE_CH) = make_float2(a[gt][0], a[gt][1]);
+    return;
+  }
+  // bias (or bias-folded table), + the x-fold / sparse-x table row of this cell, + the dense x path
+  const float* bptr = (r.xfb ? r.xfb : prm.bias) + col;
+  float q[4][2];
+#pragma unroll
+  for (int gt = 0; gt < 4; ++gt) {
+    const float2 b = __ldg(reinterpret_cast<const float2*>(bptr + gt * TILE_CH));
+    q[gt][0] = b.x; q[gt][1] = b.y;
+  }
+  if (r.xft) {
+#pragma unroll
+    for (int gt = 0; gt < 4; ++gt) {
+      const float2 t = __ldg(reinterpret_cast<const float2*>(r.xft + col + gt * TILE_CH));
+      q[gt][0] = __fadd_rn(q[gt][0], t.x); q[gt][1] = __fadd_rn(q[gt][1], t.y);
+    }
+  }
+  if (prm.xr_W) {           // + sum over taps and the two channels of x * W, fp32
+#pragma unroll 1
+    for (int k = 0; k < 18; ++k) {
+      const int tp = k >> 1, yy = r.py + tp / 3 - 1, xx = r.px + tp % 3 - 1;
+      const float xk = (yy >= 0 && yy < g.H && xx >= 0 && xx < g.W)
+                           ? __ldg(prm.xr_in + ((r.psmp * g.H + yy) * g.W + xx) * 2 + (k & 1)) : 0.f;
+#pragma unroll
+      for (int gt = 0; gt < 4; ++gt) {
+        const float2 w = __ldg(reinterpret_cast<const float2*>(prm.xr_W + k * kGates + col + gt * TILE_CH));
+        q[gt][0] = __fmaf_rn(xk, w.x, q[gt][0]); q[gt][1] = __fmaf_rn(xk, w.y, q[gt][1]);
+      }
+    }
+  }
+  float sc[4][2] = {};
+  if (FMT == 1) {
+#pragma unroll
+    for (int gt = 0; gt < 4; ++gt) {
+      const float2 s2 = __ldg(reinterpret_cast<const float2*>(prm.col_scale + col + gt * TILE_CH));
+      sc[gt][0] = s2.x; sc[gt][1] = s2.y;
+    }
+  }
+  float2 cprev = make_float2(0.f, 0.f);
+  if (prm.c_in) cprev = __ldg(reinterpret_cast<const float2*>(prm.c_in + r.src_row * kHidden + ch));
+  GateOut o[2];
+#pragma unroll
+  for (int e = 0; e < 2; ++e)
+    o[e] = lstm_update(preact<FMT>(a[0][e], sc[0][e], q[0][e]), preact<FMT>(a[1][e], sc[1][e], q[1][e]),
+                       preact<FMT>(a[2][e], sc[2][e], q[2][e]), preact<FMT>(a[3][e], sc[3][e], q[3][e]),
+                       e ? cprev.y : cprev.x, prm.forget_bias);
+  if (prm.gates_out) {
+    float* gp = prm.gates_out + r.row * kGates + col;
+    *reinterpret_cast<float2*>(gp + 0 * TILE_CH) = make_float2(o[0].ai, o[1].ai);
+    *reinterpret_cast<float2*>(gp + 1 * TILE_CH) = make_float2(o[0].aj, o[1].aj);
+    *reinterpret_cast<float2*>(gp + 2 * TILE_CH) = make_float2(o[0].af, o[1].af);
+    *reinterpret_cast<float2*>(gp + 3 * TILE_CH) = make_float2(o[0].ao, o[1].ao);
+  }
+  *reinterpret_cast<float2*>(prm.c_out + r.row * kHidden + ch) = make_float2(o[0].c, o[1].c);
+  if (prm.h32_out) *reinterpret_cast<float2*>(prm.h32_out + r.row * kHidden + ch) = make_float2(o[0].h, o[1].h);
+  if (prm.hp_out && prm.hp_mixed) {
+    uint32_t h2, e0, e1;
+    split_f16f8_x2(o[0].h, o[1].h, h2, e0, e1);
+    const int c = prm.ch_off_out + ch;
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(prm.hp_out) + r.row * prm.cpad_out + c) = h2;
+    uint8_t* b8 = reinterpret_cast<uint8_t*>(prm.hp_out) + 2 * prm.hp_plane_stride + r.row * 2 * prm.cpad_out;
+    *reinterpret_cast<uint16_t*>(b8 + f8_off(c, 0, prm.cpad_out)) = (uint16_t)e0;
+    *reinterpret_cast<uint16_t*>(b8 + f8_off(c, 1, prm.cpad_out)) = (uint16_t)e1;
+  } else if (prm.hp_out) {
+    __nv_bfloat16 p0[P], p1[P];
+    split_planes<P>(o[0].h, p0);
+    split_planes<P>(o[1].h, p1);
+#pragma unroll
+    for (int p = 0; p < P; ++p)
+      *reinterpret_cast<uint32_t*>(prm.hp_out + p * prm.hp_plane_stride + r.row * prm.cpad_out + prm.ch_off_out + ch) =
+          pack_bf16x2(p0[p], p1[p]);
+  }
+}
 
 // MC = true: clusters of two CTAs work on two M tiles of the same N tile in lock step; each loads half of every B
 // (weight) tile and TMA-multicasts it to both, so the L2 -> shared-memory traffic per CTA and stage drops from
-// 48 KB to 32 KB (P = 2).  A stage may be refilled once BOTH CTAs' MMAs have consumed it (empty barrier count 2,
-// commits multicast to the pair).
+// 48 KB to 32 KB (P = 2).  A slot may be refilled once the MMA warpgroups of BOTH CTAs have consumed it (empty
+// barrier count 4: two warpgroups per CTA arrive on their own and on the peer's barrier).
 // FMT = 1: f16f8 operands (P must be 2: same stage bytes).  tmA / tmB then describe the fp16 regions (one
-// "plane") and tmA8 / tmB8 the two fp8 planes; per 32-channel stage the issuer sends two kind::f16 MMAs (K = 16
-// each) and two kind::f8f6f4 MMAs (K = 32 each) into the same accumulator: 4 dispatches instead of 6.
-// CG = 2: the pair instead issues ONE cta_group::2 MMA of 256 rows per dispatch from CTA 0: every CTA keeps only ITS
-// half (128 rows) of each weight slot - the tensor cores of the pair read both halves in place - so the same 128 KB
-// ring holds 8 slots instead of 4 (twice the prefetch distance: the L2 -> shared-memory latency under load, not
-// bandwidth, is what left the tensor pipe idle with 4) and no byte of B is written into two shared memories.
-template <int P, int CG, int FMT>
+// "plane") and tmA8 / tmB8 the two fp8 planes; per 64-channel chunk and tap each warpgroup sends four e4m3 MMAs
+// (K = 32 each) and four fp16 MMAs (K = 16 each) into the same accumulator: 2 bf16-pass equivalents instead of 3.
+template <int P, bool MC, int FMT>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmA8, const __grid_constant__ CUtensorMap tmB8,
                 const CellParams prm) {
   static_assert(FMT == 0 || P == 2, "the f16f8 format occupies the bytes of two bf16 planes");
   using Cfg = CellCfg<P>;
-  constexpr bool MC = CG == 1, CG2 = CG == 2, PAIR = CG != 0;
-  constexpr int SLOT_BYTES = CG2 ? B_SLOT_BYTES / 2 : B_SLOT_BYTES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   const int ra8 = (BLOCK_M + 2 * (prm.W + 2) + 7) & ~7;     // rows of an A stage
   const int a_stage_bytes = Cfg::a_stage_bytes(ra8);
-  const int b_slots = Cfg::b_slots(ra8) * (CG2 ? 2 : 1);
-  uint8_t* smem_a = smem + b_slots * SLOT_BYTES;
+  const int a_load_bytes = FMT ? ra8 * ROW_BYTES : a_stage_bytes;     // f16f8: one plane per pass
+  const int b_slots = Cfg::b_slots(ra8);
+  uint8_t* smem_a = smem + b_slots * B_SLOT_BYTES;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_a + Cfg::A_STAGES * a_stage_bytes);
   uint64_t* empty_bar = full_bar + 8;
   uint64_t* afull_bar = empty_bar + 8;
   uint64_t* aempty_bar = afull_bar + Cfg::A_STAGES;
-  uint64_t* tfull_bar = aempty_bar + Cfg::A_STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;                    // 0: TMA producer; 1, 2: MMA + epilogue of rows [64 (wg - 1), +64)
   const Grid g = make_grid(prm.H, prm.W);
   // K chunks of 64 channels: the x chunk [0, 64) - of which only the cxp channels of the x block are multiplied -
   // then the four chunks of the h block [cxp + 64 j, +64).  fp8 rows (f16f8): [x: e0 (cxp) | e1 (cxp)] then per h
@@ -174,397 +283,192 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int cxp = prm.cpad - kHidden;
   const int q_begin = prm.skip_x ? 1 : 0;
   constexpr int NQ = 1 + kHidden / CHUNK;      // 5
-  constexpr int NS = FMT ? 2 : P;              // B slots per (chunk, tap)
+  // f16f8: two passes over K, the e4m3 cross terms first and then the fp16 main products.  The e4m3 MMAs accumulate
+  // with a short internal sum (about 14 significant bits of the accumulator), so they run while the accumulator holds
+  // only their own small sum (~2^-11 of the result); the fp16 MMAs, exact in fp32, then add the main products.
+  constexpr int NPASS = FMT ? 2 : 1;
+  constexpr int NS = FMT ? 1 : P;              // B slots per (pass, chunk, tap)
   const long long num_m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
   // work index w -> (m tile, n tile).  MC: the pair shares w; rank r takes m tile 2*(w / N_TILES) + r.
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const long long num_tiles = (PAIR ? (num_m_tiles + 1) / 2 : num_m_tiles) * N_TILES;
-  const long long w_begin = PAIR ? (long long)(blockIdx.x >> 1) : (long long)blockIdx.x;
-  const long long w_step = PAIR ? (long long)(gridDim.x >> 1) : (long long)gridDim.x;
+  const uint32_t rank = MC ? cluster_ctarank() : 0u;
+  const long long num_tiles = (MC ? (num_m_tiles + 1) / 2 : num_m_tiles) * N_TILES;
+  const long long w_begin = MC ? (long long)(blockIdx.x >> 1) : (long long)blockIdx.x;
+  const long long w_step = MC ? (long long)(gridDim.x >> 1) : (long long)gridDim.x;
   // iteration it of this CTA (pair) -> work index.  order 1 (default): the N tiles of an M tile run back to back on
   // the same CTA (pair), so its operand rows are re-read from L2 by the SM that fetched them; order 0: strided
   // (the N tiles of an M tile run concurrently on neighbouring CTAs).
   auto work_index = [&](long long it) -> long long {
     return prm.order ? (w_begin + (it / N_TILES) * w_step) * N_TILES + it % N_TILES : w_begin + it * w_step;
   };
-  auto tile_m0 = [&](long long w) -> long long { return ((w / N_TILES) * (PAIR ? 2 : 1) + rank) * BLOCK_M; };
+  auto tile_m0 = [&](long long w) -> long long { return ((w / N_TILES) * (MC ? 2 : 1) + rank) * BLOCK_M; };
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     if (FMT == 1) { prefetch_tmap(&tmA8); prefetch_tmap(&tmB8); }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < b_slots; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], MC ? 2 : 1); }
-    for (int s = 0; s < Cfg::A_STAGES; ++s) { mbar_init(&afull_bar[s], 1); mbar_init(&aempty_bar[s], 1); }
-    // CG2: the issuer (CTA 0) waits for the epilogue warps of BOTH CTAs before it reuses an accumulator
-    for (int a = 0; a < 2; ++a) { mbar_init(&tfull_bar[a], 1); mbar_init(&tempty_bar[a], NUM_EPI_WARPS * (CG2 ? 2 : 1)); }
+    for (int s = 0; s < b_slots; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], MC ? 4 : 2); }
+    for (int s = 0; s < Cfg::A_STAGES; ++s) { mbar_init(&afull_bar[s], 1); mbar_init(&aempty_bar[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 2) { if (CG2) tmem_alloc_2sm(tmem_slot, 512); else tmem_alloc(tmem_slot, 512); }
-  tc_fence_before();
   __syncthreads();
-  if (PAIR) cluster_sync_all();     // the peer's barriers (and, CG2, its TMEM) exist before anything is sent to them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (MC) cluster_sync_all();     // the peer's barriers exist before anything is sent to them
 
-  if (warp == 0 && lane == 0) {
-    // ===================== TMA producer =====================
-    int slot = 0, astage = 0; uint32_t phase = 0, aphase = 0;
-    for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
-      const long long m0 = tile_m0(t);
-      const int n0 = (int)(t % N_TILES) * BLOCK_N;
-      // chunk-major K order: the x block - whose terms can be orders of magnitude larger than the h terms (raw
-      // pixel offsets in the regression encoder) - is accumulated first, so the small h products are never added
-      // onto a large transient partial sum.
-      if (prm.abl & 16) continue;
-      for (int q = q_begin; q < NQ; ++q) {
-        const int c16 = q == 0 ? 0 : cxp + (q - 1) * CHUNK;              // 16-bit channel coordinate
-        const int c8 = q == 0 ? 0 : 2 * cxp + (q - 1) * 2 * CHUNK;       // fp8 byte coordinate
-        mbar_wait(&aempty_bar[astage], aphase ^ 1);
-        uint8_t* sa = smem_a + astage * a_stage_bytes;
-        if (CG2) {
-          // both CTAs' bytes are reported to CTA 0's barrier: its MMAs read the A tiles of both
-          if (rank == 0) mbar_expect_tx(&afull_bar[astage], 2 * a_stage_bytes);
-          tma_load_3d_2sm(sa, &tmA, &afull_bar[astage], c16, (int)(m0 - g.Wp - 1), 0);
-          if (FMT == 1) tma_load_3d_2sm(sa + ra8 * ROW_BYTES, &tmA8, &afull_bar[astage], c8, (int)(m0 - g.Wp - 1), 0);
-        } else {
-          mbar_expect_tx(&afull_bar[astage], a_stage_bytes);
-          tma_load_3d(sa, &tmA, &afull_bar[astage], c16, (int)(m0 - g.Wp - 1), 0);
-          if (FMT == 1) tma_load_3d(sa + ra8 * ROW_BYTES, &tmA8, &afull_bar[astage], c8, (int)(m0 - g.Wp - 1), 0);
-        }
-        if (++astage == Cfg::A_STAGES) { astage = 0; aphase ^= 1; }
-        for (int tap = 0; tap < 9; ++tap) {
+  if (wg == 0) {
+    regs_dealloc<40>();
+    if (warp == 0 && lane == 0) {
+      // ===================== TMA producer =====================
+      int slot = 0, astage = 0; uint32_t phase = 0, aphase = 0;
+      for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
+        const long long m0 = tile_m0(t);
+        const int n0 = (int)(t % N_TILES) * BLOCK_N;
+        // chunk-major K order: the x block - whose terms can be orders of magnitude larger than the h terms (raw
+        // pixel offsets in the regression encoder) - is accumulated first, so the small h products are never added
+        // onto a large transient partial sum.
+        if (prm.abl & 16) continue;
+        for (int pass = 0; pass < NPASS; ++pass)
+        for (int q = q_begin; q < NQ; ++q) {
+          const int c16 = q == 0 ? 0 : cxp + (q - 1) * CHUNK;              // 16-bit channel coordinate
+          const int c8 = q == 0 ? 0 : 2 * cxp + (q - 1) * 2 * CHUNK;       // fp8 byte coordinate
+          const bool f8 = FMT == 1 && pass == 0;
+          mbar_wait(&aempty_bar[astage], aphase ^ 1);
+          uint8_t* sa = smem_a + astage * a_stage_bytes;
+          mbar_expect_tx(&afull_bar[astage], a_load_bytes);
+          if (f8) tma_load_3d(sa, &tmA8, &afull_bar[astage], c8, (int)(m0 - g.Wp - 1), 0);
+          else tma_load_3d(sa, &tmA, &afull_bar[astage], c16, (int)(m0 - g.Wp - 1), 0);
+          if (++astage == Cfg::A_STAGES) { astage = 0; aphase ^= 1; }
+          for (int tap = 0; tap < 9; ++tap) {
 #pragma unroll
-          for (int sl = 0; sl < NS; ++sl) {
-            mbar_wait(&empty_bar[slot], phase ^ 1);
-            uint8_t* sb = smem + slot * SLOT_BYTES;
-            if (!CG2 || rank == 0) mbar_expect_tx(&full_bar[slot], B_SLOT_BYTES);
-            const bool f8 = FMT == 1 && sl == 1;
-            const CUtensorMap* tm = f8 ? &tmB8 : &tmB;
-            const int kcol = f8 ? tap * 2 * prm.cpad + c8 : tap * prm.cpad + c16;
-            const int plane = FMT == 1 ? 0 : sl;
-            // MC: this CTA's half (128 rows) of the slot, delivered to both CTAs of the pair
-            if (CG2) tma_load_3d_2sm(sb, tm, &full_bar[slot], kcol, n0 + (int)rank * (BLOCK_N / 2), plane);
-            else if (MC) tma_load_3d_mc(sb + rank * (B_SLOT_BYTES / 2), tm, &full_bar[slot], kcol,
-                                        n0 + (int)rank * (BLOCK_N / 2), plane, (uint16_t)3);
-            else tma_load_3d(sb, tm, &full_bar[slot], kcol, n0, plane);
-            if (++slot == b_slots) { slot = 0; phase ^= 1; }
+            for (int sl = 0; sl < NS; ++sl) {
+              mbar_wait(&empty_bar[slot], phase ^ 1);
+              uint8_t* sb = smem + slot * B_SLOT_BYTES;
+              mbar_expect_tx(&full_bar[slot], B_SLOT_BYTES);
+              const CUtensorMap* tm = f8 ? &tmB8 : &tmB;
+              const int kcol = f8 ? tap * 2 * prm.cpad + c8 : tap * prm.cpad + c16;
+              // MC: this CTA's half (128 rows) of the slot, delivered to both CTAs of the pair
+              if (MC) tma_load_3d_mc(sb + rank * (B_SLOT_BYTES / 2), tm, &full_bar[slot], kcol,
+                                     n0 + (int)rank * (BLOCK_N / 2), sl, (uint16_t)3);
+              else tma_load_3d(sb, tm, &full_bar[slot], kcol, n0, sl);
+              if (++slot == b_slots) { slot = 0; phase ^= 1; }
+            }
           }
         }
       }
     }
-  } else if (warp == 1 && lane == 0 && (!CG2 || rank == 0)) {
-    // ===================== MMA issuer =====================
-    // One thread; its instruction stream is the critical path at 128 cycles per dispatch (measured with the loads and
-    // the epilogue switched off: the round-2 first draft, with run-time K loops and 64-bit descriptor builds, reached
-    // only 79 % of the dispatch floor).  So: compile-time trip counts for the h chunks, one IADD per operand and
-    // dispatch (umma_lohi), the accumulate flag a compile-time constant except for the first dispatch of a tile.
-    constexpr uint32_t kIdM = CG2 ? ((2u * BLOCK_M) >> 4) << 24 : 0u;     // cta_group::2: M = 256
-    constexpr uint32_t kIdBf16 = CG2 ? ((kIdesc & 0x00FFFFFFu) | kIdM) : kIdesc;
-    constexpr uint32_t kIdF16 = CG2 ? ((kIdescF16 & 0x00FFFFFFu) | kIdM) : kIdescF16;
+  } else {
+    regs_alloc<232>();
+    // ===================== MMA + epilogue (one warpgroup per 64 rows of the tile) =====================
+    const int c = wg - 1;
+    const bool leader = (threadIdx.x & 127) == 0;          // arrives on the barriers for the warpgroup
     constexpr uint32_t kHi = smem_desc_hi(SW128_SBO, SW128_LAYOUT);
     const bool do16 = !(prm.abl & 2), do8 = !(prm.abl & 1), wait_data = !(prm.abl & 8);
     const uint32_t a_plane_lo = (uint32_t)(ra8 * ROW_BYTES) >> 4;
+    const uint32_t a_wg_lo = (uint32_t)(64 * c) * (ROW_BYTES >> 4);      // this warpgroup's 64 rows of the A tile
     int slot = 0, astage = 0; uint32_t phase = 0, aphase = 0;
-    long long it = 0;
-    for (long long t; (t = work_index(it)) < num_tiles; ++it) {
-      const int as = (int)(it & 1);
-      const uint32_t tphase = (uint32_t)((it >> 1) & 1);
-      mbar_wait(&tempty_bar[as], tphase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BLOCK_N;
-      bool fresh = true;                     // the tile's first dispatch overwrites the accumulator
+    float acc[128];
+    // release of the previous batch of MMAs' operands, once they have completed
+    int rel_slot = -1, rel_astage = -1;
+    auto release = [&]() {
+      if (leader && rel_slot >= 0) {
+        if (MC) { mbar_arrive_remote(&empty_bar[rel_slot], 0); mbar_arrive_remote(&empty_bar[rel_slot], 1); }
+        else mbar_arrive(&empty_bar[rel_slot]);
+        if (rel_astage >= 0) mbar_arrive(&aempty_bar[rel_astage]);
+      }
+      rel_slot = -1; rel_astage = -1;
+    };
+    for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
+      const long long m0 = tile_m0(t);
+      const int nt = (int)(t % N_TILES);
+      uint32_t fresh = 1;                      // the tile's first MMA overwrites the accumulator
+      auto mma16 = [&](uint32_t a_lo, uint32_t b_lo) {
+        if (FMT == 1) wgmma_f16<256, 0, 0>(acc, desc_of(a_lo, kHi), desc_of(b_lo, kHi), fresh ^ 1u);
+        else wgmma_bf16<256, 0, 0>(acc, desc_of(a_lo, kHi), desc_of(b_lo, kHi), fresh ^ 1u);
+        fresh = 0;
+      };
+      auto mma8 = [&](uint32_t a_lo, uint32_t b_lo) {
+        wgmma_e4m3_n256(acc, desc_of(a_lo, kHi), desc_of(b_lo, kHi), fresh ^ 1u);
+        fresh = 0;
+      };
+      for (int pass = 0; pass < NPASS; ++pass)
       for (int q = q_begin; q < NQ; ++q) {
+        const bool f8 = FMT == 1 && pass == 0;
         if (wait_data) mbar_wait(&afull_bar[astage], aphase);
-        const uint32_t sa_lo = smem_u32(smem_a + astage * a_stage_bytes) >> 4;
+        const uint32_t sa_lo = (smem_u32(smem_a + astage * a_stage_bytes) >> 4) + a_wg_lo;
         for (int tap = 0; tap < 9; ++tap) {
           // the tap's A tile: the stage's rows starting (dy-1) Wp + (dx-1) + (Wp+1) = dy Wp + dx rows in
           const uint32_t a_lo = sa_lo + (uint32_t)((tap / 3) * g.Wp + (tap % 3)) * (ROW_BYTES >> 4);
 #pragma unroll
           for (int sl = 0; sl < NS; ++sl) {
             if (wait_data) mbar_wait(&full_bar[slot], phase);
-            tc_fence_after();
-            const uint32_t b_lo = smem_u32(smem + slot * SLOT_BYTES) >> 4;
+            const uint32_t b_lo = smem_u32(smem + slot * B_SLOT_BYTES) >> 4;
+            wgmma_fence_regs(acc);
+            wgmma_fence();
             if (q > 0) {
-              // ---- h chunk: 64 channels = 4 K16 steps per 16-bit plane pair, 2 K32 steps per e4m3 plane ----
-              if (FMT == 1 && sl == 0) {
-                if (do16) {
-                  if (fresh) umma_lohi<0, CG2, false>(d_tmem, a_lo, b_lo, kHi, kIdF16);
-                  else umma_lohi<0, CG2, true>(d_tmem, a_lo, b_lo, kHi, kIdF16);
-                  umma_lohi<0, CG2, true>(d_tmem, a_lo + 2, b_lo + 2, kHi, kIdF16);
-                  umma_lohi<0, CG2, true>(d_tmem, a_lo + 4, b_lo + 4, kHi, kIdF16);
-                  umma_lohi<0, CG2, true>(d_tmem, a_lo + 6, b_lo + 6, kHi, kIdF16);
-                  fresh = false;
-                }
-              } else if (FMT == 1) {
-                if (do8) {
-                  const uint32_t a8 = a_lo + a_plane_lo;          // [e0 (64 B) | e1 (64 B)] per row
-                  if (fresh) umma_lohi<1, CG2, false>(d_tmem, a8, b_lo, kHi, kIdF16);
-                  else umma_lohi<1, CG2, true>(d_tmem, a8, b_lo, kHi, kIdF16);
-                  umma_lohi<1, CG2, true>(d_tmem, a8 + 2, b_lo + 2, kHi, kIdF16);
-                  umma_lohi<1, CG2, true>(d_tmem, a8 + 4, b_lo + 4, kHi, kIdF16);
-                  umma_lohi<1, CG2, true>(d_tmem, a8 + 6, b_lo + 6, kHi, kIdF16);
-                  fresh = false;
-                }
+              // ---- h chunk: 64 channels = 4 K16 steps per 16-bit plane pair, 4 K32 steps over the two e4m3 planes ----
+              if (f8) {
+                if (do8) for (int k = 0; k < 4; ++k) mma8(a_lo + 2 * k, b_lo + 2 * k);    // [e0 (64 B) | e1 (64 B)]
               } else if (do16) {
-                // B plane sl against the A planes pa with pa + sl < P
+                // B plane sl against the A planes pa with pa + sl < P (f16f8: the fp16 planes, P - sl = 1)
 #pragma unroll
-                for (int pa = 0; pa < P - sl; ++pa) {
-                  const uint32_t ap = a_lo + pa * a_plane_lo;
-                  if (fresh) umma_lohi<0, CG2, false>(d_tmem, ap, b_lo, kHi, kIdBf16);
-                  else umma_lohi<0, CG2, true>(d_tmem, ap, b_lo, kHi, kIdBf16);
-                  umma_lohi<0, CG2, true>(d_tmem, ap + 2, b_lo + 2, kHi, kIdBf16);
-                  umma_lohi<0, CG2, true>(d_tmem, ap + 4, b_lo + 4, kHi, kIdBf16);
-                  umma_lohi<0, CG2, true>(d_tmem, ap + 6, b_lo + 6, kHi, kIdBf16);
-                  fresh = false;
-                }
+                for (int pa = 0; pa < (FMT ? 1 : P - sl); ++pa)
+#pragma unroll
+                  for (int k = 0; k < 4; ++k) mma16(a_lo + pa * a_plane_lo + 2 * k, b_lo + 2 * k);
               }
             } else {
-              // ---- x chunk (only cells whose input is not folded): cxp = 32 or 64 channels, run-time trip counts ----
-              const int ks16 = cxp / UMMA_K, ks8 = cxp / 32;
+              // ---- x chunk (only cells whose input is not folded): cxp = 32 or 64 channels ----
+              const int ks16 = cxp / MMA_K, ks8 = cxp / 32;
               const uint32_t poff = (uint32_t)cxp >> 4;              // e1 sits cxp bytes after e0 in an fp8 row
-              if (FMT == 1 && sl == 0) {
-                for (int k = 0; k < ks16 && do16; ++k) {
-                  if (fresh) umma_lohi<0, CG2, false>(d_tmem, a_lo + 2 * k, b_lo + 2 * k, kHi, kIdF16);
-                  else umma_lohi<0, CG2, true>(d_tmem, a_lo + 2 * k, b_lo + 2 * k, kHi, kIdF16);
-                  fresh = false;
-                }
-              } else if (FMT == 1) {
+              if (f8) {
                 for (int pk = 0; pk < 2 * ks8 && do8; ++pk) {
                   const uint32_t o = (pk / ks8) * poff + (pk % ks8) * 2;
-                  if (fresh) umma_lohi<1, CG2, false>(d_tmem, a_lo + a_plane_lo + o, b_lo + o, kHi, kIdF16);
-                  else umma_lohi<1, CG2, true>(d_tmem, a_lo + a_plane_lo + o, b_lo + o, kHi, kIdF16);
-                  fresh = false;
+                  mma8(a_lo + o, b_lo + o);
                 }
               } else {
-                for (int pa = 0; pa < P - sl; ++pa)
-                  for (int k = 0; k < ks16 && do16; ++k) {
-                    if (fresh) umma_lohi<0, CG2, false>(d_tmem, a_lo + pa * a_plane_lo + 2 * k, b_lo + 2 * k, kHi, kIdBf16);
-                    else umma_lohi<0, CG2, true>(d_tmem, a_lo + pa * a_plane_lo + 2 * k, b_lo + 2 * k, kHi, kIdBf16);
-                    fresh = false;
-                  }
+                for (int pa = 0; pa < (FMT ? 1 : P - sl); ++pa)
+                  for (int k = 0; k < ks16 && do16; ++k) mma16(a_lo + pa * a_plane_lo + 2 * k, b_lo + 2 * k);
               }
             }
-            if (CG2) umma_commit_2sm(&empty_bar[slot]);
-            else if (MC) umma_commit_mc(&empty_bar[slot], (uint16_t)3);
-            else umma_commit(&empty_bar[slot]);
+            wgmma_commit();
+            wgmma_fence_regs(acc);
+            wgmma_wait<1>();               // the previous batch has completed: its slot (and A stage) can be refilled
+            release();
+            rel_slot = slot;
+            if (tap == 8 && sl == NS - 1) rel_astage = astage;     // this CTA's nine taps have consumed the A stage
             if (++slot == b_slots) { slot = 0; phase ^= 1; }
           }
         }
-        if (CG2) umma_commit_2sm(&aempty_bar[astage]);
-        else umma_commit(&aempty_bar[astage]);      // this CTA's nine taps have consumed the A stage
         if (++astage == Cfg::A_STAGES) { astage = 0; aphase ^= 1; }
       }
-      if (CG2) umma_commit_2sm(&tfull_bar[as]);
-      else umma_commit(&tfull_bar[as]);
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int wq = warp & 3;                 // TMEM lane quarter this warp may touch
-    const int cgp = (warp - 4) >> 2;         // column group (0/1): channels [32*cgp, +32)
-    long long it = 0;
-    for (long long t; (t = work_index(it)) < num_tiles; ++it) {
-      const int as = (int)(it & 1);
-      const uint32_t aphase = (uint32_t)((it >> 1) & 1);
-      const long long m0 = tile_m0(t);
-      const int nt = (int)(t % N_TILES);
-      const long long row = m0 + wq * 32 + lane;
-      bool valid = row < prm.R;
-      long long src_row = row;
-      const float* xfb = nullptr;      // x-fold: table row of this cell's border class (bias included)
-      int py = 0, px = 0, prem = 0;    // cell position and row offset inside its sample row
-      long long psmp = 0;
-      if (valid) {
-        const long long smp = row / g.S;
-        const int rem = (int)(row - smp * g.S);
-        const int y = rem / g.Wp, x = rem - y * g.Wp;
-        valid = (x < g.W) && (y < g.H);
-        if (valid && prm.row_map) src_row = (long long)prm.row_map[smp] * g.S + rem;
-        if (valid && prm.xf_B) {
-          const int cy = y == 0 ? 0 : (y == g.H - 1 ? 2 : 1), cx = x == 0 ? 0 : (x == g.W - 1 ? 2 : 1);
-          xfb = prm.xf_B + (cy * 3 + cx) * kGates;
-        }
-        py = y; px = x; psmp = smp; prem = rem;
-      }
-      // x-fold table row of this cell for the sample row whose arg-max cell is `a` (nullptr outside its 5x5)
-      auto xft_of = [&](int a) -> const float* {
-        const int ay = a / g.W, ax = a - ay * g.W;
-        const int ry = py - ay, rx = px - ax;
-        if (ry < -2 || ry > 2 || rx < -2 || rx > 2) return nullptr;
-        const int acy = ay == 0 ? 0 : (ay == g.H - 1 ? 2 : 1), acx = ax == 0 ? 0 : (ax == g.W - 1 ? 2 : 1);
-        return prm.xf_T2 + ((long long)(acy * 3 + acx) * 25 + (ry + 2) * 5 + (rx + 2)) * kGates;
-      };
-      float xv[18];                    // dense x path: the 3x3 neighbourhood of this cell's two raw input channels
-      if (prm.xr_W) {
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      release();
+      if (fresh) {                          // no MMA ran (debug ablations): the accumulator is zero
 #pragma unroll
-        for (int tp = 0; tp < 9; ++tp) {
-          const int yy = py + tp / 3 - 1, xx = px + tp % 3 - 1;
-          const bool ok = valid && yy >= 0 && yy < g.H && xx >= 0 && xx < g.W;
-          const float2 v = ok ? __ldg(reinterpret_cast<const float2*>(prm.xr_in + ((psmp * g.H + yy) * g.W + xx) * 2))
-                              : make_float2(0.f, 0.f);
-          xv[2 * tp] = v.x; xv[2 * tp + 1] = v.y;
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+      }
+      // ===================== epilogue =====================
+      // thread (warp w of the warpgroup, lane l) holds rows 16 w + l / 4 (+ 8) and columns 8 i + 2 (l % 4) (+ 1);
+      // column gate * 64 + j of the N tile is gate `gate` of channel j: each thread owns all four gates of its channels
+      const long long rbase = m0 + 64 * c + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const EpiRow r = epi_row(prm, g, rbase + 8 * hr);
+        if (!r.valid) continue;
+#pragma unroll
+        for (int ip = 0; ip < 8; ++ip) {
+          float a[4][2];
+#pragma unroll
+          for (int gt = 0; gt < 4; ++gt) {
+            a[gt][0] = acc[4 * (8 * gt + ip) + 2 * hr];
+            a[gt][1] = acc[4 * (8 * gt + ip) + 2 * hr + 1];
+          }
+          epi_pair<P, FMT>(prm, g, r, nt, 8 * ip + 2 * (lane & 3), a);
         }
       }
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
-      if (prm.abl & 4) valid = false;
-      const uint32_t t_row = tmem_base + ((uint32_t)(wq * 32) << 16) + as * BLOCK_N;
-#pragma unroll 1
-      for (int cc = 0; cc < 2; ++cc) {
-        const int j0 = cgp * 32 + cc * 16;            // channel offset inside the tile
-        const int ch0 = nt * TILE_CH + j0;            // hidden channel
-        uint32_t gi[16], gj[16], gf[16], go[16];
-        tmem_ld16(t_row + 0 * TILE_CH + j0, gi);
-        tmem_ld16(t_row + 1 * TILE_CH + j0, gj);
-        tmem_ld16(t_row + 2 * TILE_CH + j0, gf);
-        tmem_ld16(t_row + 3 * TILE_CH + j0, go);
-        float cprev[16];
-        if (valid && prm.c_in) {
-          const float4* cp = reinterpret_cast<const float4*>(prm.c_in + src_row * kHidden + ch0);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            const float4 q4 = __ldg(cp + v);
-            cprev[4 * v] = q4.x; cprev[4 * v + 1] = q4.y; cprev[4 * v + 2] = q4.z; cprev[4 * v + 3] = q4.w;
-          }
-        } else {
-#pragma unroll
-          for (int v = 0; v < 16; ++v) cprev[v] = 0.f;
-        }
-        tmem_ld_wait();
-        if (valid && prm.preact_out) {
-          float* gp = prm.preact_out + row * kGates + nt * BLOCK_N + j0;
-#pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            reinterpret_cast<uint4*>(gp + 0 * TILE_CH)[v] = make_uint4(gi[4 * v], gi[4 * v + 1], gi[4 * v + 2], gi[4 * v + 3]);
-            reinterpret_cast<uint4*>(gp + 1 * TILE_CH)[v] = make_uint4(gj[4 * v], gj[4 * v + 1], gj[4 * v + 2], gj[4 * v + 3]);
-            reinterpret_cast<uint4*>(gp + 2 * TILE_CH)[v] = make_uint4(gf[4 * v], gf[4 * v + 1], gf[4 * v + 2], gf[4 * v + 3]);
-            reinterpret_cast<uint4*>(gp + 3 * TILE_CH)[v] = make_uint4(go[4 * v], go[4 * v + 1], go[4 * v + 2], go[4 * v + 3]);
-          }
-        } else if (valid) {
-          const float* bptr = (xfb ? xfb : prm.bias) + nt * BLOCK_N + j0;
-          const float* xft = prm.xf_B ? xft_of(prm.xf_ids[psmp]) : nullptr;
-          if (prm.xs_tab) {          // out[p] += in[p + off(tap)] . W[tap] with the input at the label cell only
-            const int l = prm.xs_label[psmp];
-            if (l >= 0 && l < g.H * g.W) {
-              const int ly = l / g.W, dy = ly - py, dx = (l - ly * g.W) - px;
-              if (dy >= -1 && dy <= 1 && dx >= -1 && dx <= 1)
-                xft = prm.xs_tab + ((long long)psmp * 9 + (dy + 1) * 3 + (dx + 1)) * kGates;
-            }
-          }
-          const float* tptr = xft ? xft + nt * BLOCK_N + j0 : nullptr;
-          const float* sptr = FMT == 1 ? prm.col_scale + nt * BLOCK_N + j0 : bptr;
-          float cn[16], hn[16];
-#pragma unroll
-          for (int v4 = 0; v4 < 4; ++v4) {
-            // bias (or bias-folded table), the x-fold table row of this cell and the column scales: one 128-bit load
-            // per gate and 4 columns
-            const float4* b4 = reinterpret_cast<const float4*>(bptr) + v4;
-            const float4* s4 = reinterpret_cast<const float4*>(sptr) + v4;
-            float4 qi = __ldg(b4 + 0 * (TILE_CH / 4)), qj = __ldg(b4 + 1 * (TILE_CH / 4)),
-                   qf = __ldg(b4 + 2 * (TILE_CH / 4)), qo = __ldg(b4 + 3 * (TILE_CH / 4));
-            if (tptr) {
-              const float4* t4 = reinterpret_cast<const float4*>(tptr) + v4;
-              const float4 ti = __ldg(t4 + 0 * (TILE_CH / 4)), tj = __ldg(t4 + 1 * (TILE_CH / 4)),
-                           tf = __ldg(t4 + 2 * (TILE_CH / 4)), to = __ldg(t4 + 3 * (TILE_CH / 4));
-              qi.x = __fadd_rn(qi.x, ti.x); qi.y = __fadd_rn(qi.y, ti.y); qi.z = __fadd_rn(qi.z, ti.z); qi.w = __fadd_rn(qi.w, ti.w);
-              qj.x = __fadd_rn(qj.x, tj.x); qj.y = __fadd_rn(qj.y, tj.y); qj.z = __fadd_rn(qj.z, tj.z); qj.w = __fadd_rn(qj.w, tj.w);
-              qf.x = __fadd_rn(qf.x, tf.x); qf.y = __fadd_rn(qf.y, tf.y); qf.z = __fadd_rn(qf.z, tf.z); qf.w = __fadd_rn(qf.w, tf.w);
-              qo.x = __fadd_rn(qo.x, to.x); qo.y = __fadd_rn(qo.y, to.y); qo.z = __fadd_rn(qo.z, to.z); qo.w = __fadd_rn(qo.w, to.w);
-            }
-            if (prm.xr_W) {           // + sum over taps and the two channels of x * W, fp32 (warp-uniform weight loads)
-              const float* wb = prm.xr_W + nt * BLOCK_N + j0 + 4 * v4;
-#pragma unroll
-              for (int k = 0; k < 18; ++k) {
-                const float4 wi = __ldg(reinterpret_cast<const float4*>(wb + k * kGates + 0 * TILE_CH)),
-                             wj = __ldg(reinterpret_cast<const float4*>(wb + k * kGates + 1 * TILE_CH)),
-                             wf = __ldg(reinterpret_cast<const float4*>(wb + k * kGates + 2 * TILE_CH)),
-                             wo = __ldg(reinterpret_cast<const float4*>(wb + k * kGates + 3 * TILE_CH));
-                const float xk = xv[k];
-                qi.x = __fmaf_rn(xk, wi.x, qi.x); qi.y = __fmaf_rn(xk, wi.y, qi.y); qi.z = __fmaf_rn(xk, wi.z, qi.z); qi.w = __fmaf_rn(xk, wi.w, qi.w);
-                qj.x = __fmaf_rn(xk, wj.x, qj.x); qj.y = __fmaf_rn(xk, wj.y, qj.y); qj.z = __fmaf_rn(xk, wj.z, qj.z); qj.w = __fmaf_rn(xk, wj.w, qj.w);
-                qf.x = __fmaf_rn(xk, wf.x, qf.x); qf.y = __fmaf_rn(xk, wf.y, qf.y); qf.z = __fmaf_rn(xk, wf.z, qf.z); qf.w = __fmaf_rn(xk, wf.w, qf.w);
-                qo.x = __fmaf_rn(xk, wo.x, qo.x); qo.y = __fmaf_rn(xk, wo.y, qo.y); qo.z = __fmaf_rn(xk, wo.z, qo.z); qo.w = __fmaf_rn(xk, wo.w, qo.w);
-              }
-            }
-            float4 si = qi, sj = qj, sf = qf, so = qo;
-            if (FMT == 1) {
-              si = __ldg(s4 + 0 * (TILE_CH / 4)); sj = __ldg(s4 + 1 * (TILE_CH / 4));
-              sf = __ldg(s4 + 2 * (TILE_CH / 4)); so = __ldg(s4 + 3 * (TILE_CH / 4));
-            }
-            const float bi[4] = {qi.x, qi.y, qi.z, qi.w}, bj[4] = {qj.x, qj.y, qj.z, qj.w},
-                        bf[4] = {qf.x, qf.y, qf.z, qf.w}, bo[4] = {qo.x, qo.y, qo.z, qo.w};
-            const float ci[4] = {si.x, si.y, si.z, si.w}, cj[4] = {sj.x, sj.y, sj.z, sj.w},
-                        cf[4] = {sf.x, sf.y, sf.z, sf.w}, co4[4] = {so.x, so.y, so.z, so.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int v = 4 * v4 + e;
-              const GateOut r = lstm_update(preact<FMT>(__uint_as_float(gi[v]), ci[e], bi[e]),
-                                            preact<FMT>(__uint_as_float(gj[v]), cj[e], bj[e]),
-                                            preact<FMT>(__uint_as_float(gf[v]), cf[e], bf[e]),
-                                            preact<FMT>(__uint_as_float(go[v]), co4[e], bo[e]), cprev[v], prm.forget_bias);
-              cn[v] = r.c;
-              hn[v] = r.h;
-              if (prm.gates_out) {   // reuse the accumulator registers as staging for the stores below
-                gi[v] = __float_as_uint(r.ai); gj[v] = __float_as_uint(r.aj);
-                gf[v] = __float_as_uint(r.af); go[v] = __float_as_uint(r.ao);
-              }
-            }
-          }
-          const long long orow = row;
-          if (prm.gates_out) {
-            float* gp = prm.gates_out + orow * kGates + nt * BLOCK_N + j0;
-#pragma unroll
-            for (int v = 0; v < 4; ++v) {
-              reinterpret_cast<uint4*>(gp + 0 * TILE_CH)[v] = make_uint4(gi[4 * v], gi[4 * v + 1], gi[4 * v + 2], gi[4 * v + 3]);
-              reinterpret_cast<uint4*>(gp + 1 * TILE_CH)[v] = make_uint4(gj[4 * v], gj[4 * v + 1], gj[4 * v + 2], gj[4 * v + 3]);
-              reinterpret_cast<uint4*>(gp + 2 * TILE_CH)[v] = make_uint4(gf[4 * v], gf[4 * v + 1], gf[4 * v + 2], gf[4 * v + 3]);
-              reinterpret_cast<uint4*>(gp + 3 * TILE_CH)[v] = make_uint4(go[4 * v], go[4 * v + 1], go[4 * v + 2], go[4 * v + 3]);
-            }
-          }
-          float4* co = reinterpret_cast<float4*>(prm.c_out + orow * kHidden + ch0);
-#pragma unroll
-          for (int v = 0; v < 4; ++v) co[v] = make_float4(cn[4 * v], cn[4 * v + 1], cn[4 * v + 2], cn[4 * v + 3]);
-          if (prm.h32_out) {
-            float4* ho = reinterpret_cast<float4*>(prm.h32_out + orow * kHidden + ch0);
-#pragma unroll
-            for (int v = 0; v < 4; ++v) ho[v] = make_float4(hn[4 * v], hn[4 * v + 1], hn[4 * v + 2], hn[4 * v + 3]);
-          }
-          if (prm.hp_out && prm.hp_mixed) {
-            const float (&h0)[8] = *reinterpret_cast<const float (*)[8]>(&hn[0]);
-            const float (&h1)[8] = *reinterpret_cast<const float (*)[8]>(&hn[8]);
-            store_f16f8_x8(prm.hp_out, prm.hp_plane_stride, orow, prm.ch_off_out + ch0, prm.cpad_out, h0);
-            store_f16f8_x8(prm.hp_out, prm.hp_plane_stride, orow, prm.ch_off_out + ch0 + 8, prm.cpad_out, h1);
-          } else if (prm.hp_out) {
-            uint32_t pk[P][8];
-#pragma unroll
-            for (int v = 0; v < 8; ++v) {
-              __nv_bfloat16 a[P], b[P];
-              split_planes<P>(hn[2 * v], a);
-              split_planes<P>(hn[2 * v + 1], b);
-#pragma unroll
-              for (int p = 0; p < P; ++p) pk[p][v] = pack_bf16x2(a[p], b[p]);
-            }
-#pragma unroll
-            for (int p = 0; p < P; ++p) {
-              uint4* po = reinterpret_cast<uint4*>(prm.hp_out + p * prm.hp_plane_stride +
-                                                   orow * prm.cpad_out + prm.ch_off_out + ch0);
-              po[0] = make_uint4(pk[p][0], pk[p][1], pk[p][2], pk[p][3]);
-              po[1] = make_uint4(pk[p][4], pk[p][5], pk[p][6], pk[p][7]);
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) { if (CG2) mbar_arrive_cta0(&tempty_bar[as]); else mbar_arrive(&tempty_bar[as]); }
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (PAIR) cluster_sync_all();     // the peer may still send into this CTA's smem / barriers / TMEM
-  if (warp == 2) { if (CG2) tmem_dealloc_2sm(tmem_base, 512); else tmem_dealloc(tmem_base, 512); }
+  if (MC) cluster_sync_all();     // the peer may still send into this CTA's smem / barriers
 }
 
 // ----------------------------------------------------------------------------------
@@ -836,10 +740,10 @@ static void note_variant(int planes, int pair) {
 struct CellMaps { CUtensorMap A, B, Bh, A8, B8, B8h; };
 
 // Work order of a launch (CellParams::order, work_index()).  1: the four N tiles of an M tile (pair) run back to back
-// on the same CTA (pair) - measured on the K=20 beam step: DRAM reads 1.05x algorithmic instead of 1.39x, 3 % faster.
+// on the same CTA (pair), so the tile's operand rows are re-read from L2 by the SM that fetched them.
 // 0: work items strided over the CTAs.  A launch of few M tiles (the encoders and the greedy decoders of a small
-// shard: 32 trajectories of 36x18 = 176 M tiles on 148 CTAs) is bound by its longest CTA instead: back to back the
-// busiest CTA runs 2 x 4 items, strided ceil(704 / 148) = 5.  Strided whenever that makespan is shorter and the
+// shard: 32 trajectories of 36x18 = 176 M tiles on 132 CTAs) is bound by its longest CTA instead: back to back the
+// busiest CTA runs 2 x 4 items, strided ceil(704 / 132) = 6.  Strided whenever that makespan is shorter and the
 // launch is small enough for its operands to stay in L2.
 static int pick_order(int forced, long long units, long long ctas) {
   if (forced == 0 || forced == 1) return forced;
@@ -855,12 +759,8 @@ static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms
   const int ra8 = (BLOCK_M + 2 * (prm.W + 2) + 7) & ~7;
   const int smem_bytes = Cfg::smem_bytes(ra8);
   MVB_REQUIRE(ra8 <= Cfg::MAX_RA8 && smem_bytes <= 227 * 1024, "cell_fwd: grid width W=%d too large (A stage of %d rows, %d B shared memory)", prm.W, ra8, smem_bytes);
-  static SmemOptIn opt_cg2;
-  MVB_CHECK_CUDA(smem_opt_in(opt_plain, cell_fwd_kernel<P, 0, FMT>, smem_bytes));
-  MVB_CHECK_CUDA(smem_opt_in(opt_mc, cell_fwd_kernel<P, 1, FMT>, smem_bytes));
-  MVB_CHECK_CUDA(smem_opt_in(opt_cg2, cell_fwd_kernel<P, 2, FMT>, smem_bytes));
-  // pair mode: 2 = cta_group::2 (default), 1 = two cta_group::1 CTAs with weight multicast (MVB_CELL_PAIR=1)
-  static const int pair_mode = [] { const char* e = getenv("MVB_CELL_PAIR"); return e ? atoi(e) : 2; }();
+  MVB_CHECK_CUDA(smem_opt_in(opt_plain, cell_fwd_kernel<P, false, FMT>, smem_bytes));
+  MVB_CHECK_CUDA(smem_opt_in(opt_mc, cell_fwd_kernel<P, true, FMT>, smem_bytes));
   const long long m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
   if (multicast && m_tiles >= 2 * (long long)num_sms) {
     prm.order = pick_order(prm_in.order, (m_tiles + 1) / 2, num_sms / 2);
@@ -871,8 +771,7 @@ static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    if (pair_mode == 2) MVB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, cell_fwd_kernel<P, 2, FMT>, tm.A, tm.Bh, tm.A8, tm.B8h, prm));
-    else MVB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, cell_fwd_kernel<P, 1, FMT>, tm.A, tm.Bh, tm.A8, tm.B8h, prm));
+    MVB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, cell_fwd_kernel<P, true, FMT>, tm.A, tm.Bh, tm.A8, tm.B8h, prm));
     count_launch(1);
     note_variant(FMT ? kPlanesF16F8 : P, 1);
     return MVB_OK;
@@ -880,7 +779,7 @@ static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms
   const long long num_tiles = m_tiles * N_TILES;
   const int grid = (int)(num_tiles < num_sms ? num_tiles : num_sms);
   prm.order = pick_order(prm_in.order, m_tiles, grid);
-  cell_fwd_kernel<P, 0, FMT><<<grid, NUM_THREADS, smem_bytes, stream>>>(tm.A, tm.B, tm.A8, tm.B8, prm);
+  cell_fwd_kernel<P, false, FMT><<<grid, NUM_THREADS, smem_bytes, stream>>>(tm.A, tm.B, tm.A8, tm.B8, prm);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   note_variant(FMT ? kPlanesF16F8 : P, 0);

@@ -1,4 +1,4 @@
-// Common device/host helpers for libmultiverse_b200 (sm_100a only).
+// Common device/host helpers for libmultiverse_b200 (H100, sm_90a only).
 //
 // Internal "halo" layout used by every kernel of the hot path:
 //   a location grid of H x W cells is stored with ONE shared zero column and ONE
@@ -17,6 +17,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
+#include "mvb_wgmma.cuh"
 
 namespace mvb {
 
@@ -82,11 +83,11 @@ __device__ __forceinline__ void split_planes(float v, __nv_bfloat16 (&out)[P]) {
 // ----------------------------------------------------------------------------------
 // "f16f8" operand format (planes code kPlanesF16F8): v = a0 + a1 with a0 = fp16(v); the tensor cores see
 //   a0 (fp16 plane), e0 = e4m3(a0) and e1 = e4m3(a1 * 2^12) (two fp8 planes), and the product of two such
-// operands is accumulated as   a0*b0 (kind::f16)  +  e0(a)*e0'(b)  +  e1(a)*e1'(b)  (kind::f8f6f4, twice the rate)
+// operands is accumulated as   a0*b0 (fp16 wgmma)  +  e0(a)*e0'(b)  +  e1(a)*e1'(b)  (e4m3 wgmma, twice the rate)
 // where for the WEIGHT operand e0' = e4m3(b1) and e1' = e4m3(b0 * 2^-12): the two fp8 products are the cross
 // terms a0*b1 and a1*b0 to 4 significant bits, i.e. to 2^-17 of the main product; a1*b1 (2^-24) is dropped.
-// All three products have the same scale, so they share ONE fp32 TMEM accumulator.  2 bf16-pass equivalents
-// instead of 3 at the accuracy class of the bf16 x 2-plane scheme (profiles/r02_numerics_gate*.json).
+// All three products have the same scale, so they share ONE fp32 accumulator.  2 bf16-pass equivalents
+// instead of 3 at the accuracy class of the bf16 x 2-plane scheme.
 // Buffer layout for R rows of cpad channels: [fp16 R*cpad][fp8: R rows of 2*cpad bytes] = the bytes of two bf16
 // planes, so the same allocations serve both formats.  Inside an fp8 row the two planes are interleaved per K chunk
 // of the cell kernel, so that ONE 128-byte TMA row carries both (f8_off): [x block: e0 (cxp) | e1 (cxp)] then per
@@ -194,15 +195,15 @@ inline cudaError_t smem_opt_in(SmemOptIn& st, Kernel kernel, size_t bytes) {
   return e;
 }
 
-// Number of SMs of the current device (cached per device; 148 on B200): grid-stride launchers size their grids in
+// Number of SMs of the current device (cached per device; 132 on the H100 SXM): grid-stride launchers size their grids in
 // multiples of it instead of a hard-coded constant.
 inline int sm_count() {
   static int cached[64] = {};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (!cached[dev]) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -227,23 +228,12 @@ __device__ __forceinline__ float warp_fold8(const float (&v)[8], int lane) {
 }
 __device__ __forceinline__ int warp_fold8_index(int lane) { return ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1); }
 
-// Packed fp32 pairs: sm_100 issues two FMAs per lane from one instruction (SASS FFMA2).  The graph-attention and
-// head kernels are bound by instruction issue, not by the FMA pipe, so their dot products and weighted sums work on
-// float2.
+// fp32 pairs: the graph-attention and head kernels write their dot products and weighted sums on float2; each lane
+// is one correctly rounded fma / mul (H100 has no packed fp32 FMA instruction).
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("{\n\t.reg .b64 ra, rb, rc, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-      "fma.rn.f32x2 rd, ra, rb, rc;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-      : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-  return d;
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-  float2 d;
-  asm("{\n\t.reg .b64 ra, rb, rd;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-      "mul.rn.f32x2 rd, ra, rb;\n\tmov.b64 {%0, %1}, rd;\n\t}"
-      : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
-}
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -257,7 +247,7 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // ----------------------------------------------------------------------------------
-// PTX wrappers: mbarrier, TMA, tcgen05
+// PTX wrappers: mbarrier, TMA, clusters, wgmma descriptors
 // ----------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -315,7 +305,7 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ---- 2-CTA (cta_group::2) variants: a CTA pair of one cluster shares one 256-row UMMA ----
+// ---- clusters: CTAs of one cluster exchange operand tiles and barrier arrivals ----
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -325,18 +315,7 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // shared::cluster address of the same offset in CTA 0 of the pair
 
-// TMA load issued by both CTAs of a pair; data lands in the issuing CTA's smem, the transaction
-// bytes are reported to CTA 0's barrier.
-__device__ __forceinline__ void tma_load_3d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar,
-                                                int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 // TMA load multicast to the CTAs of `mask`: the box lands at the same smem offset in each of them and each of
 // their barriers (same offset) receives the transaction bytes.
 __device__ __forceinline__ void tma_load_3d_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0,
@@ -345,14 +324,6 @@ __device__ __forceinline__ void tma_load_3d_mc(void* dst, const CUtensorMap* m, 
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
       " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_u32(dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
-      : "memory");
-}
-// tcgen05.commit of this CTA's MMAs, arriving on the barrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
       : "memory");
 }
 // arrive on the barrier at the same offset in CTA `cta` of the cluster
@@ -366,160 +337,33 @@ __device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) 
       "r"(cta)
       : "memory");
 }
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                              uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f8_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the barrier at this offset in CTA 0 of the pair (from either CTA)
-__device__ __forceinline__ void mbar_arrive_cta0(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-// arrive on the barrier at this offset in BOTH CTAs once the pair's previously issued MMAs retire
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
 
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
+// Register budget of a warpgroup (setmaxnreg): the TMA producer warpgroup hands its registers to the MMA
+// warpgroups, whose fp32 accumulators live in registers.
+template <int R>
+__device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// Allocate `ncols` TMEM columns (power of two >= 32); whole warp executes.
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 x bf16 -> fp32, one CTA.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// D[tmem] (+)= A * B with 8-bit float operands (e4m3 / e5m2 chosen by idesc), fp32 accumulate, one CTA.
-__device__ __forceinline__ void umma_f8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Issue-thread-cheap forms: the MMA issuer is ONE thread and every instruction it executes costs ~4-6 cycles of its
-// dependent-issue latency; with a dispatch due every 128 cycles, descriptor arithmetic must stay at one IADD per operand.
-// A shared-memory descriptor is {lo = (address >> 4) [+ lbo << 16], hi = sbo >> 4 | 1 << 14 | layout << 29}: only `lo`
-// moves along K / rows, by (bytes >> 4).  KIND: 0 = kind::f16, 1 = kind::f8f6f4; CG2: cta_group::2; ACC: accumulate.
-constexpr uint32_t smem_desc_hi(uint32_t sbo_bytes, uint32_t layout_type) {
-  return (sbo_bytes >> 4) | (1u << 14) | (layout_type << 29);
-}
-template <int KIND, bool CG2, bool ACC>
-__device__ __forceinline__ void umma_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc) {
-  if (KIND == 0 && !CG2)
-    asm volatile("{\n.reg .pred p;\n.reg .b64 ad, bd;\nsetp.ne.b32 p, %5, 0;\nmov.b64 ad, {%1, %3};\nmov.b64 bd, {%2, %3};\n"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], ad, bd, %4, p;\n}\n" ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(hi),
-                 "r"(idesc), "n"(ACC ? 1 : 0) : "memory");
-  else if (KIND == 0)
-    asm volatile("{\n.reg .pred p;\n.reg .b64 ad, bd;\nsetp.ne.b32 p, %5, 0;\nmov.b64 ad, {%1, %3};\nmov.b64 bd, {%2, %3};\n"
-                 "tcgen05.mma.cta_group::2.kind::f16 [%0], ad, bd, %4, p;\n}\n" ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(hi),
-                 "r"(idesc), "n"(ACC ? 1 : 0) : "memory");
-  else if (!CG2)
-    asm volatile("{\n.reg .pred p;\n.reg .b64 ad, bd;\nsetp.ne.b32 p, %5, 0;\nmov.b64 ad, {%1, %3};\nmov.b64 bd, {%2, %3};\n"
-                 "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], ad, bd, %4, p;\n}\n" ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(hi),
-                 "r"(idesc), "n"(ACC ? 1 : 0) : "memory");
-  else
-    asm volatile("{\n.reg .pred p;\n.reg .b64 ad, bd;\nsetp.ne.b32 p, %5, 0;\nmov.b64 ad, {%1, %3};\nmov.b64 bd, {%2, %3};\n"
-                 "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], ad, bd, %4, p;\n}\n" ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(hi),
-                 "r"(idesc), "n"(ACC ? 1 : 0) : "memory");
-}
-
-// mbarrier arrive once all previously issued tcgen05.mma of this thread retire.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-
-// TMEM -> registers: this thread's lane (row), 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// K-major shared-memory matrix descriptor (SM100 "version 1"), swizzle given by
-// layout_type (2 = 128B, 4 = 64B, 6 = 32B); sbo = byte stride between 8-row groups.
+// K-major or MN-major shared-memory matrix descriptor of wgmma (sm_90): start address, leading / stride byte offsets
+// and the swizzle of the TMA-written tile (layout_type 1 = 128B, 2 = 64B, 3 = 32B).  The hardware applies the swizzle
+// to the absolute shared-memory address bits, like the TMA unit that wrote the tile, so a descriptor may start at
+// any 16-byte step inside a swizzled row (K) and at any row.  sbo = byte stride between 8-row groups.
+constexpr uint32_t kSwizzle128B = 1, kSwizzle64B = 2;
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t sbo_bytes,
                                                    uint32_t layout_type, uint32_t lbo_bytes = 0) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)(lbo_bytes >> 4) << 16;
   d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout_type << 61;
+  d |= (uint64_t)layout_type << 62;
   return d;
 }
+// the same as {lo, hi} halves: only `lo` (address >> 4) moves along K / rows
+constexpr uint32_t smem_desc_hi(uint32_t sbo_bytes, uint32_t layout_type) {
+  return (sbo_bytes >> 4) | (layout_type << 30);
+}
+__device__ __forceinline__ uint64_t desc_of(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
 
 // ----------------------------------------------------------------------------------
 // host: TMA descriptor encode through the runtime's driver entry point (no -lcuda)

@@ -4,17 +4,15 @@
 //   lstm_gates_bwd   pointwise: (dh_t, dc_t, gates_t, c_{t-1}, c_t) -> dG_t (pre-activation gate
 //                    gradients, bf16 planes, packed column order), dc_{t-1}, dbias
 //   cell dgrad       dxh[r, c]  = sum_tap sum_g dG[r - shift(tap), g] * W[tap, c, g]
-//                    = one tcgen05 implicit GEMM  [R, 9*1024] x [9*1024, cpad]   (same halo trick
+//                    = one wgmma implicit GEMM  [R, 9*1024] x [9*1024, cpad]   (same halo trick
 //                    as the forward: a tap is a constant row shift of the dG matrix)
 //   cell wgrad       dW[tap, c, g] = sum_r xh[r + shift(tap), c] * dG[r, g]
-//                    = tcgen05 GEMM  dG^T [1024, R] x xh^T_tap [cpad, R]^T over 9 tap-shifted
-//                    transposes of the activations; 8 x 18 output tiles = one wave of CTAs,
-//                    each looping over all R rows (K) and adding into the fp32 dW accumulator
+//                    = wgmma GEMM  dG^T [1024, R] x xh^T_tap [cpad, R]^T over 9 tap-shifted
+//                    transposes of the activations; 8 x 18 output tiles, each CTA looping over all R rows (K)
+//                    and adding into the fp32 dW accumulator
 // Both GEMMs use the forward kernel's operand-plane scheme (P bf16 planes, products i+j<P) and
-// the same TMA / mbarrier / TMEM pipeline.  dgrad tiles: two N tiles of cpad/2 when the x block is
-// needed, one N = 256 tile (h block only) when it is not (regression encoder).  Measured on B200: MMA
-// time is proportional to N (no granule penalty at N = 144); a separate 32-wide x tile is TMA-bound and
-// costs 30 % of an h tile; a cta_group::2 variant gave no gain (the kernel is not smem-bandwidth bound).
+// the same TMA / mbarrier pipeline with register accumulators.  dgrad tiles: two N tiles of cpad/2 when the x
+// block is needed, one N = 256 tile (h block only) when it is not (regression encoder).
 // Algorithmic FLOPs: dgrad = wgrad = forward (2*R*9*cpad*1024 each).
 #include "mvb_common.cuh"
 #include "mvb_kernels.h"
@@ -22,35 +20,30 @@
 
 namespace mvb {
 
-constexpr int G_BLOCK_M = 128;
+constexpr int G_BLOCK_M = 128;                         // two MMA warpgroups of 64 rows
 constexpr int G_BLOCK_K = 32;
-constexpr int G_UMMA_K = 16;
+constexpr int G_MMA_K = 16;
 constexpr int G_MAX_BN = 256;
-constexpr int G_EPI_WARPS = 4;
-constexpr int G_THREADS = 128 + 32 * G_EPI_WARPS;
+constexpr int G_THREADS = 384;
 constexpr int G_A_PLANE = G_BLOCK_M * G_BLOCK_K * 2;   // 8 KB
 constexpr int G_B_PLANE = G_MAX_BN * G_BLOCK_K * 2;    // 16 KB (smaller N tiles use part of it)
-constexpr uint32_t G_SW64_LAYOUT = 4;
+constexpr uint32_t G_SW64_LAYOUT = kSwizzle64B;
 constexpr uint32_t G_SW64_SBO = 512;
 
 enum { MODE_DGRAD = 0, MODE_WGRAD = 1, MODE_WGRAD_MN = 2 };
 
-// MT = number of 128-row M sub-tiles of one CTA tile.  MT = 2 halves the B traffic per MMA (the backward GEMMs
-// are L2->smem feed bound at MT = 1: 79 / 69 B/clk/SM against ~60 the forward sustains); its two accumulators
-// fill TMEM's 512 columns, so there is one accumulator stage and the (light) epilogue is not overlapped.
-template <int P, int MT> struct GemmCfg {
-  static constexpr int A_BYTES = MT * P * G_A_PLANE;
+template <int P> struct GemmCfg {
+  static constexpr int A_BYTES = P * G_A_PLANE;
   static constexpr int STAGE_BYTES = A_BYTES + P * G_B_PLANE;
   static constexpr int STAGES = (227 * 1024 - 2048) / STAGE_BYTES > 8 ? 8 : (227 * 1024 - 2048) / STAGE_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
-  static constexpr int NACC = MT == 1 ? 2 : 1;
 };
 
 struct GemmParams {
   float* out;          // dgrad: [R, cpad] fp32;  wgrad: [1024, 9*cpad] fp32 accumulator (+=)
   long long R;         // halo rows
   int H, W;
-  int cpad, bn;        // N tile of the wgrad modes
+  int cpad, bn;        // N tile
   int cxp;             // dgrad: width of the x block
   int need_x;          // dgrad: 1 -> two N tiles of cpad/2 covering [0, cpad); 0 -> one N tile [cxp, cxp+256) (h only)
   int num_kb;          // k-blocks per tile
@@ -62,151 +55,135 @@ struct GemmParams {
   int upt;             // units per N tile (bn = upt * ubn): two 96-wide units are paired into N = 192
   int n_units;         // 9 * n_per_tap
   int ksplit;          // K (= halo rows) is split over this many work items, each with its own fp32 slab
-  uint32_t lbo, sbo;   // UMMA descriptor strides of the MN-major SWIZZLE_64B tiles
+  uint32_t lbo, sbo;   // descriptor strides of the MN-major SWIZZLE_64B tiles
 };
 
-template <int P, int MODE, int MT>
+// BN = N tile (columns of the accumulator).  Warpgroup 0 loads; warpgroups 1 and 2 multiply and store 64 rows each.
+template <int P, int MODE, int BN>
 __global__ void __launch_bounds__(G_THREADS, 1)
 pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const GemmParams prm) {
-  using Cfg = GemmCfg<P, MT>;
+  using Cfg = GemmCfg<P>;
+  constexpr bool MN = MODE == MODE_WGRAD_MN;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tfull_bar = empty_bar + Cfg::STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const Grid g = make_grid(prm.H, prm.W);
-  const long long num_tiles = prm.num_m_tiles * prm.num_n_tiles;     // num_m_tiles counts CTA tiles of MT*128 rows
-  const uint32_t stage_tx = (uint32_t)(Cfg::A_BYTES + P * prm.bn * G_BLOCK_K * 2);
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(prm.bn >> 3) << 17) |
-                         ((uint32_t)(G_BLOCK_M >> 4) << 24) |
-                         (MODE == MODE_WGRAD_MN ? ((1u << 15) | (1u << 16)) : 0u);   // A, B MN-major
-  // byte offset of (M sub-tile j, plane pa) inside a stage's A region
-  auto a_off = [&](int j, int pa) -> uint32_t {
-    return MODE == MODE_WGRAD_MN ? (uint32_t)(pa * MT * G_A_PLANE + j * G_A_PLANE)    // one TMA box [P][4*MT blocks]
-                                 : (uint32_t)((j * P + pa) * G_A_PLANE);              // MT boxes of [P][128 rows]
-  };
-
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tfull_bar[a], 1); mbar_init(&tempty_bar[a], G_EPI_WARPS); }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  const long long num_tiles = prm.num_m_tiles * prm.num_n_tiles;
+  const uint32_t stage_tx = (uint32_t)(Cfg::A_BYTES + P * BN * G_BLOCK_K * 2);
 
   if (warp == 0 && lane == 0) {
-    // ===================== TMA producer =====================
+    prefetch_tmap(&tmA); prefetch_tmap(&tmB);
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    regs_dealloc<40>();
+    if (warp == 0 && lane == 0) {
+      // ===================== TMA producer =====================
+      int stage = 0; uint32_t phase = 0;
+      for (long long t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const long long mt = t / prm.num_n_tiles;
+        const int ntile = (int)(t % prm.num_n_tiles);
+        for (int kb = 0; kb < prm.num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
+          uint8_t* sb = sa + Cfg::A_BYTES;
+          mbar_expect_tx(&full_bar[stage], stage_tx);
+          if (MODE == MODE_DGRAD) {
+            // A = dG[rows - shift(tap), 32 gate columns];  B = Wd[N channels, tap*1024 + 32 gate columns]
+            const int q = kb / 9, tap = kb - q * 9;
+            const int shift = (tap / 3 - 1) * g.Wp + (tap % 3 - 1);
+            tma_load_3d(sa, &tmA, &full_bar[stage], q * G_BLOCK_K, (int)(mt * G_BLOCK_M - shift), 0);
+            tma_load_3d(sb, &tmB, &full_bar[stage], tap * kGates + q * G_BLOCK_K,
+                        prm.need_x ? ntile * BN : prm.cxp, 0);
+          } else if (MODE == MODE_WGRAD) {
+            // A = dG^T[128 gate rows, 32 halo rows];  B = tap-shifted xh^T[tap][bn channels, 32 halo rows]
+            const int tap = ntile >> 1, half = ntile & 1;
+            tma_load_3d(sa, &tmA, &full_bar[stage], kb * G_BLOCK_K, (int)(mt * G_BLOCK_M), 0);
+            tma_load_3d(sb, &tmB, &full_bar[stage], kb * G_BLOCK_K, tap * prm.cpad + half * BN, 0);
+          } else {
+            // MN-major: A = dG[32 halo rows (K), 4 blocks of 32 gate columns]; B = `upt` units, each
+            // xh[32 halo rows + shift(tap), nb blocks of 32 channels]; ntile = (unit group, k-split)
+            const int ks = ntile % prm.ksplit, grp = ntile / prm.ksplit;
+            const int k0 = (ks * prm.num_kb + kb) * G_BLOCK_K;
+            tma_load_4d(sa, &tmA, &full_bar[stage], 0, k0, (int)mt * 4, 0);
+            for (int j = 0; j < prm.upt; ++j) {
+              int u = grp * prm.upt + j;
+              if (u >= prm.n_units) u = prm.n_units - 1;     // odd tail: duplicate, discarded by the epilogue
+              const int tap = u / prm.n_per_tap, chunk = u - tap * prm.n_per_tap;
+              const int shift = (tap / 3 - 1) * g.Wp + (tap % 3 - 1);
+              for (int p = 0; p < P; ++p)
+                tma_load_4d(sb + p * (BN * 64) + j * (prm.ubn * 64), &tmB, &full_bar[stage], 0, k0 + shift,
+                            chunk * prm.nb, p);
+            }
+          }
+          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    regs_alloc<232>();
+    // ===================== MMA + epilogue: rows [64 c, +64) of the tile =====================
+    const int c = wg - 1;
+    const bool leader = (threadIdx.x & 127) == 0;          // arrives on the barriers for the warpgroup
+    constexpr uint32_t b_plane = (uint32_t)BN * G_BLOCK_K * 2;   // TMA packs planes back to back
+    // this warpgroup's 64 rows: K-major: 64 rows of 64 B; MN-major: two 32-wide MN blocks of [32 K rows][64 B]
+    const uint32_t a_wg = MN ? (uint32_t)c * 2 * 2048 : (uint32_t)c * 64 * 64;
+    float acc[BN / 2];
     int stage = 0; uint32_t phase = 0;
     for (long long t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const long long mt = t / prm.num_n_tiles;
       const int ntile = (int)(t % prm.num_n_tiles);
-      for (int kb = 0; kb < prm.num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-        uint8_t* sb = sa + Cfg::A_BYTES;
-        mbar_expect_tx(&full_bar[stage], stage_tx);
-        if (MODE == MODE_DGRAD) {
-          // A = dG[rows - shift(tap), 32 gate columns];  B = Wd[N channels, tap*1024 + 32 gate columns]
-          const int q = kb / 9, tap = kb - q * 9;
-          const int shift = (tap / 3 - 1) * g.Wp + (tap % 3 - 1);
-          for (int j = 0; j < MT; ++j)
-            tma_load_3d(sa + a_off(j, 0), &tmA, &full_bar[stage], q * G_BLOCK_K,
-                        (int)((mt * MT + j) * G_BLOCK_M - shift), 0);
-          tma_load_3d(sb, &tmB, &full_bar[stage], tap * kGates + q * G_BLOCK_K,
-                      prm.need_x ? ntile * prm.bn : prm.cxp, 0);
-        } else if (MODE == MODE_WGRAD) {
-          // A = dG^T[128 gate rows, 32 halo rows];  B = tap-shifted xh^T[tap][bn channels, 32 halo rows]
-          const int tap = ntile >> 1, half = ntile & 1;
-          tma_load_3d(sa, &tmA, &full_bar[stage], kb * G_BLOCK_K, (int)(mt * G_BLOCK_M), 0);
-          tma_load_3d(sb, &tmB, &full_bar[stage], kb * G_BLOCK_K, tap * prm.cpad + half * prm.bn, 0);
-        } else {
-          // MN-major: A = dG[32 halo rows (K), 4*MT blocks of 32 gate columns]; B = `upt` units, each
-          // xh[32 halo rows + shift(tap), nb blocks of 32 channels]; ntile = (unit group, k-split)
-          const int ks = ntile % prm.ksplit, grp = ntile / prm.ksplit;
-          const int k0 = (ks * prm.num_kb + kb) * G_BLOCK_K;
-          tma_load_4d(sa, &tmA, &full_bar[stage], 0, k0, (int)mt * 4 * MT, 0);
-          for (int j = 0; j < prm.upt; ++j) {
-            int u = grp * prm.upt + j;
-            if (u >= prm.n_units) u = prm.n_units - 1;     // odd tail: duplicate, discarded by the epilogue
-            const int tap = u / prm.n_per_tap, chunk = u - tap * prm.n_per_tap;
-            const int shift = (tap / 3 - 1) * g.Wp + (tap % 3 - 1);
-            for (int p = 0; p < P; ++p)
-              tma_load_4d(sb + p * (prm.bn * 64) + j * (prm.ubn * 64), &tmB, &full_bar[stage], 0, k0 + shift,
-                          chunk * prm.nb, p);
-          }
-        }
-        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ===================== MMA issuer =====================
-    int stage = 0; uint32_t phase = 0;
-    long long it = 0;
-    for (long long t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-      const int as = (int)(it % Cfg::NACC);
-      const uint32_t aphase = (uint32_t)((it / Cfg::NACC) & 1);
-      mbar_wait(&tempty_bar[as], aphase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * MT * 256;
-      const uint32_t b_plane = (uint32_t)prm.bn * G_BLOCK_K * 2;   // TMA packs planes back to back
+      int prev = -1;
       for (int kb = 0; kb < prm.num_kb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
         const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
         const uint32_t sb = sa + Cfg::A_BYTES;
+        uint32_t accumulate = kb == 0 ? 0u : 1u;
+        wgmma_fence_regs(acc);
+        wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < MT; ++j) {
-          uint32_t first = (kb == 0) ? 0u : 1u;
+        for (int pa = 0; pa < P; ++pa) {
 #pragma unroll
-          for (int pa = 0; pa < P; ++pa) {
+          for (int pb = 0; pb < P - pa; ++pb) {
 #pragma unroll
-            for (int pb = 0; pb < P - pa; ++pb) {
-#pragma unroll
-              for (int k = 0; k < G_BLOCK_K / G_UMMA_K; ++k) {
-                uint64_t ad, bd;
-                if (MODE == MODE_WGRAD_MN) {
-                  // one UMMA consumes 16 K rows = two 8-row groups (sbo apart) of every 32-wide MN block
-                  ad = make_smem_desc(sa + a_off(j, pa) + k * 2 * prm.sbo, prm.sbo, G_SW64_LAYOUT, prm.lbo);
-                  bd = make_smem_desc(sb + pb * b_plane + k * 2 * prm.sbo, prm.sbo, G_SW64_LAYOUT, prm.lbo);
-                } else {
-                  ad = make_smem_desc(sa + a_off(j, pa) + k * G_UMMA_K * 2, G_SW64_SBO, G_SW64_LAYOUT);
-                  bd = make_smem_desc(sb + pb * b_plane + k * G_UMMA_K * 2, G_SW64_SBO, G_SW64_LAYOUT);
-                }
-                umma_bf16(d_tmem + j * 256, ad, bd, idesc, first);
-                first = 1u;
+            for (int k = 0; k < G_BLOCK_K / G_MMA_K; ++k) {
+              uint64_t ad, bd;
+              if (MN) {
+                // one MMA consumes 16 K rows = two 8-row groups (sbo apart) of every 32-wide MN block
+                ad = make_smem_desc(sa + pa * G_A_PLANE + a_wg + k * 2 * prm.sbo, prm.sbo, G_SW64_LAYOUT, prm.lbo);
+                bd = make_smem_desc(sb + pb * b_plane + k * 2 * prm.sbo, prm.sbo, G_SW64_LAYOUT, prm.lbo);
+              } else {
+                ad = make_smem_desc(sa + pa * G_A_PLANE + a_wg + k * G_MMA_K * 2, G_SW64_SBO, G_SW64_LAYOUT);
+                bd = make_smem_desc(sb + pb * b_plane + k * G_MMA_K * 2, G_SW64_SBO, G_SW64_LAYOUT);
               }
+              wgmma_bf16<BN, MN ? 1 : 0, MN ? 1 : 0>(acc, ad, bd, accumulate);
+              accumulate = 1u;
             }
           }
         }
-        umma_commit(&empty_bar[stage]);
+        wgmma_commit();
+        wgmma_fence_regs(acc);
+        wgmma_wait<1>();                       // the previous k-block's MMAs have completed: refill its stage
+        if (leader && prev >= 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
         if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
       }
-      umma_commit(&tfull_bar[as]);
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue: TMEM -> fp32 global =====================
-    const int wq = warp & 3;
-    long long it = 0;
-    for (long long t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-      const int as = (int)(it % Cfg::NACC);
-      const uint32_t aphase = (uint32_t)((it / Cfg::NACC) & 1);
-      const long long mt = t / prm.num_n_tiles;
-      const int ntile = (int)(t % prm.num_n_tiles);
-      mbar_wait(&tfull_bar[as], aphase);
-      tc_fence_after();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (leader && prev >= 0) mbar_arrive(&empty_bar[prev]);
+      // ===================== epilogue: registers -> fp32 global =====================
+      // thread (warp w of the warpgroup, lane l) holds rows 16 w + l / 4 (+ 8) and columns 8 i + 2 (l % 4) (+ 1)
 #pragma unroll
-      for (int j = 0; j < MT; ++j) {
-        const long long row = (mt * MT + j) * G_BLOCK_M + wq * 32 + lane;
+      for (int hr = 0; hr < 2; ++hr) {
+        const long long row = mt * G_BLOCK_M + 64 * c + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
         bool valid;
         float* dst;
         if (MODE == MODE_DGRAD) {
@@ -216,49 +193,35 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             const int y = rem / g.Wp, x = rem - y * g.Wp;
             valid = (x < g.W) && (y < g.H);
           }
-          dst = prm.out + row * prm.cpad + (prm.need_x ? ntile * prm.bn : prm.cxp);
+          dst = prm.out + row * prm.cpad + (prm.need_x ? ntile * BN : prm.cxp);
         } else if (MODE == MODE_WGRAD) {
           valid = row < kGates;
           const int tap = ntile >> 1, half = ntile & 1;
-          dst = prm.out + row * (9LL * prm.cpad) + tap * prm.cpad + half * prm.bn;
+          dst = prm.out + row * (9LL * prm.cpad) + tap * prm.cpad + half * BN;
         } else {
           valid = row < kGates;
           dst = prm.out + (long long)(ntile % prm.ksplit) * kGates * 9LL * prm.cpad + row * (9LL * prm.cpad);
         }
-        const uint32_t t_row = tmem_base + ((uint32_t)(wq * 32) << 16) + (as * MT + j) * 256;
-        for (int c0 = 0; c0 < prm.bn; c0 += 16) {
-          uint32_t v[16];
-          tmem_ld16(t_row + c0, v);
-          tmem_ld_wait();
-          bool ok = valid;
-          float4* d4 = reinterpret_cast<float4*>(dst + c0);
-          if (MODE == MODE_WGRAD_MN) {
-            // column c0 of the tile -> (unit, channel): dW[tap][chunk*ubn + c]; this (tile, k-split) owns its slab
-            const int ju = c0 / prm.ubn;
-            const int u = (ntile / prm.ksplit) * prm.upt + ju;
-            ok = valid && u < prm.n_units;
-            const int tap = u / prm.n_per_tap, chunk = u - tap * prm.n_per_tap;
-            d4 = reinterpret_cast<float4*>(dst + tap * prm.cpad + chunk * prm.ubn + (c0 - ju * prm.ubn));
-          }
-          if (ok) {
+        if (!valid) continue;
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              float4 o = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]),
-                                     __uint_as_float(v[4 * q + 2]), __uint_as_float(v[4 * q + 3]));
-              if (MODE != MODE_DGRAD) { const float4 old = d4[q]; o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w; }
-              d4[q] = o;
-            }
+        for (int i = 0; i < BN / 8; ++i) {
+          const int col = 8 * i + 2 * (lane & 3);
+          float2* d2 = reinterpret_cast<float2*>(dst + col);
+          if (MN) {
+            // column of the tile -> (unit, channel): dW[tap][chunk*ubn + c]; this (tile, k-split) owns its slab
+            const int ju = col / prm.ubn;
+            const int u = (ntile / prm.ksplit) * prm.upt + ju;
+            if (u >= prm.n_units) continue;
+            const int tap = u / prm.n_per_tap, chunk = u - tap * prm.n_per_tap;
+            d2 = reinterpret_cast<float2*>(dst + tap * prm.cpad + chunk * prm.ubn + (col - ju * prm.ubn));
           }
+          float2 o = make_float2(acc[4 * i + 2 * hr], acc[4 * i + 2 * hr + 1]);
+          if (MODE != MODE_DGRAD) { const float2 old = *d2; o.x += old.x; o.y += old.y; }
+          *d2 = o;
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[as]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
 }
 
 // ----------------------------------------------------------------------------------
@@ -436,18 +399,32 @@ __global__ void unpack_wgrad_kernel(const float* __restrict__ dwp, const float* 
   }
 }
 
-template <int P, int MODE, int MT>
-static int launch_pgemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& prm, int num_sms,
-                        cudaStream_t stream) {
-  using Cfg = GemmCfg<P, MT>;
+template <int P, int MODE, int BN>
+static int launch_pgemm_n(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& prm, int num_sms,
+                          cudaStream_t stream) {
+  using Cfg = GemmCfg<P>;
   static SmemOptIn opt;
-  MVB_CHECK_CUDA(smem_opt_in(opt, pgemm_kernel<P, MODE, MT>, Cfg::SMEM_BYTES));
+  MVB_CHECK_CUDA(smem_opt_in(opt, pgemm_kernel<P, MODE, BN>, Cfg::SMEM_BYTES));
   const long long tiles = prm.num_m_tiles * prm.num_n_tiles;
   const int grid = (int)(tiles < num_sms ? tiles : num_sms);
-  pgemm_kernel<P, MODE, MT><<<grid, G_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, prm);
+  pgemm_kernel<P, MODE, BN><<<grid, G_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, prm);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;
+}
+
+// the N tiles the three GEMMs use: cpad / 2 (144, 160), 192 (two 96-wide units) and 256
+template <int P, int MODE>
+static int launch_pgemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& prm, int num_sms,
+                        cudaStream_t stream) {
+  switch (prm.bn) {
+    case 144: return launch_pgemm_n<P, MODE, 144>(tmA, tmB, prm, num_sms, stream);
+    case 160: return launch_pgemm_n<P, MODE, 160>(tmA, tmB, prm, num_sms, stream);
+    case 192: return launch_pgemm_n<P, MODE, 192>(tmA, tmB, prm, num_sms, stream);
+    case 256: return launch_pgemm_n<P, MODE, 256>(tmA, tmB, prm, num_sms, stream);
+    default: MVB_REQUIRE(false, "pgemm: N tile %d unsupported", prm.bn);
+  }
+  return MVB_ERR_INVALID;
 }
 
 static int num_sms_of_device(int* out) {
@@ -470,8 +447,7 @@ int cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, long lo
                                G_BLOCK_K, G_BLOCK_M, P, 64);
   if (rc) return rc;
   const uint64_t ktot = 9ull * kGates;
-  // with the x block: two N tiles of cpad/2 (144 / 160); h only: one N tile of 256.  (Measured: MMA time is
-  // proportional to N, and a separate 32-wide x tile is TMA-bound and costs 30 % of an h tile.)
+  // with the x block: two N tiles of cpad/2 (144 / 160); h only: one N tile of 256
   const int bn = need_x ? cpad / 2 : 256;
   MVB_REQUIRE(bn % 16 == 0, "cell_dgrad: cpad=%d unsupported", cpad);
   rc = encode_tmap_3d_bf16(&tmB, wd_planes, ktot, (uint64_t)cpad, P, ktot * 2, ktot * cpad * 2, G_BLOCK_K, bn, P, 64);
@@ -479,24 +455,14 @@ int cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, long lo
   GemmParams prm = {};
   prm.out = dxh; prm.R = R; prm.H = H; prm.W = W; prm.cpad = cpad; prm.bn = bn; prm.cxp = cxp; prm.need_x = need_x;
   prm.num_kb = 9 * (kGates / G_BLOCK_K);
-  // with the x block (N = 144 / 160) a CTA tile is 256 rows (two accumulators sharing every B tile);
-  // the h-only N = 256 tile already has the forward kernel's operand intensity
-  const int mt_sub = need_x ? 2 : 1;
-  prm.num_m_tiles = (R + G_BLOCK_M * mt_sub - 1) / (G_BLOCK_M * mt_sub);
+  prm.num_m_tiles = (R + G_BLOCK_M - 1) / G_BLOCK_M;
   prm.num_n_tiles = need_x ? 2 : 1;
   int sms = 0;
   if ((rc = num_sms_of_device(&sms))) return rc;
-  if (need_x) {
-    switch (P) {
-      case 1: return launch_pgemm<1, MODE_DGRAD, 2>(tmA, tmB, prm, sms, stream);
-      case 2: return launch_pgemm<2, MODE_DGRAD, 2>(tmA, tmB, prm, sms, stream);
-      default: return launch_pgemm<3, MODE_DGRAD, 2>(tmA, tmB, prm, sms, stream);
-    }
-  }
   switch (P) {
-    case 1: return launch_pgemm<1, MODE_DGRAD, 1>(tmA, tmB, prm, sms, stream);
-    case 2: return launch_pgemm<2, MODE_DGRAD, 1>(tmA, tmB, prm, sms, stream);
-    default: return launch_pgemm<3, MODE_DGRAD, 1>(tmA, tmB, prm, sms, stream);
+    case 1: return launch_pgemm<1, MODE_DGRAD>(tmA, tmB, prm, sms, stream);
+    case 2: return launch_pgemm<2, MODE_DGRAD>(tmA, tmB, prm, sms, stream);
+    default: return launch_pgemm<3, MODE_DGRAD>(tmA, tmB, prm, sms, stream);
   }
 }
 
@@ -521,9 +487,9 @@ int cell_wgrad(const void* dgT_planes, const void* xhT_planes, float* dwp, long 
   int sms = 0;
   if ((rc = num_sms_of_device(&sms))) return rc;
   switch (P) {
-    case 1: return launch_pgemm<1, MODE_WGRAD, 1>(tmA, tmB, prm, sms, stream);
-    case 2: return launch_pgemm<2, MODE_WGRAD, 1>(tmA, tmB, prm, sms, stream);
-    default: return launch_pgemm<3, MODE_WGRAD, 1>(tmA, tmB, prm, sms, stream);
+    case 1: return launch_pgemm<1, MODE_WGRAD>(tmA, tmB, prm, sms, stream);
+    case 2: return launch_pgemm<2, MODE_WGRAD>(tmA, tmB, prm, sms, stream);
+    default: return launch_pgemm<3, MODE_WGRAD>(tmA, tmB, prm, sms, stream);
   }
 }
 
@@ -545,7 +511,7 @@ int cell_wgrad_mn(const void* dg_planes, const void* xh_planes, float* dwp, long
   {
     const uint64_t dims[4] = {32, (uint64_t)R, kGates / 32, (uint64_t)P};
     const uint64_t st[3] = {kGates * 2ull, 64, (uint64_t)R * kGates * 2};
-    const uint32_t box[4] = {32, G_BLOCK_K, 8, (uint32_t)P};      // MT = 2: 256 gate columns per CTA tile
+    const uint32_t box[4] = {32, G_BLOCK_K, 4, (uint32_t)P};      // 128 gate columns per CTA tile
     int rc = encode_tmap_4d_bf16(&tmA, dg_planes, dims, st, box, 64);
     if (rc) return rc;
   }
@@ -558,11 +524,11 @@ int cell_wgrad_mn(const void* dg_planes, const void* xh_planes, float* dwp, long
   }
   prm.out = dwp; prm.R = R; prm.H = H; prm.W = W; prm.cpad = cpad;
   const long long kb_total = (R + G_BLOCK_K - 1) / G_BLOCK_K;
-  // work items = 4 M tiles (256 gate columns) x unit groups x k-splits, sized to fill whole waves of 148 CTAs:
-  // cpad 288: 4 x 14 x 5 = 280 (1.9 waves); cpad 320: 4 x 18 x 2 = 144
+  // work items = 8 M tiles (128 gate columns) x unit groups x k-splits: cpad 288: 8 x 14 x 5 = 560; cpad 320:
+  // 8 x 18 x 2 = 288
   prm.ksplit = cell_wgrad_mn_slabs(cpad);
   prm.num_kb = (int)((kb_total + prm.ksplit - 1) / prm.ksplit);
-  prm.num_m_tiles = kGates / (2 * G_BLOCK_M);
+  prm.num_m_tiles = kGates / G_BLOCK_M;
   prm.num_n_tiles = ((prm.n_units + prm.upt - 1) / prm.upt) * prm.ksplit;
   prm.lbo = 32 * 64;   // bytes between 32-wide MN blocks ([32 K rows][64 B] each)
   prm.sbo = 8 * 64;    // bytes between groups of 8 K rows
@@ -570,9 +536,9 @@ int cell_wgrad_mn(const void* dg_planes, const void* xh_planes, float* dwp, long
   int rc = num_sms_of_device(&sms);
   if (rc) return rc;
   switch (P) {
-    case 1: return launch_pgemm<1, MODE_WGRAD_MN, 2>(tmA, tmB, prm, sms, stream);
-    case 2: return launch_pgemm<2, MODE_WGRAD_MN, 2>(tmA, tmB, prm, sms, stream);
-    default: return launch_pgemm<3, MODE_WGRAD_MN, 2>(tmA, tmB, prm, sms, stream);
+    case 1: return launch_pgemm<1, MODE_WGRAD_MN>(tmA, tmB, prm, sms, stream);
+    case 2: return launch_pgemm<2, MODE_WGRAD_MN>(tmA, tmB, prm, sms, stream);
+    default: return launch_pgemm<3, MODE_WGRAD_MN>(tmA, tmB, prm, sms, stream);
   }
 }
 

@@ -17,6 +17,7 @@ from __future__ import annotations
 import contextlib
 import os
 import types
+import weakref
 
 import numpy as np
 
@@ -39,8 +40,12 @@ class Variable(object):
     self.dtype = dtype
     self.trainable = trainable
     self.initializer_fn = initializer
-    self.owner = owner
+    self._owner = None if owner is None else weakref.ref(owner)     # the owning model holds its variables
     self.value = np.zeros(shape, dtype=dtype)
+
+  @property
+  def owner(self):
+    return None if self._owner is None else self._owner()
 
   def get_shape(self):
     return self.shape

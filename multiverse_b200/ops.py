@@ -370,7 +370,7 @@ def cell_wgrad(dgT, xhT, dw_packed, h, w, ns):
 
 
 def cell_wgrad_direct(dg_planes, xh, dw_packed, h, w, ns):
-  """wgrad straight from the row-major planes (MN-major tcgen05 operands, no transposes)."""
+  """wgrad straight from the row-major planes (MN-major wgmma operands, no transposes)."""
   _lib.call("mvb_cell_wgrad_direct", _p(dg_planes), _p(xh), _p(dw_packed), ns, h, w, xh.shape[2],
             xh.shape[0], _stream())
 

@@ -1,5 +1,5 @@
 # coding=utf-8
-"""The reference's `pred_models` call surface on top of the B200 engine.
+"""The reference's `pred_models` call surface on top of the H100 engine.
 
 Mirrors code/pred_models.py of JunweiLiang/Multiverse: `get_model` (:19), `Model` (:32) with the
 same placeholder / fetch attribute names, `get_feed_dict` (:1042-1194), `Trainer` (:1636) and
@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import os
 import sys
+import weakref
 
 import numpy as np
 
@@ -39,10 +40,17 @@ tf = _shim()
 
 
 class Handle(object):
-  """Placeholder or fetch handle owned by a Model (what `sess.run` receives)."""
+  """Placeholder or fetch handle owned by a Model (what `sess.run` receives).  The owner is held weakly: the model
+  holds its handles, and a strong back-reference would keep a dropped model - and the device memory of its engine -
+  alive until Python's cycle collector happens to run."""
 
   def __init__(self, owner, kind, name, index=None):
-    self.owner, self.kind, self.name, self.index = owner, kind, name, index
+    self._owner = weakref.ref(owner)
+    self.kind, self.name, self.index = kind, name, index
+
+  @property
+  def owner(self):
+    return self._owner()
 
   def __repr__(self):
     return "<%s %s%s>" % (self.kind, self.name, "" if self.index is None else "[%d]" % self.index)
@@ -127,7 +135,7 @@ class Model(object):
   def _var(self, name, shape, dtype="float32", init=None, trainable=True):
     fn = None
     if init is not None:
-      fn = lambda shp, init=init: init(tuple(shp), self._rng)
+      fn = lambda shp, init=init, rng=self._rng: init(tuple(shp), rng)     # no reference back to the model
     v = tf.Variable(name, shape, dtype=dtype, initializer=fn, trainable=trainable, owner=self)
     tf._GRAPH.add(v)
     self._own_vars.append(v)
@@ -429,9 +437,8 @@ class Model(object):
   def _pinned_block(self, shape, dtype, busy, keep=4):
     """A pinned host tensor for one fetch.  Blocks are kept per (shape, dtype) and handed out again once the numpy
     array that wrapped them (and every view of it) is gone (`busy`: ids of the blocks already handed out during
-    the current call, which have no array yet) - measured on the B200 box: a fresh 40 MB pinned
-    allocation per Session.run costs 33 ms of host time and ~8 ms of device time (64 trajectories, K=20), which
-    torch's own host allocator paid on every call here."""
+    the current call, which have no array yet): a fresh 40 MB pinned allocation per Session.run costs tens of ms of
+    host time, which torch's own host allocator would pay on every call here."""
     import torch
     use_count = getattr(torch._C, "_storage_Use_Count", None)
     if use_count is None:                   # no way to tell whether a block is still referenced: do not pool

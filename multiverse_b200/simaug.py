@@ -1,5 +1,5 @@
 # coding=utf-8
-"""SimAug's white-box attack on the scene input, on the B200 engine (SURVEY.md section 8 row f-4, first part).
+"""SimAug's white-box attack on the scene input, on the H100 engine (SURVEY.md section 8 row f-4, first part).
 
 Mirrors ``white_box_attack`` of ``SimAug/code/pred_models.py:60-170`` - same argument meaning, same config
 attributes (``adv_epsilon, adv_step_size, adv_num_iter, adv_start_from_clean_prob, adv_use_fgsm, use_mixup,

@@ -7,7 +7,7 @@ all-reduce of the flat fp32 gradient buffer (SURVEY.md §8e): sum, scale by 1/G 
 optimizer kernel, then clip, which reproduces the single-GPU batch semantics because every loss
 is a mean over equal shards.
 
-Per cell step the backward is  lstm_gates_bwd -> cell_dgrad (tcgen05) -> cell_wgrad_direct (tcgen05,
+Per cell step the backward is  lstm_gates_bwd -> cell_dgrad (wgmma) -> cell_wgrad_direct (wgmma,
 MN-major operands read straight from the stored planes);  around it: head_bwd, emb_bwd, gnn_bwd, enc_class_input_bwd, scene_*_bwd.
 """
 from __future__ import annotations

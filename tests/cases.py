@@ -7,6 +7,7 @@ oracle's fp64 outputs."""
 from __future__ import annotations
 
 import math
+import os
 
 import numpy as np
 
@@ -156,3 +157,47 @@ def grad_sample_stride(size):
 
 
 ADV_SAMPLE_STRIDE = 7      # every 7th element of the augmented features is stored in simaug_multiview.npz
+
+
+# ---- executions of the reference's own graph code (tests/golden/make_golden_refexec.py)
+# name -> (config overrides, seed)
+REFEXEC_FORWARD = {
+    "beam_k5_plain": ROLLOUTS["beam_k5_plain"],
+    "beam_k20_diverse": (dict(batch_size=3, use_grids=[False, True], use_beam_search=True, beam_size=20,
+                              diverse_beam=True, diverse_gamma=0.01, fix_num_timestep=1), 7),
+    "greedy_two_scale": (dict(batch_size=2, scene_h=24, scene_w=16), 8),
+    "no_gnn": (dict(batch_size=2, use_grids=[False, True], use_gnn=False), 9),
+}
+REFEXEC_TRAIN = (dict(batch_size=2, use_grids=[False, True], grid_loss_weight=1.0, grid_reg_loss_weight=0.1, wd=0.001),
+                 10, dict(grid_loss_weight=1.0, grid_reg_loss_weight=0.1, wd=0.001))
+SAMPLE_MAX = 4096
+
+
+def sample_stride(size):
+  """Stride of the strided samples of large arrays in the reference-execution goldens."""
+  return max(1, -(-size // SAMPLE_MAX))
+
+
+def sample(a):
+  """Every sample_stride-th element of the flattened array, fp64."""
+  flat = np.asarray(a, np.float64).reshape(-1)
+  return flat[::sample_stride(flat.size)]
+
+
+def attack_spec(mode, spec, cfg):
+  """SimAug white_box_attack case: (random target offsets, step size, iterations, mixup beta) of `mode`."""
+  rng = np.random.default_rng(3)
+  off = rng.integers(1, 18 * 9, size=(spec["n"], cfg.pred_len)).astype(np.int32)
+  return (off, spec["eps"], 1, None) if mode == "fgsm" else (off, 0.03, 3, 0.4)
+
+# drop-in Model.get_feed_dict against the reference's: the two model configurations (refexec_feed_dict_<i>.npz)
+FEED_CONFIGS = (dict(), dict(use_grids=[True, False]))
+
+
+def load_golden(path):
+  """tests/golden/<name>.npz as a dict, merged with <name>_zero.npz where a cell golden keeps its zero-state outputs
+  in a file of their own (every golden file stays under 1 MB)."""
+  g = dict(np.load(path + ".npz"))
+  if os.path.exists(path + "_zero.npz"):
+    g.update(np.load(path + "_zero.npz"))
+  return g

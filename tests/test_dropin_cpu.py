@@ -2,11 +2,9 @@
 """CPU tests of the drop-in boundary (host logic only - no kernel runs here).
 
 With multiverse_b200/dropin first on sys.path the reference's callers import OUR `pred_models`
-and the `tensorflow`-named shim.  When the reference tree is mounted (this container; it does not
-exist on the GPU box) its unchanged code/test.py flow and its own Model.get_feed_dict are run
-against ours."""
-import importlib
-import importlib.util
+and the `tensorflow`-named shim.  The reference's own Model.get_feed_dict (and SimAug's), executed on our Model
+(tests/golden/make_golden_refexec.py), is held against ours through the feed dicts it returned
+(tests/golden/refexec_feed_dict_*.npz)."""
 import os
 import sys
 import types
@@ -16,8 +14,35 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DROPIN = os.path.join(ROOT, "multiverse_b200", "dropin")
-REF = "/root/reference/code"
-have_ref = os.path.exists(os.path.join(REF, "pred_utils.py"))
+GOLD = os.path.join(ROOT, "tests", "golden")
+# the reference repository's code/ directory: only tests/golden/make_golden_refexec.py reads it
+REF = os.path.join(os.environ.get("MVB_REFERENCE_ROOT", "/root/reference"), "code")
+
+
+def handle_key(h):
+  return "%s/%s" % (h.name, "-" if h.index is None else h.index)
+
+
+def stored_feed(g, prefix, ours):
+  """The stored feed dict under `prefix`, keyed by the handles of `ours` (same placeholder name / index)."""
+  by_key = {handle_key(h): h for h in ours}
+  keys = [k[len(prefix):] for k in g.files if k.startswith(prefix)]
+  assert set(keys) <= set(by_key), sorted(set(keys) - set(by_key))
+  return {by_key[k]: g[prefix + k] for k in keys}
+
+
+def stored_batch(g, bi):
+  """batch.data and the grid centres of batch.shared as the reference's pred_utils produced them
+  (tests/golden/make_golden_refexec.py:feed_goldens)."""
+  data, shared = {}, {}
+  for k in g.files:
+    if k.startswith("batch%d/" % bi):
+      kind, name = k.split("/", 2)[1:]
+      if kind == "shared":
+        shared[name] = g[k]
+      else:
+        data[name] = list(g[k]) if kind == "list" else (g[k].item() if g[k].ndim == 0 else g[k])
+  return types.SimpleNamespace(data=data, shared=shared)
 
 
 def as_host(out, wanted):
@@ -128,29 +153,25 @@ def test_saver_relative_path_round_trip(dropin, tmp_path, monkeypatch):
   assert os.path.exists(st2.model_checkpoint_path + ".npz")
 
 
-@pytest.mark.skipif(not have_ref, reason="reference tree not mounted")
-def test_get_feed_dict_equals_the_references(dropin, tmp_path, monkeypatch):
-  """Our vectorised Model.get_feed_dict against the reference's own method
-  (code/pred_models.py:1042-1194) executed on our Model instance."""
+def test_get_feed_dict_equals_the_references(dropin, tmp_path):
+  """Our vectorised Model.get_feed_dict against the reference's own method (code/pred_models.py:1042-1194) executed on
+  our Model instance for batches read by the reference's pred_utils (stored: the batches and its feed dicts)."""
+  import cases
   tf, pm = dropin
-  from multiverse_b200 import synthetic
-  monkeypatch.syspath_prepend(REF)
-  spec = importlib.util.spec_from_file_location("ref_pred_models", os.path.join(REF, "pred_models.py"))
-  ref = importlib.util.module_from_spec(spec)
-  spec.loader.exec_module(ref)
-  import pred_utils
-  for kw in (dict(), dict(use_grids=[True, False])):
+  for ci, kw in enumerate(cases.FEED_CONFIGS):
     tf.reset_default_graph()
     args, cfg = make_args(tmp_path, **kw)
-    args.prepropath = str(tmp_path)
-    synthetic.write_npz(str(tmp_path / "data_test.npz"), cfg, 5, seed=3)
-    data = pred_utils.read_data(args, "test")
     model = pm.get_model(args, gpuid=0)
-    for is_train in (False, True):
-      for _, batch in data.get_batches(args.batch_size, full=True, shuffle=False):
-        theirs = ref.Model.get_feed_dict(model, batch, is_train=is_train)
+    g = np.load(os.path.join(GOLD, "refexec_feed_dict_%d.npz" % ci))
+    assert str(g["source"]) == "reference_exec"
+    batches = sorted({int(k.split("/")[0][5:]) for k in g.files if k.startswith("batch")})
+    assert len(batches) == 2                     # 5 trajectories in batches of 3
+    for bi in batches:
+      batch = stored_batch(g, bi)
+      for is_train in (False, True):
         args.device_grid_feeds = False           # the reference's feed dict, key for key
         ours = model.get_feed_dict(batch, is_train=is_train)
+        theirs = stored_feed(g, "feed%d_%d/" % (bi, is_train), ours)
         assert set(ours) == set(theirs)
         for k in theirs:
           a, b = np.asarray(ours[k]), np.asarray(theirs[k])
@@ -174,199 +195,6 @@ def test_get_feed_dict_equals_the_references(dropin, tmp_path, monkeypatch):
     # a batch whose dense targets do not come from its trajectories keeps the dense path
     batch.data["obs_grid_target_all_0"] = [a + 1.0 for a in batch.data["obs_grid_target_all_0"]]
     assert model.obs_traj not in model.get_feed_dict(batch, is_train=False)
-
-
-@pytest.mark.skipif(not have_ref, reason="reference tree not mounted")
-def test_reference_test_py_flow_runs_unchanged(dropin, tmp_path, monkeypatch, capsys):
-  """code/test.py (byte-identical) imported and driven end to end - argparse, process_args,
-  read_data, get_model, initialize(load) through our Saver, Tester, evaluate and the metric
-  print-out - with the device forward stubbed out (there is no GPU in this container)."""
-  tf, pm = dropin
-  from multiverse_b200 import synthetic
-  import multiverse_b200.pred_models as impl
-  monkeypatch.syspath_prepend(REF)
-  cfg = synthetic.make_config(batch_size=4, use_grids=[True, False])
-  prepro = tmp_path / "prepro"; prepro.mkdir()
-  synthetic.write_npz(str(prepro / "data_test.npz"), cfg, 6, seed=4)
-  argv = ["test.py", str(prepro), str(tmp_path / "out"), "modelname", "--runId", "0", "--load_best",
-          "--is_baseline" if False else "--use_scene_enc", "--use_gnn", "--scene_h", "72", "--scene_w", "36",
-          "--scene_grid_strides", "2,4", "--use_grids", "1,0", "--batch_size", "4", "--emb_size", "32",
-          "--scene_conv_dim", "64", "--scene_class", "11", "--activation_func", "tanh", "--obs_len", "8",
-          "--pred_len", "12", "--convlstm_kernel", "3", "--enc_hidden_size", "256", "--dec_hidden_size", "256"]
-  monkeypatch.setattr(sys, "argv", argv)
-  spec = importlib.util.spec_from_file_location("ref_test", os.path.join(REF, "test.py"))
-  ref_test = importlib.util.module_from_spec(spec)
-  spec.loader.exec_module(ref_test)
-  import pred_utils
-  args = ref_test.parser.parse_args()
-  args.is_train, args.is_test = False, True
-  args = pred_utils.process_args(args)
-  assert args.scene_grids == [(36, 18), (18, 9)]
-
-  # a "trained" checkpoint in the location test.py --load_best expects
-  model0 = pm.get_model(args, gpuid=0)
-  tf.global_variables_initializer().run()
-  tf.train.Saver().save(tf.Session(), args.save_dir_best_model, global_step=model0.global_step)
-  tf.reset_default_graph()
-
-  calls = []
-
-  def fake_forward(self, feed, wanted):
-    import torch
-    n, tp = self.N, self.config.pred_len
-    calls.append(feed)
-    out = dict(grid_pred_decoded=[], grid_pred_reg_decoded=[], beam_outputs=None)
-    for i, (h, w) in enumerate(self.config.scene_grids):
-      if not self.config.use_grids[i]:
-        out["grid_pred_decoded"].append([]); out["grid_pred_reg_decoded"].append([])
-      else:
-        out["grid_pred_decoded"].append(torch.zeros(n, tp, h, w, 1))
-        out["grid_pred_reg_decoded"].append(torch.zeros(n, tp, h, w, 2))
-    return as_host(out, wanted)
-
-  monkeypatch.setattr(impl.Model, "_engine_forward", fake_forward)
-  ref_test.main(args)
-  text = capsys.readouterr().out
-  assert "total test samples:6" in text and "grid0_traj_ade" in text
-  assert len(calls) == 2                                  # ceil(6 / 4) batches
-  assert calls[0][[k for k in calls[0] if getattr(k, "name", "") == "scene_feat"][0]].shape[1:] == (72, 36, 11)
-
-
-@pytest.mark.skipif(not have_ref, reason="reference tree not mounted")
-def test_reference_train_py_flow_runs_unchanged(dropin, tmp_path, monkeypatch, capsys):
-  """code/train.py (byte-identical): argparse -> process_args -> read_data -> get_model -> Trainer /
-  Tester -> the training loop with periodic save + evaluate, on our surface; the device work
-  (Model._train_step / _engine_forward) is stubbed because this container has no GPU."""
-  tf, pm = dropin
-  from multiverse_b200 import synthetic
-  import multiverse_b200.pred_models as impl
-  monkeypatch.syspath_prepend(REF)
-  cfg = synthetic.make_config(batch_size=4, use_grids=[True, False])
-  prepro = tmp_path / "prepro"; prepro.mkdir()
-  synthetic.write_npz(str(prepro / "data_train.npz"), cfg, 10, seed=5)
-  synthetic.write_npz(str(prepro / "data_val.npz"), cfg, 6, seed=6)
-  argv = ["train.py", str(prepro), str(tmp_path / "out"), "modelname", "--runId", "0", "--use_scene_enc", "--use_gnn",
-          "--scene_h", "72", "--scene_w", "36", "--scene_grid_strides", "2,4", "--use_grids", "1,0",
-          "--batch_size", "4", "--emb_size", "32", "--scene_conv_dim", "64", "--scene_class", "11",
-          "--activation_func", "tanh", "--obs_len", "8", "--pred_len", "12", "--train_w_onehot", "--wd", "0.001",
-          "--num_epochs", "2", "--save_period", "3", "--init_lr", "0.3", "--grid_reg_loss_weight", "0.2",
-          "--val_grid_num", "0"]
-  monkeypatch.setattr(sys, "argv", argv)
-  spec = importlib.util.spec_from_file_location("ref_train", os.path.join(REF, "train.py"))
-  ref_train = importlib.util.module_from_spec(spec)
-  spec.loader.exec_module(ref_train)
-  import pred_utils
-  args = ref_train.parser.parse_args()
-  args.is_train = True
-  args.is_test = False
-  args = pred_utils.process_args(args)
-  steps = []
-
-  def fake_train_step(self, feed, apply=True):
-    steps.append(int(self.global_step.value))
-    self.global_step.value = np.asarray(int(self.global_step.value) + 1, dtype="int32")
-    lr = self.learning_rate(steps[-1])
-    assert abs(lr - 0.3 * 0.95 ** (steps[-1] // int(10 / 4 * 2.0))) < 1e-12      # staircase decay, :1656-1665
-    return dict(loss=np.float32(1.0 / (1 + len(steps))), wd_loss=np.float32(0.1), train_op=None,
-                classification_loss={0: np.float32(0.5)}, regression_loss={0: np.float32(0.4)})
-
-  def fake_forward(self, feed, wanted):
-    import torch
-    n, tp = self.N, self.config.pred_len
-    out = dict(grid_pred_decoded=[], grid_pred_reg_decoded=[], beam_outputs=None)
-    for i, (h, w) in enumerate(self.config.scene_grids):
-      ok = self.config.use_grids[i]
-      out["grid_pred_decoded"].append(torch.zeros(n, tp, h, w, 1) if ok else [])
-      out["grid_pred_reg_decoded"].append(torch.zeros(n, tp, h, w, 2) if ok else [])
-    return as_host(out, wanted)
-
-  monkeypatch.setattr(impl.Model, "_train_step", fake_train_step)
-  monkeypatch.setattr(impl.Model, "_engine_forward", fake_forward)
-  ref_train.main(args)
-  text = capsys.readouterr().out
-  assert steps == list(range(6))                       # ceil(10/4) * 2 epochs
-  assert "best eval on val grid0_traj_ade" in text
-  ck = tf.train.get_checkpoint_state(args.save_dir)
-  assert ck is not None and os.path.exists(ck.model_checkpoint_path + ".npz")
-  assert tf.train.get_checkpoint_state(args.save_dir_best) is not None
-
-
-@pytest.mark.skipif(not have_ref, reason="reference tree not mounted")
-def test_reference_multifuture_inference_pieces_run_unchanged(dropin, tmp_path, monkeypatch):
-  """code/multifuture_inference.py (byte-identical): its PredictionModelInference subclass of OUR Model,
-  its Namespace config (:419-452), load_model_weights (:275-299) through our Saver, its own
-  get_feed_dict (:304-385) and the fetch list of :462-472 - the device forward is stubbed."""
-  tf, pm = dropin
-  from multiverse_b200 import synthetic
-  import multiverse_b200.pred_models as impl
-  import argparse
-  monkeypatch.syspath_prepend(REF)
-  monkeypatch.setattr(sys, "argv", ["multifuture_inference.py", "a", "b", "c", "d"])
-  spec = importlib.util.spec_from_file_location("ref_mfi", os.path.join(REF, "multifuture_inference.py"))
-  mfi = importlib.util.module_from_spec(spec)
-  spec.loader.exec_module(mfi)                      # __main__ guard: only definitions run
-  args = mfi.parser.parse_args(["traj", "mf", "model", "out.p", "--num_out", "20", "--diverse_beam",
-                                "--diverse_gamma", "0.01", "--fix_num_timestep", "1", "--use_gnn",
-                                "--use_scene_enc", "--emb_size", "32", "--scene_h", "72", "--scene_w", "36"])
-  mfi.add_grid(args)
-  assert args.scene_grids == [(36, 18), (18, 9)] and args.use_grids == [True, False]
-  args.use_beam_search = True
-  model_config = argparse.Namespace(
-      modelname="model", batch_size=1, beam_size=args.num_out, use_beam_search=args.use_beam_search,
-      diverse_beam=args.diverse_beam, diverse_gamma=args.diverse_gamma, fix_num_timestep=args.fix_num_timestep,
-      use_teacher_forcing=False, is_train=False, scene_h=args.scene_h, scene_w=args.scene_w,
-      scene_class=args.scene_class, use_soft_grid_class=args.use_soft_grid_class,
-      use_single_decoder=args.use_single_decoder, pred_len=12, emb_size=args.emb_size,
-      enc_hidden_size=args.enc_hidden_size, dec_hidden_size=args.dec_hidden_size, activation_func=tf.nn.tanh,
-      scene_conv_kernel=args.scene_conv_kernel, use_scene_enc=args.use_scene_enc,
-      scene_conv_dim=args.scene_conv_dim, convlstm_kernel=args.convlstm_kernel, use_gnn=args.use_gnn,
-      keep_prob=1.0, scene_grid_strides=args.scene_grid_strides, scene_grids=args.scene_grids,
-      use_grids=args.use_grids)
-  # a checkpoint of the same architecture, written through the shim Saver
-  cfg = synthetic.make_config(batch_size=1, use_grids=[True, False])
-  donor_args = types.SimpleNamespace(**vars(cfg)); donor_args.modelname = "donor"
-  donor_args.use_soft_grid_class = False
-  donor = pm.get_model(donor_args, gpuid=0)
-  tf.global_variables_initializer().run()
-  want = {k: v.copy() for k, v in donor.weights().items()}
-  tf.train.Saver().save(tf.Session(), str(tmp_path / "ckpt" / "save"), global_step=7)
-  tf.reset_default_graph()
-
-  with tf.Session() as sess:
-    with tf.device("/gpu:0"):
-      model = mfi.PredictionModelInference(model_config, model_config.modelname)
-    mfi.load_model_weights(str(tmp_path / "ckpt"), sess, top_scope="person_pred")
-    for k, v in model.weights().items():
-      assert np.array_equal(v, want[k]), k
-    # inputs in the layout get_inputs (:158-272) produces, for 2 trajectories with 12 / 17 future steps
-    f = synthetic.make_feeds(cfg, 2, 3)
-    inputs = dict(obs_grid_class=[np.stack([f["grid_obs_labels"][j][i] for j in range(2)]) for i in range(2)],
-                  obs_grid_target=[[f["grid_obs_regress"][j][i] for j in range(2)] for i in range(2)],
-                  obs_scene=[np.full((8, 1), i, dtype="int32") for i in range(2)],
-                  scene_feats=f["scene_feat"], max_pred_lengths=[12, 17])
-    seen = []
-
-    def fake_forward(self, feed, wanted):
-      import torch
-      tp = self._fed_pred_len(feed)
-      seen.append(tp)
-      h, w = self.config.scene_grids[0]
-      return as_host(dict(grid_pred_decoded=[torch.zeros(1, tp, h, w, 1), []],
-                          grid_pred_reg_decoded=[torch.zeros(1, tp, h, w, 2), []],
-                          beam_outputs=[torch.zeros(1, 20, tp, h * w), torch.zeros(1, 20, tp, dtype=torch.int32),
-                                        torch.zeros(1, 20)]), wanted)
-
-    monkeypatch.setattr(impl.Model, "_engine_forward", fake_forward)
-    for i in range(2):
-      feed_dict = model.get_feed_dict(inputs, args, i)
-      assert feed_dict[model.scene_feat].shape == (1, 72, 36, 11)
-      output_tensors = [model.grid_pred_decoded[0], model.grid_pred_reg_decoded[0], model.beam_outputs]
-      class_output, reg_output, beam_outputs = sess.run(output_tensors, feed_dict=feed_dict)
-      pred_len = inputs["max_pred_lengths"][i]
-      assert reg_output.reshape([1, pred_len, -1, 2]).shape[2] == 36 * 18      # :479
-      beam_logits, beam_grid_ids, beam_logprobs = beam_outputs
-      assert beam_grid_ids.shape == (1, 20, pred_len) and beam_logits.shape == (1, 20, pred_len, 648)
-    assert seen == [12, 17]          # the rollout length follows the FED pred_length, not config.pred_len
 
 
 def test_tf_checkpoint_bundle_reader(dropin, tmp_path):
@@ -581,6 +409,25 @@ def test_forward_graph_cache_policy_without_a_gpu(monkeypatch):
   assert not eng._graphs
 
 
+def test_dropped_model_is_freed_without_the_cycle_collector(dropin, tmp_path):
+  """A Model owns its engine's device buffers (tens of GB at benchmark sizes): dropping the last reference must free
+  it at once.  Its handles and variables point back at it only weakly, and their initializers not at all."""
+  import gc
+  import weakref
+  tf, pm = dropin
+  args, _ = make_args(tmp_path)
+  gc.disable()
+  try:
+    model = pm.get_model(args, gpuid=0)
+    assert model.scene_feat.owner is model and tf.global_variables()[-1].owner is model
+    ref = weakref.ref(model)
+    del model
+    tf.reset_default_graph()
+    assert ref() is None
+  finally:
+    gc.enable()
+
+
 def test_session_run_leaves_no_reference_cycle_on_the_results(monkeypatch):
   """The fetched arrays must die with the caller's last reference (their pinned blocks are reused then), not at
   the next cyclic-GC pass."""
@@ -611,22 +458,10 @@ def test_session_run_leaves_no_reference_cycle_on_the_results(monkeypatch):
     gc.enable()
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/SimAug/code/pred_models.py"), reason="reference tree not mounted")
-def test_multiview_feed_dict_equals_simaugs(dropin, tmp_path, monkeypatch):
-  """The extra-view feeds of a multiview_train batch (obs_scene_extra, grid_*_extra) against SimAug's own
-  Model.get_feed_dict (SimAug/code/pred_models.py:1457-1560) executed on our Model instance, key for key on every
-  placeholder that method fills."""
-  tf, pm = dropin
-  import types
-  monkeypatch.syspath_prepend(os.path.join(ROOT, "oracle", "tf1_eager"))
-  spec = importlib.util.spec_from_file_location("ref_simaug_pred_models", "/root/reference/SimAug/code/pred_models.py")
-  saved = sys.modules.get("tensorflow")
-  ref = importlib.util.module_from_spec(spec)
-  spec.loader.exec_module(ref)                    # binds `tf` to whatever `tensorflow` is importable: only numpy is used below
-  if saved is not None:
-    sys.modules["tensorflow"] = saved
-  tf.reset_default_graph()
+def multiview_case(pm, tmp_path):
+  """A drop-in Model in multiview_train mode (3 other camera views) and a seeded batch for it."""
   args, cfg = make_args(tmp_path, use_grids=[False, True])
+  args.batch_size = 2
   n, m = args.batch_size, 3
   args.is_train, args.multiview_train, args.multiview_max_num, args.multiview_exp = True, True, m, 1
   model = pm.get_model(args, gpuid=0)
@@ -650,8 +485,22 @@ def test_multiview_feed_dict_equals_simaugs(dropin, tmp_path, monkeypatch):
       ex["pred_grid_target_all_%d" % j] = [rng.standard_normal((t_pred, h, w, 2)).astype(np.float32) for _ in range(m)]
     data["extra"].append(ex)
   batch = types.SimpleNamespace(data=data)
-  theirs = ref.Model.get_feed_dict(model, batch, is_train=True)
+  return model, batch
+
+
+def test_multiview_feed_dict_equals_simaugs(dropin, tmp_path):
+  """The extra-view feeds of a multiview_train batch (obs_scene_extra, grid_*_extra) against SimAug's own
+  Model.get_feed_dict (SimAug/code/pred_models.py:1457-1560) executed on our Model instance (stored feed dict), key
+  for key on every placeholder that method fills."""
+  tf, pm = dropin
+  tf.reset_default_graph()
+  model, batch = multiview_case(pm, tmp_path)
+  args = model.config
+  ns = len(args.scene_grids)
+  g = np.load(os.path.join(GOLD, "refexec_feed_dict_simaug.npz"))
+  assert str(g["source"]) == "reference_exec"
   ours = model.get_feed_dict(batch, is_train=True)
+  theirs = stored_feed(g, "feed/", ours)
   assert set(theirs) <= set(ours)
   extra_keys = [model.obs_scene_extra] + [p for j in range(ns) if cfg_use(args, j) for p in
                                           (model.grid_obs_labels_extra[j], model.grid_pred_labels_T_extra[j],

@@ -22,7 +22,7 @@ TIGHT = 3e-5   # what the P=2 plane scheme actually delivers per kernel
 
 
 def gold(name):
-  return np.load(os.path.join(GOLD, name + ".npz"))
+  return cases.load_golden(os.path.join(GOLD, name))
 
 
 def rel(a, b):

@@ -1,10 +1,10 @@
 # coding=utf-8
 """SURVEY.md section 8 row f-4, the pin: SimAug's multi-view augmentation as EXECUTED FROM THE REFERENCE'S OWN FILE
-(unmodified /root/reference/SimAug/code/pred_models.py on the eager TF-1.15 stand-in, oracle/tf1_eager/run_simaug.py)
-against (a) the committed golden tests/golden/simaug_multiview.npz and (b) the same pipeline written on the oracle
-(oracle/multiverse_ref_torch.py: autograd input gradient, per-view losses, selection, mixup, mixed-label objective) -
-the expectation the GPU tests of multiverse_b200/simaug.py and TrainEngine's mixup path are held to.
-Skipped where /root/reference does not exist (the GPU box)."""
+(the unmodified SimAug/code/pred_models.py of the reference repository on the eager TF-1.15 stand-in,
+oracle/tf1_eager/run_simaug.py), stored in tests/golden/simaug_multiview.npz and tests/golden/refexec_attack.npz,
+against the same pipeline written on the oracle (oracle/multiverse_ref_torch.py: autograd input gradient, per-view
+losses, selection, mixup, mixed-label objective) - the expectation the GPU tests of multiverse_b200/simaug.py and
+TrainEngine's mixup path are held to."""
 import os
 import sys
 
@@ -17,10 +17,9 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import cases  # noqa: E402
 from oracle import multiverse_ref as R  # noqa: E402
 from oracle import multiverse_ref_torch as RT  # noqa: E402
-from oracle.tf1_eager import run_simaug as RS  # noqa: E402
 
-pytestmark = pytest.mark.skipif(not RS.available(), reason="needs /root/reference (not on the GPU box)")
 GOLD = os.path.join(ROOT, "tests", "golden", "simaug_multiview.npz")
+ATTACK = os.path.join(ROOT, "tests", "golden", "refexec_attack.npz")
 
 
 def oracle_pipeline(exp):
@@ -71,35 +70,29 @@ def oracle_pipeline(exp):
 
 @pytest.mark.parametrize("exp", [1, 4, 3])
 def test_reference_execution_matches_golden_and_oracle_pipeline(exp):
+  """The oracle's pipeline against the reference execution's augmented features (a strided fp32 sample), mixing
+  weight, losses and - experiment 3 - selected views, focal weights and every variable gradient (sampled)."""
   cfg, w, f, extra, spec = cases.simaug_case()
-  rcfg = R.default_config(**spec["config"])
-  ref = RS.multiview(rcfg, w, f, extra, spec["m"], exp, spec["eps"], spec["beta_draw"], with_trainer=(exp == 3),
-                     double_weighting=(exp == 3))
   g = np.load(GOLD)
   assert str(g["source"]).startswith("reference_exec")
-  samp = ref["adv_final"].reshape(-1)[::cases.ADV_SAMPLE_STRIDE]
-  assert np.abs(samp - g["exp%d_adv_final_sample" % exp]).max() < 1e-6
-  assert abs(ref["beta_weight"] - float(g["exp%d_beta" % exp])) < 1e-12
-  assert np.abs(np.array(ref["losses"]) - g["exp%d_losses" % exp]).max() < 1e-9
-  # ---- the oracle's pipeline
   o = oracle_pipeline(exp)
-  assert abs(o["beta"] - ref["beta_weight"]) < 1e-12
-  d = np.abs(o["adv_final"] - ref["adv_final"])
-  # both are fp64: the sign of an input-gradient entry that is ~0 is the only thing that may differ
-  assert (d <= 1e-9).mean() > 0.99999 and d.max() <= 2 * spec["eps"] + 1e-9
-  assert np.abs(np.array(o["losses"]) - np.array(ref["losses"])).max() < 1e-6 * max(ref["losses"])
+  assert abs(o["beta"] - float(g["exp%d_beta" % exp])) < 1e-12
+  d = np.abs(o["adv_final"].reshape(-1)[::cases.ADV_SAMPLE_STRIDE] - g["exp%d_adv_final_sample" % exp])
+  # fp64 both, stored as fp32: the sign of an input-gradient entry that is ~0 is the only thing that may differ
+  assert (d <= 1e-6).mean() > 0.9999 and d.max() <= 2 * spec["eps"] + 1e-6
+  ref_losses = g["exp%d_losses" % exp]
+  assert np.abs(np.array(o["losses"]) - ref_losses).max() < 1e-6 * ref_losses.max()
   if exp == 3:
-    assert np.array_equal(o["selected"], ref["selected_extra_indices"])
-    assert np.abs(o["focal"] - ref["focal_loss_weight"]).max() < 1e-9
+    assert np.array_equal(o["selected"], g["exp3_selected"])
+    assert np.abs(o["focal"] - g["exp3_focal"]).max() < 1e-9
     worst = 0.0
-    for k, gr in ref["grads"].items():
-      og = o["grads"][k]
-      scale = max(np.abs(gr).max(), 1e-30)
-      worst = max(worst, np.abs(og - gr).max() / scale)
-      samp_g = gr.reshape(-1)[::cases.grad_sample_stride(gr.size)]
-      assert np.abs(samp_g - g["exp3_grad_sample/" + k]).max() <= 1e-6 * scale + 1e-12, k
-    print("exp 3: oracle vs reference-exec gradients, worst relative error %.2e over %d variables" % (worst, len(ref["grads"])))
-    assert worst < 1e-6
+    for k, og in o["grads"].items():
+      scale = max(float(g["exp3_grad_norms/" + k][2]), 1e-30)          # max |gradient| of the reference run
+      samp = np.asarray(og, np.float64).reshape(-1)[::cases.grad_sample_stride(og.size)]
+      err = np.abs(samp - g["exp3_grad_sample/" + k]).max() / scale
+      worst = max(worst, err)
+      assert err <= 1e-6, k
+    print("exp 3: oracle vs reference-exec gradients, worst relative error %.2e over %d variables" % (worst, len(o["grads"])))
 
 
 @pytest.mark.parametrize("mode", ["fgsm", "pgd_mixup"])
@@ -110,14 +103,13 @@ def test_white_box_attack_reference_execution_matches_oracle_pipeline(mode):
   white_box_attack and mvb_adv_step / mvb_mix implement (GPU: test_simaug_scene_input_gradient_and_attack)."""
   cfg, w, f, extra, spec = cases.simaug_case()
   rcfg = R.default_config(**spec["config"])
-  n, eps, hw = spec["n"], spec["eps"], 18 * 9
-  rng = np.random.default_rng(3)
-  off = rng.integers(1, hw, size=(n, cfg.pred_len)).astype(np.int32)
-  fgsm = mode == "fgsm"
-  step, iters, beta = (eps, 1, None) if fgsm else (0.03, 3, 0.4)
-  ref = RS.adversarial(rcfg, w, f, eps, off, fgsm=fgsm, step_size=step, num_iter=iters, mixup_beta=beta)
+  n, eps = spec["n"], spec["eps"]
+  off, step, iters, beta = cases.attack_spec(mode, spec, cfg)
+  ref = np.load(ATTACK)
+  assert str(ref["source"]).startswith("reference_exec")
+  hw = 18 * 9
   target = (f["grid_pred_labels"][1].astype(np.int64) + off) % hw                       # create_random_target
-  assert np.array_equal(ref["target_label"], target) and not (target == f["grid_pred_labels"][1]).any()
+  assert np.array_equal(ref[mode + "/target_label"], target) and not (target == f["grid_pred_labels"][1]).any()
   # the oracle's pipeline: one private frame per (sample, step) row, like the reference's [N*T,SH,SW,SC] input
   t_obs = cfg.obs_len
   x = f["scene_feat"].astype(np.float64)[f["obs_scene"]].reshape((n * t_obs,) + f["scene_feat"].shape[1:])
@@ -125,13 +117,13 @@ def test_white_box_attack_reference_execution_matches_oracle_pipeline(mode):
   lo, hi = np.clip(x - eps, -1, 1), np.clip(x + eps, -1, 1)
   adv = x.copy()
   for _ in range(iters):
-    g = RT.scene_input_grad(rcfg, w, dict(rows, scene_feat=adv), target, 1)
-    adv = np.minimum(np.maximum(adv - step * np.sign(g), lo), hi)
+    gr = RT.scene_input_grad(rcfg, w, dict(rows, scene_feat=adv), target, 1)
+    adv = np.minimum(np.maximum(adv - step * np.sign(gr), lo), hi)
   if beta is not None:
     adv = x * beta + adv * (1 - beta)
-  d = np.abs(adv - ref["adv_final"])
-  print("white_box_attack %s: %.6f of the pixels equal, max diff %.3g" % (mode, (d <= 1e-9).mean(), d.max()))
+  d = np.abs(cases.sample(adv) - ref[mode + "/adv_final"])
+  print("white_box_attack %s: %.6f of the sampled pixels equal, max diff %.3g" % (mode, (d <= 1e-9).mean(), d.max()))
   assert (d <= 1e-9).mean() > 0.9999 and d.max() <= 2 * eps + 1e-9
   # and the training tower on the attacked features
-  _, losses, _, _ = RT.loss_and_grads(rcfg, w, dict(rows, scene_feat=ref["adv_final"]))
-  assert np.abs(np.array(losses) - np.array(ref["losses"])).max() < 1e-9 * max(ref["losses"])
+  _, losses, _, _ = RT.loss_and_grads(rcfg, w, dict(rows, scene_feat=adv))
+  assert np.abs(np.array(losses) - ref[mode + "/losses"]).max() < 1e-9 * ref[mode + "/losses"].max()

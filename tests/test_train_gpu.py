@@ -373,7 +373,7 @@ def test_simaug_scene_input_gradient_and_attack(dev):
 @pytest.mark.parametrize("exp", [1, 4, 3])
 def test_simaug_against_reference_execution(dev, exp):
   """Row f-4 against the reference itself: multiview_augmentation (and, for experiment 3, the label-mixed training
-  objective with focal weights and all its variable gradients) on the B200 vs tests/golden/simaug_multiview.npz, which
+  objective with focal weights and all its variable gradients) on the GPU vs tests/golden/simaug_multiview.npz, which
   holds what the UNMODIFIED SimAug/code/pred_models.py computes for the same seeded inputs when it is executed on the
   eager TF stand-in (tests/golden/make_golden_simaug.py; tests/test_simaug_reference_cpu.py re-runs it).  SimAug's
   model variant: the greedy decoder's graph attention sees h alone (gnn_scene_in_greedy=False)."""

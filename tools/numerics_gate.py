@@ -165,8 +165,12 @@ def main():
       row[scheme] = r
       print(name, scheme, json.dumps(r), flush=True)
     res[name] = row
-  with open(os.path.join(ROOT, "profiles", os.environ.get("GATE_OUT", "r02_numerics_gate.json")), "w") as fh:
-    json.dump(res, fh, indent=1)
+  out = sys.argv[1] if len(sys.argv) > 1 else None          # python tools/numerics_gate.py [RESULT.json]
+  if out:
+    with open(out, "w") as fh:
+      json.dump(res, fh, indent=1)
+  else:
+    print(json.dumps(res, indent=1))
 
 
 if __name__ == "__main__":
