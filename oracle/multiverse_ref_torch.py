@@ -8,7 +8,8 @@ unmodified reference graph code over the eager TF-1.15 stand-in of oracle/tf1_ea
 itself cannot run here, so "the reference's own CPU path" as a timed baseline is this restatement of
 code/pred_models.py with the same op decomposition TF uses
 (conv2d -> oneDNN convolution, dense [HW,HW] graph attention via batched matmul, full sort for
-the diverse-beam rank), running on all host threads.
+the diverse-beam rank), running on all host threads.  ``loss_and_grads`` also runs on a CUDA device (fp64, the
+convolutions as im2col matmuls): the truth of the at-size whole-model gradient test.
 """
 from __future__ import annotations
 
@@ -22,11 +23,17 @@ from . import multiverse_ref as R
 
 
 def conv2d_same(x, w, stride=1):
-  """tf.nn.conv2d(..., "SAME") on NHWC tensors / HWIO filters (code/pred_models.py:1363)."""
+  """tf.nn.conv2d(..., "SAME") on NHWC tensors / HWIO filters (code/pred_models.py:1363).  CUDA tensors go through
+  an im2col matmul: fp64 convolutions have no fast cuDNN algorithm, fp64 GEMMs run on the tensor cores."""
   n, h, wd, c = x.shape
   kh, kw = w.shape[0], w.shape[1]
-  _, pt, pb = R.same_pad(h, kh, stride)
-  _, pl, pr = R.same_pad(wd, kw, stride)
+  oh, pt, pb = R.same_pad(h, kh, stride)
+  ow, pl, pr = R.same_pad(wd, kw, stride)
+  if x.is_cuda:
+    p = F.pad(x, (0, 0, pl, pr, pt, pb))
+    cols = torch.cat([p[:, dy:dy + stride * (oh - 1) + 1:stride, dx:dx + stride * (ow - 1) + 1:stride]
+                      for dy in range(kh) for dx in range(kw)], -1)
+    return (cols.reshape(-1, kh * kw * c) @ w.reshape(kh * kw * c, -1)).reshape(n, oh, ow, -1)
   xn = F.pad(x.permute(0, 3, 1, 2), (pl, pr, pt, pb))
   y = F.conv2d(xn.contiguous(), w.permute(3, 2, 0, 1).contiguous(), stride=stride)
   return y.permute(0, 2, 3, 1)
@@ -40,9 +47,9 @@ def convlstm_cell(x, c, h, kernel, biases, forget_bias=1.0):
   return new_c, torch.tanh(new_c) * torch.sigmoid(go)
 
 
-def neighbour_mask(h, w, dtype=torch.float32):
-  eye = torch.eye(h * w, dtype=dtype).reshape(h * w, h, w, 1)
-  return conv2d_same(eye, torch.ones(3, 3, 1, 1, dtype=dtype)).reshape(h * w, h * w)
+def neighbour_mask(h, w, dtype=torch.float32, device=None):
+  eye = torch.eye(h * w, dtype=dtype, device=device).reshape(h * w, h, w, 1)
+  return conv2d_same(eye, torch.ones(3, 3, 1, 1, dtype=dtype, device=device)).reshape(h * w, h * w)
 
 
 def gnn_dense(hs, scene_mean, mask):
@@ -61,16 +68,17 @@ def grid_emb(x, W, b):
   return torch.tanh(conv2d_same(x, W) + b)
 
 
-def encoder(inputs, kernel, biases, ch):
+def encoder(inputs, kernel, biases, ch, device=None):
   n, t, h, w, _ = inputs.shape
-  c = torch.zeros(n, h, w, ch, dtype=inputs.dtype)
-  hs = torch.zeros(n, h, w, ch, dtype=inputs.dtype)
+  c = torch.zeros(n, h, w, ch, dtype=inputs.dtype, device=device)
+  hs = torch.zeros(n, h, w, ch, dtype=inputs.dtype, device=device)
   for s in range(t):
     c, hs = convlstm_cell(inputs[:, s], c, hs, kernel, biases)
   return c, hs
 
 
-def one_hot_map(ids, h, w, dtype=torch.float32):
+def one_hot_map(ids, h, w, dtype=torch.float32, device=None):
+  ids = ids if device is None else ids.to(device)
   return F.one_hot(ids.long(), h * w).to(dtype).reshape(-1, h, w, 1)
 
 
@@ -167,50 +175,56 @@ def scene_input_grad(cfg, weights, feeds, target_labels, scale_idx, dtype=torch.
   return sf.grad.numpy()
 
 
-def loss_and_grads(cfg, weights, feeds, dtype=torch.float64):
+def loss_and_grads(cfg, weights, feeds, dtype=torch.float64, device="cpu", return_logits=False):
   """Training objective of Model.build_loss (code/pred_models.py:961-1040) on the greedy
   train-mode forward (train_w_onehot: the class decoder is fed one_hot(argmax), :285) and its
   gradients w.r.t. every trainable variable by torch autograd - the truth for the hand-written
-  backward kernels.  Returns (total, [cls_0, reg_0, cls_1, ...], wd_loss, {name: grad})."""
-  w = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dtype).requires_grad_(True)
+  backward kernels.  Returns (total, [cls_0, reg_0, cls_1, ...], wd_loss, {name: grad}), computed on `device`
+  (gradients returned as numpy arrays); with return_logits, also the decoded class logits of every scale
+  (numpy [N, Tp, h, w, 1], an empty list for an unused scale) as a fifth element."""
+  w = {k: torch.from_numpy(np.ascontiguousarray(v)).to(device=device, dtype=dtype).requires_grad_(True)
        for k, v in weights.items()}
-  out = _forward(cfg, w, feeds, dtype)
+  out = _forward(cfg, w, feeds, dtype, device)
   losses = []
   n = cfg.batch_size
   for i, (h, ww) in enumerate(cfg.scene_grids):
     if not cfg.use_grids[i]:
       continue
     logits = out["grid_pred_decoded"][i].reshape(-1, h * ww)
-    labels = torch.from_numpy(feeds["grid_pred_labels"][i]).long().reshape(-1)
+    labels = torch.from_numpy(feeds["grid_pred_labels"][i]).to(device).long().reshape(-1)
     mixup = feeds.get("mixup")
     if mixup is None:
       cls = F.cross_entropy(logits, labels) * cfg.grid_loss_weight        # :991-995, :1024
     else:
       # SimAug multiview_exp 3 (SimAug/code/pred_models.py:1371-1405): softmax CE against the mixed labels, per-row
       # focal weights under double_weighting, then the mean
-      beta = torch.tensor(np.float32(mixup["beta"])).to(dtype)
-      l2 = torch.from_numpy(np.asarray(mixup["pred_labels2"][i])).long().reshape(-1)
+      beta = torch.tensor(np.float32(mixup["beta"])).to(device=device, dtype=dtype)
+      l2 = torch.from_numpy(np.asarray(mixup["pred_labels2"][i])).to(device).long().reshape(-1)
       soft = F.one_hot(labels, h * ww).to(dtype) * beta + F.one_hot(l2, h * ww).to(dtype) * (1 - beta)
       rows = -(soft * F.log_softmax(logits, dim=1)).sum(1)
       if mixup.get("focal") is not None:
-        fw = torch.from_numpy(np.asarray(mixup["focal"])).to(dtype)
+        fw = torch.from_numpy(np.asarray(mixup["focal"])).to(device=device, dtype=dtype)
         rows = rows * fw[:, None].expand(n, cfg.pred_len).reshape(-1)
       cls = rows.mean() * cfg.grid_loss_weight
-    tgt = torch.from_numpy(feeds["grid_pred_regress"][i]).to(dtype)
+    tgt = torch.from_numpy(feeds["grid_pred_regress"][i]).to(device=device, dtype=dtype)
     reg = F.huber_loss(out["grid_pred_reg_decoded"][i], tgt, delta=1.0) * cfg.grid_reg_loss_weight
     losses += [cls, reg]
   # wd_cost(".*/W", wd): wd * l2_loss(p) = wd * sum(p^2)/2 for variables whose name ends in /W
   wd = sum(cfg.wd * 0.5 * (v * v).sum() for k, v in w.items() if k.endswith("/W"))
   total = sum(losses) + wd
   total.backward()
-  grads = {k: (v.grad.numpy() if v.grad is not None else np.zeros(v.shape)) for k, v in w.items()}
+  grads = {k: (v.grad.cpu().numpy() if v.grad is not None else np.zeros(v.shape)) for k, v in w.items()}
+  if return_logits:
+    logits = [d.detach().cpu().numpy() if torch.is_tensor(d) else d for d in out["grid_pred_decoded"]]
+    return float(total), [float(l) for l in losses], float(wd), grads, logits
   return float(total), [float(l) for l in losses], float(wd), grads
 
 
-def _forward(cfg, w, feeds, dtype):
+def _forward(cfg, w, feeds, dtype, device=None):
   n = cfg.batch_size
   scene_feat = feeds["scene_feat"] if torch.is_tensor(feeds["scene_feat"]) else torch.from_numpy(feeds["scene_feat"]).to(dtype)
-  obs_scene = torch.from_numpy(feeds["obs_scene"]).long()
+  scene_feat = scene_feat if device is None else scene_feat.to(device)
+  obs_scene = torch.from_numpy(feeds["obs_scene"]).to(scene_feat.device).long()
   x = scene_feat[obs_scene.reshape(-1)]              # embedding_lookup, :148-152
   convs = []
   for i in range(len(cfg.scene_grid_strides)):
@@ -223,17 +237,17 @@ def _forward(cfg, w, feeds, dtype):
       out["grid_pred_decoded"].append([]); out["grid_pred_reg_decoded"].append([])
       continue
     sw = R.scale_weights(w, i)
-    labels = torch.from_numpy(feeds["grid_obs_labels"][i]).long()
+    labels = torch.from_numpy(feeds["grid_obs_labels"][i]).to(device).long()
     onehot = F.one_hot(labels, h * ww).to(dtype).reshape(n, -1, h, ww, 1)
     mixup = feeds.get("mixup")
     if mixup is not None:      # SimAug multiview_exp 3 (SimAug/code/pred_models.py:616-635): mixed observed class maps
-      beta = torch.tensor(np.float32(mixup["beta"])).to(dtype)
-      other = F.one_hot(torch.from_numpy(np.asarray(mixup["obs_labels2"][i])).long(), h * ww).to(dtype)
+      beta = torch.tensor(np.float32(mixup["beta"])).to(device=device, dtype=dtype)
+      other = F.one_hot(torch.from_numpy(np.asarray(mixup["obs_labels2"][i])).to(device).long(), h * ww).to(dtype)
       onehot = beta * onehot + other.reshape(n, -1, h, ww, 1) * (1 - beta)
-    obs_reg = torch.from_numpy(feeds["grid_obs_regress"][i]).to(dtype)
-    mask = neighbour_mask(h, ww, dtype)
-    enc = encoder(convs[i] * onehot, sw.enc_class[0], sw.enc_class[1], cfg.enc_hidden_size)
-    enc_r = encoder(obs_reg, sw.enc_reg[0], sw.enc_reg[1], cfg.enc_hidden_size)
+    obs_reg = torch.from_numpy(feeds["grid_obs_regress"][i]).to(device=device, dtype=dtype)
+    mask = neighbour_mask(h, ww, dtype, device)
+    enc = encoder(convs[i] * onehot, sw.enc_class[0], sw.enc_class[1], cfg.enc_hidden_size, device)
+    enc_r = encoder(obs_reg, sw.enc_reg[0], sw.enc_reg[1], cfg.enc_hidden_size, device)
     scene_mean = convs[i].mean(1)
     if cfg.use_beam_search:
       margins = []
