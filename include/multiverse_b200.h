@@ -192,12 +192,32 @@ int mvb_cell_wgrad_slabs(int cpad);
 int mvb_loss_fwd_bwd(const float* logits, const int32_t* labels, float* dlogits, int64_t rows, int V,
                      float cls_weight, const float* reg, const float* target, float* dreg,
                      int64_t nreg, float reg_weight, float* loss_out, void* stream);
+/* --use_soft_grid_class (:986-989): loss_out[0] += cls_weight * mean_rows softmax_cross_entropy_with_logits(
+ * labels[rows,V], logits[rows,V]) = sum_v y_v (logsumexp(l) - l_v);  dlogits = (sum(y) softmax(l) - y) * cls_weight
+ * / rows (the label maps need not sum to one). */
+int mvb_soft_ce_fwd_bwd(const float* logits, const float* labels, float* dlogits, int64_t rows, int V,
+                        float cls_weight, float* loss_out, void* stream);
+/* --mask_grid_regression (:999-1018): the foreground is the cells whose label is > 0 - of the dense maps
+ * soft_labels fp32 [rows,V], or (soft_labels NULL) the cell labels[r] of each row of int32 [rows] that lies in [0,V).
+ * mvb_fg_count: *fg_count += its size K (an fp64 scalar on the device, exact to 2^53; the caller zeroes it).
+ * mvb_masked_huber_fwd_bwd: loss_out[1] += reg_weight * sum_fg Huber_delta1(reg - target) / (2 K), both channels
+ * of every foreground cell of reg / target fp32 [rows,V,2]; dreg = its gradient, zero off the foreground.  K is read
+ * from *fg_count, so a micro-batch can be divided by the count of its whole batch (or, data parallel, by the
+ * all-reduced count over the number of ranks); K = 0 gives a zero loss and
+ * gradient (TF's div_no_nan).  No host synchronisation. */
+int mvb_fg_count(const float* soft_labels, const int32_t* labels, int64_t rows, int V, double* fg_count,
+                 void* stream);
+int mvb_masked_huber_fwd_bwd(const float* reg, const float* target, float* dreg, const float* soft_labels,
+                             const int32_t* labels, int64_t rows, int V, const double* fg_count, float reg_weight,
+                             float* loss_out, void* stream);
 /* ---- a13: backward of the heads / embedding / attention / scene CNN (tf.gradients :1698) ----
  * hidden2grid: dWo[3,3,256,Pout] += ..., dh[NS*S,256] (=|+=) conv3x3^T(dout[NS,HW,Pout], Wo). */
 int mvb_head_bwd(const float* h32, const float* dout, const float* Wo, int Pout, float* dWo,
                  float* dh, int accumulate_dh, int64_t NS, int H, int W, void* stream);
 /* grid_emb: dxh = gradient w.r.t. concat([x,h]) rows (x block = columns [0,E)); input is
- * one_hot(ids) (Pout=1) or the dense map in_map[NS,HW,2] (Pout=2, also yields d_in). */
+ * one_hot(ids) (Pout=1), the dense map in_map[NS,HW,1] (Pout=1, ids NULL: the logits fed back by the class decoder
+ * when training without --train_w_onehot) or in_map[NS,HW,2] (Pout=2); a dense input also yields d_in
+ * (accumulate_din: +=). */
 int mvb_emb_bwd(const float* dxh, int cpad, const int32_t* ids, const float* in_map, const float* We,
                 const float* be, int E, int Pout, float* dWe, float* dbe, float* d_in,
                 int accumulate_din, int64_t NS, int H, int W, void* stream);
@@ -263,6 +283,12 @@ int mvb_head_class_fwd(const float* h32, const float* Wo, float* logits_out, int
                        const float* We, const float* be, int E, void* xh_next,
                        int64_t plane_stride, int cpad, int64_t NS, int H, int W, int planes,
                        void* stream);
+/* Class head of the training-mode decoder without --train_w_onehot (:426-435): as mvb_head_class_fwd, but
+ * the x block receives tanh(conv3x3(logits, We[3,3,1,E]) + be) - the embedded logits map itself, not the one-hot
+ * of its arg-max.  planes 1-3 only (a training format). */
+int mvb_head_class_fwd_dense(const float* h32, const float* Wo, float* logits_out, int32_t* ids_out,
+                             const float* We, const float* be, int E, void* xh_next, int64_t plane_stride, int cpad,
+                             int64_t NS, int H, int W, int planes, void* stream);
 /* Regression head: off[s,HW,2] = conv3x3(h, Wo[3,3,256,2]);
  * if xh_next: x block <- planes of tanh(conv3x3(off, We[3,3,2,E]) + be). */
 int mvb_head_reg_fwd(const float* h32, const float* Wo, float* off_out, const float* We,

@@ -47,6 +47,9 @@ SIGNATURES = {
     "mvb_unpack_cell_wgrad": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "mvb_cell_wgrad_slabs": [_i],
     "mvb_loss_fwd_bwd": [_vp, _vp, _vp, _i64, _i, _f, _vp, _vp, _vp, _i64, _f, _vp, _vp],
+    "mvb_soft_ce_fwd_bwd": [_vp, _vp, _vp, _i64, _i, _f, _vp, _vp],
+    "mvb_fg_count": [_vp, _vp, _i64, _i, _vp, _vp],
+    "mvb_masked_huber_fwd_bwd": [_vp, _vp, _vp, _vp, _vp, _i64, _i, _vp, _f, _vp, _vp],
     "mvb_head_bwd": [_vp, _vp, _vp, _i, _vp, _vp, _i, _i64, _i, _i, _vp],
     "mvb_emb_bwd": [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i64, _i, _i, _vp],
     "mvb_gnn_attend_bwd": [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i64, _i, _i, _vp],
@@ -62,6 +65,7 @@ SIGNATURES = {
     "mvb_scene_time_mean": [_vp, _vp, _vp, _i64, _i, _i64, _vp],
     "mvb_gnn_attend_fwd": [_vp, _vp, _vp, _i, _vp, _i64, _i, _i, _i64, _i, _i, _i, _vp],
     "mvb_head_class_fwd": [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i64, _i, _i64, _i, _i, _i, _vp],
+    "mvb_head_class_fwd_dense": [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i64, _i, _i64, _i, _i, _i, _vp],
     "mvb_head_reg_fwd": [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i64, _i, _i64, _i, _i, _i, _vp],
     "mvb_emb_onehot_fwd": [_vp, _vp, _vp, _i, _vp, _i64, _i, _i64, _i, _i, _i, _vp],
     "mvb_emb_dense_fwd": [_vp, _vp, _vp, _i, _vp, _i64, _i, _i64, _i, _i, _i, _vp],

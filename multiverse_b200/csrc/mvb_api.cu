@@ -112,7 +112,7 @@ static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s)
 extern "C" {
 
 const char* mvb_last_error(void) { return get_error(); }
-int mvb_abi_version(void) { return 11; }
+int mvb_abi_version(void) { return 12; }
 int mvb_cell_last_variant(void) { return cell_last_variant(); }
 long long mvb_cell_variants_seen(int reset) { return (long long)cell_variants_seen(reset); }
 long long mvb_launch_count(void) { return g_launches; }
@@ -231,6 +231,19 @@ int mvb_loss_fwd_bwd(const float* logits, const int32_t* labels, float* dlogits,
   return loss_fwd_bwd(logits, labels, dlogits, rows, V, cls_weight, reg, target, dreg, nreg,
                       reg_weight, loss_out, S(stream));
 }
+int mvb_soft_ce_fwd_bwd(const float* logits, const float* labels, float* dlogits, int64_t rows, int V,
+                        float cls_weight, float* loss_out, void* stream) {
+  return soft_ce_fwd_bwd(logits, labels, dlogits, rows, V, cls_weight, loss_out, S(stream));
+}
+int mvb_fg_count(const float* soft_labels, const int32_t* labels, int64_t rows, int V, double* count, void* stream) {
+  return fg_count(soft_labels, labels, rows, V, count, S(stream));
+}
+int mvb_masked_huber_fwd_bwd(const float* reg, const float* target, float* dreg, const float* soft_labels,
+                             const int32_t* labels, int64_t rows, int V, const double* fg_count, float reg_weight,
+                             float* loss_out, void* stream) {
+  return masked_huber_fwd_bwd(reg, target, dreg, soft_labels, labels, rows, V, fg_count, reg_weight, loss_out,
+                              S(stream));
+}
 int mvb_head_bwd(const float* h32, const float* dout, const float* Wo, int Pout, float* dWo,
                  float* dh, int accumulate_dh, int64_t NS, int H, int W, void* stream) {
   return head_bwd(h32, dout, Wo, Pout, dWo, dh, accumulate_dh, NS, H, W, S(stream));
@@ -311,6 +324,12 @@ int mvb_head_class_fwd(const float* h32, const float* Wo, float* logits_out, int
                        void* stream) {
   return head_fwd(h32, Wo, 1, logits_out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, H,
                   W, planes, S(stream));
+}
+int mvb_head_class_fwd_dense(const float* h32, const float* Wo, float* logits_out, int32_t* ids_out,
+                             const float* We, const float* be, int E, void* xh_next, int64_t plane_stride, int cpad,
+                             int64_t NS, int H, int W, int planes, void* stream) {
+  return head_class_fwd_dense(h32, Wo, logits_out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, H, W,
+                              planes, S(stream));
 }
 int mvb_head_reg_fwd(const float* h32, const float* Wo, float* off_out, const float* We,
                      const float* be, int E, void* xh_next, int64_t plane_stride, int cpad,

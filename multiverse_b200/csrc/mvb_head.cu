@@ -10,7 +10,8 @@
 // kernel moves 4*HW*(256+P) bytes per sample row (HBM-bound).  The class head then does the
 // argmax (first index on ties, as tf.argmax) and writes the embedded one-hot - tanh(b) everywhere
 // except the <=9 cells around the arg-max - as the bf16 x-planes of the next cell step; the
-// regression head embeds its own dense 2-channel output the same way.
+// regression head embeds its own dense 2-channel output the same way.  The logits-fed variant of
+// the class head (training without --train_w_onehot, :426-435) embeds its dense logits map instead.
 #include "mvb_common.cuh"
 #include "mvb_kernels.h"
 
@@ -19,22 +20,22 @@ namespace mvb {
 constexpr int HEAD_THREADS = 256;
 
 // x block (channels [0,E)) of xh_next for one sample row.
-//   POUT == 1: input is one_hot(amax);  POUT == 2: input is the dense map `vals` [HW][2] in smem.
-template <int P, int POUT>
+//   ONEHOT: input is one_hot(amax) (POUT == 1);  else the dense map `vals` [HW][POUT] in smem.
+template <int P, int POUT, bool ONEHOT = (POUT == 1)>
 __device__ __forceinline__ void emb_write(const float* __restrict__ vals, int amax,
                                           const float* __restrict__ We, const float* __restrict__ be,
                                           int E, __nv_bfloat16* __restrict__ xh, long long plane_stride,
                                           int cpad, long long s, const Grid& g) {
   const int hw = g.H * g.W;
   const int groups = E / 8;
-  const int ay = (POUT == 1) ? amax / g.W : 0, ax = (POUT == 1) ? amax % g.W : 0;
+  const int ay = ONEHOT ? amax / g.W : 0, ax = ONEHOT ? amax % g.W : 0;
   for (int i = threadIdx.x; i < hw * groups; i += blockDim.x) {
     const int p = i / groups, e0 = (i % groups) * 8;
     const int y = p / g.W, x = p % g.W;
     float v[8];
 #pragma unroll
     for (int c = 0; c < 8; ++c) v[c] = __ldg(be + e0 + c);
-    if (POUT == 1) {
+    if (ONEHOT) {
       // out[p] = sum_tap onehot[p + off(tap)] * We[tap]  ->  non-zero iff amax - p is a tap offset
       const int dy = ay - y, dx = ax - x;
       if (dy >= -1 && dy <= 1 && dx >= -1 && dx <= 1) {
@@ -47,12 +48,13 @@ __device__ __forceinline__ void emb_write(const float* __restrict__ vals, int am
       for (int tap = 0; tap < 9; ++tap) {
         const int yy = y + tap / 3 - 1, xx = x + tap % 3 - 1;
         if (yy < 0 || yy >= g.H || xx < 0 || xx >= g.W) continue;
-        const float i0 = vals[(yy * g.W + xx) * 2], i1 = vals[(yy * g.W + xx) * 2 + 1];
+        float in[POUT];
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          v[c] = fmaf(i0, __ldg(We + (tap * 2 + 0) * E + e0 + c), v[c]);
-          v[c] = fmaf(i1, __ldg(We + (tap * 2 + 1) * E + e0 + c), v[c]);
-        }
+        for (int ci = 0; ci < POUT; ++ci) in[ci] = vals[(yy * g.W + xx) * POUT + ci];
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+#pragma unroll
+          for (int ci = 0; ci < POUT; ++ci) v[c] = fmaf(in[ci], __ldg(We + (tap * POUT + ci) * E + e0 + c), v[c]);
       }
     }
     if (P == kPlanesF16F8) {      // f16f8 operand format (mvb_common.cuh)
@@ -78,7 +80,8 @@ __device__ __forceinline__ void emb_write(const float* __restrict__ vals, int am
   }
 }
 
-template <int P, int POUT>
+// DENSE_FB (POUT == 1 only): the feedback embeds the logits map itself, not one_hot(argmax)
+template <int P, int POUT, bool DENSE_FB = false>
 __global__ void __launch_bounds__(HEAD_THREADS)
 head_kernel(const float* __restrict__ h32, const float* __restrict__ Wo, float* __restrict__ out,
             int* __restrict__ ids_out, const float* __restrict__ We, const float* __restrict__ be,
@@ -220,7 +223,7 @@ head_kernel(const float* __restrict__ h32, const float* __restrict__ Wo, float* 
     __syncthreads();
   }
   // phase 4: embedded feedback input of the next cell step
-  if (xh_next) emb_write<P, POUT>(o_s, amax, We, be, E, xh_next, plane_stride, cpad, s, g);
+  if (xh_next) emb_write<P, POUT, POUT == 1 && !DENSE_FB>(o_s, amax, We, be, E, xh_next, plane_stride, cpad, s, g);
 }
 
 template <int P>
@@ -243,7 +246,7 @@ emb_dense_kernel(const float* __restrict__ x, const float* __restrict__ We, cons
   emb_write<P, 2>(sm, 0, We, be, E, xh_next, plane_stride, cpad, s, g);
 }
 
-template <int P, int POUT>
+template <int P, int POUT, bool DENSE_FB = false>
 static int launch_head(const float* h32, const float* Wo, float* out, int* ids_out, const float* We,
                        const float* be, int E, void* xh_next, long long plane_stride, int cpad,
                        long long NS, const Grid& g, cudaStream_t stream) {
@@ -251,9 +254,9 @@ static int launch_head(const float* h32, const float* Wo, float* out, int* ids_o
   static SmemOptIn opt;
   if (smem > 48 * 1024) {
     MVB_REQUIRE(smem <= 227 * 1024, "head_fwd: grid %dx%d needs %zu B shared memory", g.H, g.W, smem);
-    MVB_CHECK_CUDA(smem_opt_in(opt, head_kernel<P, POUT>, smem));
+    MVB_CHECK_CUDA(smem_opt_in(opt, head_kernel<P, POUT, DENSE_FB>, smem));
   }
-  head_kernel<P, POUT><<<(unsigned)NS, HEAD_THREADS, smem, stream>>>(
+  head_kernel<P, POUT, DENSE_FB><<<(unsigned)NS, HEAD_THREADS, smem, stream>>>(
       h32, Wo, out, ids_out, We, be, E, reinterpret_cast<__nv_bfloat16*>(xh_next), plane_stride, cpad, g);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
@@ -276,6 +279,21 @@ int head_fwd(const float* h32, const float* Wo, int Pout, float* out, int* ids_o
   MVB_HEAD_CASE(kPlanesF16F8, 1) MVB_HEAD_CASE(kPlanesF16F8, 2)
 #undef MVB_HEAD_CASE
   return MVB_ERR_INVALID;
+}
+
+int head_class_fwd_dense(const float* h32, const float* Wo, float* out, int* ids_out, const float* We,
+                         const float* be, int E, void* xh_next, long long plane_stride, int cpad, long long NS,
+                         int H, int W, int P, cudaStream_t stream) {
+  MVB_REQUIRE(P >= 1 && P <= 3, "head_class_fwd_dense: planes P=%d (training formats only)", P);
+  MVB_REQUIRE(h32 && Wo && out && NS > 0, "head_class_fwd_dense: bad args");
+  if (xh_next) MVB_REQUIRE(We && be && E > 0 && E % 8 == 0 && E <= cpad - kHidden && cpad % 8 == 0,
+                           "head_class_fwd_dense: emb needs We/be and E (=%d) a multiple of 8 within the x block", E);
+  const Grid g = make_grid(H, W);
+  switch (P) {
+    case 1: return launch_head<1, 1, true>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream);
+    case 2: return launch_head<2, 1, true>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream);
+    default: return launch_head<3, 1, true>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream);
+  }
 }
 
 int emb_onehot_fwd(const int* ids, const float* We, const float* be, int E, void* xh_next,

@@ -51,6 +51,9 @@ int gnn_attend_fwd(const float* h32, const int* row_map, const float* scene_mean
 int head_fwd(const float* h32, const float* Wo, int Pout, float* out, int* ids_out, const float* We,
              const float* be, int E, void* xh_next, long long plane_stride, int cpad, long long NS,
              int H, int W, int P, cudaStream_t stream);
+int head_class_fwd_dense(const float* h32, const float* Wo, float* out, int* ids_out, const float* We,
+                         const float* be, int E, void* xh_next, long long plane_stride, int cpad, long long NS,
+                         int H, int W, int P, cudaStream_t stream);
 int emb_onehot_fwd(const int* ids, const float* We, const float* be, int E, void* xh_next,
                    long long plane_stride, int cpad, long long NS, int H, int W, int P,
                    cudaStream_t stream);
@@ -95,6 +98,12 @@ int cell_wgrad_mn_slabs(int cpad);
 int loss_fwd_bwd(const float* logits, const int* labels, float* dlogits, long long rows, int V,
                  float cls_scale, const float* reg, const float* target, float* dreg, long long nreg,
                  float reg_scale, float* loss_out, cudaStream_t stream);
+int soft_ce_fwd_bwd(const float* logits, const float* labels, float* dlogits, long long rows, int V, float cls_scale,
+                    float* loss_out, cudaStream_t stream);
+int fg_count(const float* soft, const int* labels, long long rows, int V, double* count, cudaStream_t stream);
+int masked_huber_fwd_bwd(const float* reg, const float* target, float* dreg, const float* soft, const int* labels,
+                         long long rows, int V, const double* count, float reg_scale, float* loss_out,
+                         cudaStream_t stream);
 int head_bwd(const float* h32, const float* dout, const float* Wo, int Pout, float* dWo, float* dh,
              int accumulate_dh, long long NS, int H, int W, cudaStream_t stream);
 int emb_bwd(const float* dxh, int cpad, const int* ids, const float* in_map, const float* We,

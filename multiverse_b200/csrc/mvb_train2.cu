@@ -1,6 +1,9 @@
 // Backward kernels of everything around the cell (all HBM- or latency-bound, fp32):
 //   loss_fwd_bwd        Model.build_loss (code/pred_models.py:961-1040): sparse softmax CE (mean over
 //                       N*Tp) and Huber(delta=1) (mean over N*Tp*HW*2), values + gradients
+//   soft_ce_fwd_bwd     the --use_soft_grid_class CE (:986-989) against dense label maps
+//   fg_count, masked_huber_fwd_bwd
+//                       the --mask_grid_regression Huber (:999-1018): over the cells whose label is > 0 only
 //   head_bwd            hidden2grid (:925-959): dWo, dh
 //   emb_onehot_bwd      grid_emb on a one-hot input (:442-446): dWe, dbe (no input gradient)
 //   emb_dense_bwd       grid_emb on the 2-channel offset map: dWe, dbe, d(input)
@@ -71,6 +74,90 @@ huber_loss_kernel(const float* __restrict__ pred, const float* __restrict__ targ
     const float a = fabsf(e);
     acc += (a <= 1.f) ? 0.5f * e * e : a - 0.5f;
     dpred[i] = fminf(fmaxf(e, -1.f), 1.f) * scale;
+  }
+  acc = block_sum_256(acc, red);
+  if (threadIdx.x == 0) atomicAdd(loss_sum, acc * scale);
+}
+
+// one CTA per (n,t) row: softmax_cross_entropy_with_logits against a dense label row y[V]:
+//   loss = sum_v y_v (lse - l_v),  grad = (sum(y) softmax - y) * scale
+// (the soft maps of :1085-1136 do not sum to one, and lose mass where the kernel is clipped at the border)
+__global__ void __launch_bounds__(256)
+soft_ce_loss_kernel(const float* __restrict__ logits, const float* __restrict__ labels,
+                    float* __restrict__ dlogits, float* __restrict__ loss_sum, int V, float scale) {
+  __shared__ float red[8];
+  __shared__ float bc[3];
+  const long long r = blockIdx.x;
+  const float* lg = logits + r * V;
+  const float* y = labels + r * V;
+  float m = -INFINITY;
+  for (int v = threadIdx.x; v < V; v += blockDim.x) m = fmaxf(m, lg[v]);
+  m = warp_max(m);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) { float t = red[0]; for (int i = 1; i < 8; ++i) t = fmaxf(t, red[i]); bc[0] = t; }
+  __syncthreads();
+  m = bc[0];
+  float s = 0.f;
+  for (int v = threadIdx.x; v < V; v += blockDim.x) s += expf(lg[v] - m);
+  s = block_sum_256(s, red);
+  if (threadIdx.x == 0) bc[1] = s;
+  __syncthreads();
+  s = bc[1];
+  const float lse = logf(s) + m;
+  float sy = 0.f, l = 0.f;
+  for (int v = threadIdx.x; v < V; v += blockDim.x) {
+    const float yv = y[v];
+    sy += yv;
+    l = fmaf(yv, lse - lg[v], l);
+  }
+  sy = block_sum_256(sy, red);
+  if (threadIdx.x == 0) bc[2] = sy;
+  l = block_sum_256(l, red);
+  __syncthreads();
+  sy = bc[2];
+  const float inv = 1.0f / s;
+  for (int v = threadIdx.x; v < V; v += blockDim.x)
+    dlogits[r * V + v] = (sy * (expf(lg[v] - m) * inv) - y[v]) * scale;
+  if (threadIdx.x == 0) atomicAdd(loss_sum, l * scale);
+}
+
+// foreground of the masked regression loss: cells with label > 0 (dense maps) or the label cell of each row
+// (tf.one_hot of an in-range sparse label); count += their number
+__global__ void __launch_bounds__(256)
+fg_count_kernel(const float* __restrict__ soft, const int* __restrict__ labels, long long rows, int V,
+                double* __restrict__ count) {
+  const long long n = soft ? rows * V : rows;
+  unsigned c = 0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    c += soft ? (soft[i] > 0.f) : (labels[i] >= 0 && labels[i] < V);
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, (double)c);       // integers: exact up to 2^53
+}
+
+// Huber(delta=1) over the foreground cells only (tf.where + tf.gather, Reduction.MEAN over the 2K gathered
+// elements, div_no_nan: 0 when K = 0); dpred = 0 off the foreground.  K is read from the device: the count
+// of the whole batch, which a micro-batch may be only a part of.
+__global__ void __launch_bounds__(256)
+masked_huber_kernel(const float2* __restrict__ pred, const float2* __restrict__ target, float2* __restrict__ dpred,
+                    const float* __restrict__ soft, const int* __restrict__ labels,
+                    const double* __restrict__ fg_count, float* __restrict__ loss_sum, long long cells,
+                    int V, float weight) {
+  __shared__ float red[8];
+  const double K = *fg_count;
+  const float scale = K > 0.0 ? (float)(weight / (2.0 * K)) : 0.f;
+  float acc = 0.f;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < cells;
+       i += (long long)gridDim.x * blockDim.x) {
+    const bool fg = soft ? soft[i] > 0.f : labels[i / V] == (int)(i % V);
+    float2 d = make_float2(0.f, 0.f);
+    if (fg) {
+      const float2 p = pred[i], t = target[i];
+      const float e0 = p.x - t.x, e1 = p.y - t.y, a0 = fabsf(e0), a1 = fabsf(e1);
+      acc += ((a0 <= 1.f) ? 0.5f * e0 * e0 : a0 - 0.5f) + ((a1 <= 1.f) ? 0.5f * e1 * e1 : a1 - 0.5f);
+      d = make_float2(fminf(fmaxf(e0, -1.f), 1.f) * scale, fminf(fmaxf(e1, -1.f), 1.f) * scale);
+    }
+    dpred[i] = d;
   }
   acc = block_sum_256(acc, red);
   if (threadIdx.x == 0) atomicAdd(loss_sum, acc * scale);
@@ -152,8 +239,9 @@ head_bwd_kernel(const float* __restrict__ h32, const float* __restrict__ dout,
 
 // ------------------------------------------------------------------------------ emb backward
 // x = tanh(pre), pre = be + conv3x3(in, We);  dpre = dx * (1 - x^2)
-// one CTA per sample row.  POUT == 1: in = one_hot(id);  POUT == 2: in = dense [HW][2] map.
-template <int POUT>
+// one CTA per sample row.  ONEHOT (POUT == 1): in = one_hot(id);  else in = dense [HW][POUT] map (POUT = 1: the
+// class decoder's logits feedback, 2: the offset map).
+template <int POUT, bool ONEHOT = (POUT == 1)>
 __global__ void __launch_bounds__(256)
 emb_bwd_kernel(const float* __restrict__ dxh, int cpad, const int* __restrict__ ids,
                const float* __restrict__ in_map, const float* __restrict__ We,
@@ -161,15 +249,15 @@ emb_bwd_kernel(const float* __restrict__ dxh, int cpad, const int* __restrict__ 
                float* __restrict__ d_in, int accumulate_din, Grid g) {
   extern __shared__ float sm[];
   const int hw = g.H * g.W;
-  float* in_s = sm;                      // [HW][2] (POUT == 2)
+  float* in_s = sm;                      // [HW][POUT] (dense input)
   float* dpre_s = in_s + hw * 2;         // [HW][E]
   float* accw = dpre_s + hw * E;         // [9][POUT][E]
   float* accb = accw + 9 * POUT * E;     // [E]
   const long long s = blockIdx.x;
-  const int amax = (POUT == 1) ? ids[s] : 0;
+  const int amax = ONEHOT ? ids[s] : 0;
   const int ay = amax / g.W, ax = amax % g.W;
-  if (POUT == 2)
-    for (int i = threadIdx.x; i < hw * 2; i += blockDim.x) in_s[i] = in_map[s * hw * 2 + i];
+  if (!ONEHOT)
+    for (int i = threadIdx.x; i < hw * POUT; i += blockDim.x) in_s[i] = in_map[s * hw * POUT + i];
   for (int i = threadIdx.x; i < 9 * POUT * E + E; i += blockDim.x) accw[i] = 0.f;
   __syncthreads();
   // pass 1: dpre for every (pixel, e)
@@ -177,7 +265,7 @@ emb_bwd_kernel(const float* __restrict__ dxh, int cpad, const int* __restrict__ 
     const int p = i / E, e = i % E;
     const int y = p / g.W, x = p % g.W;
     float pre = be[e];
-    if (POUT == 1) {
+    if (ONEHOT) {
       const int dy = ay - y, dx = ax - x;
       if (dy >= -1 && dy <= 1 && dx >= -1 && dx <= 1) pre += We[((dy + 1) * 3 + (dx + 1)) * E + e];
     } else {
@@ -185,8 +273,8 @@ emb_bwd_kernel(const float* __restrict__ dxh, int cpad, const int* __restrict__ 
       for (int t = 0; t < 9; ++t) {
         const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
         if (yy < 0 || yy >= g.H || xx < 0 || xx >= g.W) continue;
-        pre = fmaf(in_s[(yy * g.W + xx) * 2], We[(t * 2 + 0) * E + e], pre);
-        pre = fmaf(in_s[(yy * g.W + xx) * 2 + 1], We[(t * 2 + 1) * E + e], pre);
+#pragma unroll
+        for (int ci = 0; ci < POUT; ++ci) pre = fmaf(in_s[(yy * g.W + xx) * POUT + ci], We[(t * POUT + ci) * E + e], pre);
       }
     }
     const float xv = tanhf(pre);
@@ -203,7 +291,7 @@ emb_bwd_kernel(const float* __restrict__ dxh, int cpad, const int* __restrict__ 
   for (int i = threadIdx.x; i < 9 * POUT * E; i += blockDim.x) {
     const int e = i % E, po = (i / E) % POUT, t = i / (E * POUT);
     float a = 0.f;
-    if (POUT == 1) {
+    if (ONEHOT) {
       // out[p] += onehot[p + off(t)] * We[t]  ->  only p = amax - off(t)
       const int y = ay - (t / 3 - 1), x = ax - (t % 3 - 1);
       if (y >= 0 && y < g.H && x >= 0 && x < g.W) a = dpre_s[(y * g.W + x) * E + e];
@@ -211,14 +299,14 @@ emb_bwd_kernel(const float* __restrict__ dxh, int cpad, const int* __restrict__ 
       for (int p = 0; p < hw; ++p) {
         const int yy = p / g.W + t / 3 - 1, xx = p % g.W + t % 3 - 1;
         if (yy < 0 || yy >= g.H || xx < 0 || xx >= g.W) continue;
-        a = fmaf(in_s[(yy * g.W + xx) * 2 + po], dpre_s[p * E + e], a);
+        a = fmaf(in_s[(yy * g.W + xx) * POUT + po], dpre_s[p * E + e], a);
       }
     }
     atomicAdd(dWe + (t * POUT + po) * E + e, a);
   }
-  if (POUT == 2 && d_in) {
-    for (int i = threadIdx.x; i < hw * 2; i += blockDim.x) {
-      const int q = i / 2, po = i % 2;
+  if (!ONEHOT && d_in) {
+    for (int i = threadIdx.x; i < hw * POUT; i += blockDim.x) {
+      const int q = i / POUT, po = i % POUT;
       const int y = q / g.W, x = q % g.W;
       float a = 0.f;
 #pragma unroll
@@ -226,10 +314,10 @@ emb_bwd_kernel(const float* __restrict__ dxh, int cpad, const int* __restrict__ 
         const int py = y - (t / 3 - 1), px = x - (t % 3 - 1);   // out[p] uses in[p + off] -> p = q - off
         if (py < 0 || py >= g.H || px < 0 || px >= g.W) continue;
         const float* dp = dpre_s + (py * g.W + px) * E;
-        const float* wv = We + (t * 2 + po) * E;
+        const float* wv = We + (t * POUT + po) * E;
         for (int e = 0; e < E; ++e) a = fmaf(dp[e], wv[e], a);
       }
-      const long long o = s * hw * 2 + i;
+      const long long o = s * hw * POUT + i;
       d_in[o] = accumulate_din ? d_in[o] + a : a;
     }
   }
@@ -565,6 +653,39 @@ int loss_fwd_bwd(const float* logits, const int* labels, float* dlogits, long lo
   return MVB_OK;
 }
 
+int soft_ce_fwd_bwd(const float* logits, const float* labels, float* dlogits, long long rows, int V, float cls_scale,
+                    float* loss_out, cudaStream_t stream) {
+  MVB_REQUIRE(logits && labels && dlogits && loss_out && rows > 0 && V > 0, "soft_ce_fwd_bwd: bad args");
+  soft_ce_loss_kernel<<<(unsigned)rows, 256, 0, stream>>>(logits, labels, dlogits, loss_out, V, cls_scale / (float)rows);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
+int fg_count(const float* soft, const int* labels, long long rows, int V, double* count, cudaStream_t stream) {
+  MVB_REQUIRE((soft || labels) && count && rows > 0 && V > 0, "fg_count: bad args");
+  fg_count_kernel<<<grid_for(soft ? rows * V : rows, 256), 256, 0, stream>>>(
+      soft, soft ? nullptr : labels, rows, V, count);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
+int masked_huber_fwd_bwd(const float* reg, const float* target, float* dreg, const float* soft, const int* labels,
+                         long long rows, int V, const double* count, float reg_scale, float* loss_out,
+                         cudaStream_t stream) {
+  MVB_REQUIRE(reg && target && dreg && (soft || labels) && count && loss_out && rows > 0 && V > 0,
+              "masked_huber_fwd_bwd: bad args");
+  const long long cells = rows * V;
+  masked_huber_kernel<<<grid_for(cells, 256), 256, 0, stream>>>(
+      reinterpret_cast<const float2*>(reg), reinterpret_cast<const float2*>(target), reinterpret_cast<float2*>(dreg),
+      soft, soft ? nullptr : labels, count, loss_out + 1, cells, V,
+      reg_scale);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
 int head_bwd(const float* h32, const float* dout, const float* Wo, int Pout, float* dWo, float* dh,
              int accumulate_dh, long long NS, int H, int W, cudaStream_t stream) {
   MVB_REQUIRE(h32 && dout && Wo && dWo && dh && NS > 0 && (Pout == 1 || Pout == 2), "head_bwd: bad args");
@@ -587,14 +708,17 @@ int emb_bwd(const float* dxh, int cpad, const int* ids, const float* in_map, con
             const float* be, int E, int Pout, float* dWe, float* dbe, float* d_in, int accumulate_din,
             long long NS, int H, int W, cudaStream_t stream) {
   MVB_REQUIRE(dxh && We && be && dWe && dbe && NS > 0 && E > 0, "emb_bwd: bad args");
-  MVB_REQUIRE((Pout == 1 && ids) || (Pout == 2 && in_map), "emb_bwd: need ids (Pout=1) or in_map (Pout=2)");
+  MVB_REQUIRE((Pout == 1 && (ids || in_map)) || (Pout == 2 && in_map),
+              "emb_bwd: need ids or in_map (Pout=1) or in_map (Pout=2)");
   const Grid g = make_grid(H, W);
   const size_t smem = sizeof(float) * ((size_t)H * W * (2 + E) + 9 * Pout * E + E);
-  static SmemOptIn opt1, opt2;
+  static SmemOptIn opt1, opt1d, opt2;
   MVB_CHECK_CUDA(smem_opt_in(opt1, emb_bwd_kernel<1>, 160 * 1024));
+  MVB_CHECK_CUDA(smem_opt_in(opt1d, emb_bwd_kernel<1, false>, 160 * 1024));
   MVB_CHECK_CUDA(smem_opt_in(opt2, emb_bwd_kernel<2>, 160 * 1024));
   MVB_REQUIRE(smem <= 160 * 1024, "emb_bwd: grid too large");
-  if (Pout == 1) emb_bwd_kernel<1><<<(unsigned)NS, 256, smem, stream>>>(dxh, cpad, ids, in_map, We, be, E, dWe, dbe, d_in, accumulate_din, g);
+  if (Pout == 1 && ids) emb_bwd_kernel<1><<<(unsigned)NS, 256, smem, stream>>>(dxh, cpad, ids, in_map, We, be, E, dWe, dbe, d_in, accumulate_din, g);
+  else if (Pout == 1) emb_bwd_kernel<1, false><<<(unsigned)NS, 256, smem, stream>>>(dxh, cpad, ids, in_map, We, be, E, dWe, dbe, d_in, accumulate_din, g);
   else emb_bwd_kernel<2><<<(unsigned)NS, 256, smem, stream>>>(dxh, cpad, ids, in_map, We, be, E, dWe, dbe, d_in, accumulate_din, g);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);

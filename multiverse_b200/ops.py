@@ -290,6 +290,17 @@ def head_class_fwd(h32, Wo, logits_out, ids_out, We, be, xh_next, h, w, ns, plan
             _p(xh_next), stride, cpad, ns, h, w, planes, _stream())
 
 
+def head_class_fwd_dense(h32, Wo, logits_out, ids_out, We, be, xh_next, h, w, ns, planes=None):
+  """head_class_fwd whose feedback embeds the logits map itself (training without --train_w_onehot)."""
+  e = 0 if We is None else We.shape[3]
+  if xh_next is not None:
+    stride, cpad, planes = xh_next.stride(0), xh_next.shape[2], planes_of(xh_next)
+  else:
+    stride, cpad, planes = 0, 0, planes or DEFAULT_PLANES
+  _lib.call("mvb_head_class_fwd_dense", _p(h32), _p(Wo), _p(logits_out), _p(ids_out), _p(We), _p(be), e,
+            _p(xh_next), stride, cpad, ns, h, w, planes, _stream())
+
+
 def head_reg_fwd(h32, Wo, off_out, We, be, xh_next, h, w, ns, planes=None):
   e = 0 if We is None else We.shape[3]
   if xh_next is not None:
@@ -391,6 +402,33 @@ def loss_fwd_bwd(logits, labels, dlogits, cls_weight, reg, target, dreg, reg_wei
   nreg = reg.numel() if reg is not None else 0
   _lib.call("mvb_loss_fwd_bwd", _p(logits), _p(labels), _p(dlogits), rows, v, float(cls_weight),
             _p(reg), _p(target), _p(dreg), nreg, float(reg_weight), _p(loss_out), _stream())
+
+
+def soft_ce_fwd_bwd(logits, labels, dlogits, cls_weight, loss_out):
+  """loss_out[0] += weighted mean soft-label CE of logits fp32 [..., V] against labels fp32 [..., V]; dlogits written."""
+  v = logits.shape[-1]
+  assert labels.dtype == torch.float32 and labels.numel() == logits.numel()
+  _lib.call("mvb_soft_ce_fwd_bwd", _p(logits), _p(labels), _p(dlogits), logits.numel() // v, v, float(cls_weight),
+            _p(loss_out), _stream())
+
+
+def fg_count(labels, v, count):
+  """count fp64 [1] += number of foreground cells of labels: fp32 maps [..., V] (> 0) or int32 cells [...]."""
+  soft = labels.dtype == torch.float32
+  rows = labels.numel() // v if soft else labels.numel()
+  _lib.call("mvb_fg_count", _p(labels) if soft else None, None if soft else _p(labels), rows, v, _p(count),
+            _stream())
+
+
+def masked_huber_fwd_bwd(reg, target, dreg, labels, count, reg_weight, loss_out):
+  """loss_out[1] += reg_weight * Huber over the foreground cells of `labels` (as fg_count) / (2 * count[0]);
+  reg / target / dreg fp32 [..., V, 2]."""
+  v = reg.shape[-2]
+  soft = labels.dtype == torch.float32
+  rows = reg.numel() // (2 * v)
+  assert count.dtype == torch.float64 and (labels.numel() == rows * v if soft else labels.numel() == rows)
+  _lib.call("mvb_masked_huber_fwd_bwd", _p(reg), _p(target), _p(dreg), _p(labels) if soft else None,
+            None if soft else _p(labels), rows, v, _p(count), float(reg_weight), _p(loss_out), _stream())
 
 
 def head_bwd(h32, dout, Wo, dWo, dh, accumulate_dh, h, w, ns):

@@ -499,11 +499,16 @@ class Model(object):
     cfg = self.config
     if getattr(cfg, "optimizer", "adadelta") not in ("adadelta", "momentum", "adam", "rmsprop"):
       raise Exception("Optimizer not implemented")            # code/pred_models.py:1681
-    if getattr(cfg, "use_soft_grid_class", False) or getattr(cfg, "mask_grid_regression", False):
-      raise NotImplementedError("soft grid labels / masked regression loss are not implemented")
-    if not getattr(cfg, "train_w_onehot", False):
-      raise NotImplementedError("training feeds one_hot(argmax) to the decoder (--train_w_onehot, "
-                                "every published command); the soft-feedback variant is not built")
+    soft = bool(getattr(cfg, "use_soft_grid_class", False))
+    options = [name for name, on in (("use_soft_grid_class", soft),
+                                     ("mask_grid_regression", getattr(cfg, "mask_grid_regression", False)),
+                                     ("no train_w_onehot", not getattr(cfg, "train_w_onehot", True))) if on]
+    augment = [k for k in ("adv_train", "multiview_train") if getattr(cfg, k, False)]
+    if options and augment:
+      raise NotImplementedError("%s combined with SimAug's --%s is not implemented"
+                                % (" / ".join(options), " / --".join(augment)))
+    if soft and any(hasattr(cfg, k) for k in ("adv_train", "multiview_train")):
+      raise NotImplementedError("SimAug's model ignores --use_soft_grid_class; this combination is not implemented")
     eng = self._ensure_engine()
     dev = eng.device
     feeds = self._device_feeds(feed)
@@ -512,7 +517,7 @@ class Model(object):
     feeds["grid_pred_regress"] = [None] * len(cfg.scene_grids)
     for i in range(len(cfg.scene_grids)):
       if cfg.use_grids[i]:
-        feeds["grid_pred_labels"][i] = up(feed[self.grid_pred_labels_T[i]], np.int32)
+        feeds["grid_pred_labels"][i] = up(feed[self.grid_pred_labels_T[i]], np.float32 if soft else np.int32)
         feeds["grid_pred_regress"][i] = up(feed[self.grid_pred_regress[i]], np.float32)
     feeds = self._simaug_feeds(eng, feeds, feed)
     step = int(self.global_step.value)
@@ -649,7 +654,8 @@ def _engine_config(config):
   d["obs_len"] = getattr(config, "obs_len", None)    # multifuture_inference.py's Namespace has none (:419-452)
   d["activation_func"] = "tanh"
   for k, default in (("grid_loss_weight", 1.0), ("grid_reg_loss_weight", 0.1), ("wd", 0.0),
-                     ("clip_gradient_norm", None), ("is_train", False), ("optimizer", "adadelta")):
+                     ("clip_gradient_norm", None), ("is_train", False), ("optimizer", "adadelta"),
+                     ("mask_grid_regression", False), ("train_w_onehot", True)):
     d[k] = getattr(config, k, default)
   # SimAug's pred_models.py differs from Multiverse's in one line of gnn_edge (scene features only under
   # tile_to_beam): a config that carries SimAug's flags selects that variant unless it says otherwise
@@ -664,8 +670,9 @@ def _engine_config(config):
 
 
 def _soft_labels(cls, h, w, mode):
-  """Soft grid labels of code/pred_models.py:1085-1136 (3x3 / 5x5 neighbourhood smoothing)."""
-  from scipy import ndimage
+  """Soft grid labels of code/pred_models.py:1085-1136 (3x3 / 5x5 neighbourhood smoothing), for all rows at once.
+  The reference convolves each one-hot map (ndimage.convolve, mode='constant'); the kernels are symmetric, so every
+  cell receives exactly the kernel value at its offset from the label cell, or 0 outside the kernel."""
   tables = {1: (0.1, 1.0), 2: (0.01, 1.0), 3: (0.05, 1.0), 4: (0.0125, 0.9), 5: (0.05, 0.6), 6: (0.1, 0.2)}
   if mode == 7:
     k = np.full((5, 5), 0.0625)
@@ -676,13 +683,13 @@ def _soft_labels(cls, h, w, mode):
     k = np.full((3, 3), side)
     k[1, 1] = centre
   n, t = cls.shape
-  out = np.zeros((n, t, h, w, 1), dtype="float32")
-  for i in range(n):
-    for s in range(t):
-      m = np.zeros((h * w,), dtype="float")
-      m[cls[i, s]] = 1.0
-      out[i, s, :, :, 0] = ndimage.convolve(m.reshape(h, w), k, mode="constant", cval=0.0)
-  return out
+  r = k.shape[0] // 2
+  cell = np.arange(h * w)[np.asarray(cls).reshape(-1)]      # numpy indexing, as the reference's m[cls] = 1.0
+  dy = np.arange(h)[None, :] - (cell // w)[:, None] + r     # [M, h] kernel row of every cell
+  dx = np.arange(w)[None, :] - (cell % w)[:, None] + r      # [M, w]
+  inside = ((dy >= 0) & (dy <= 2 * r))[:, :, None] & ((dx >= 0) & (dx <= 2 * r))[:, None, :]
+  vals = k[np.clip(dy, 0, 2 * r)[:, :, None], np.clip(dx, 0, 2 * r)[:, None, :]]
+  return np.where(inside, vals, 0.0).astype("float32").reshape(n, t, h, w, 1)
 
 
 class Trainer(object):

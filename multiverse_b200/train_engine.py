@@ -7,6 +7,12 @@ all-reduce of the flat fp32 gradient buffer (SURVEY.md §8e): sum, scale by 1/G 
 optimizer kernel, then clip, which reproduces the single-GPU batch semantics because every loss
 is a mean over equal shards.
 
+Three training options of code/train.py:85-92 change the step: soft grid-class label maps
+(--use_soft_grid_class, feeds["grid_pred_labels"][i] fp32 [N,Tp,h,w,1]), the regression loss masked to the cells
+whose label is > 0 (--mask_grid_regression, divided by the foreground count K of the whole batch - a device scalar,
+all-reduced across ranks) and the class decoder fed its own logits map instead of one_hot(argmax) (no
+--train_w_onehot, the train.py default; gradient flows through that feedback).
+
 Per cell step the backward is  lstm_gates_bwd -> cell_dgrad (wgmma) -> cell_wgrad_direct (wgmma,
 MN-major operands read straight from the stored planes);  around it: head_bwd, emb_bwd, gnn_bwd, enc_class_input_bwd, scene_*_bwd.
 """
@@ -114,7 +120,11 @@ class TrainEngine(ConvRNNEngine):
       ops.cell_fwd_train(xh[t], sw.enc_class, None if t == 0 else c[t - 1], c[t],
                          h32_last if last else None, nxt, g[t], h, w, n)
     S.update(xh_ec=xh, c_ec=c, g_ec=g, h32_ec=h32_last)
-    # ---- class decoder (greedy, one-hot feedback: no gradient through the arg-max)
+    # ---- class decoder (greedy, one-hot feedback: no gradient through the arg-max; without train_w_onehot the
+    # embedded logits map is fed back, :426-435, and the gradient flows through it)
+    dense_fb = not getattr(cfg, "train_w_onehot", True)
+    assert not (dense_fb and mix is not None), "the logits-fed decoder is not combined with SimAug's mixup"
+    head = ops.head_class_fwd_dense if dense_fb else ops.head_class_fwd
     c = st("c_dc", Tp); g = gt("g_dc", Tp); h32 = st("h32_dc", Tp)
     logits = self._one(("logits", i, n), lambda: torch.empty((Tp, n, h * w), device=dev))
     ids = self._one(("ids", i, n), lambda: torch.empty((Tp, n), dtype=torch.int32, device=dev))
@@ -142,10 +152,10 @@ class TrainEngine(ConvRNNEngine):
       last = t == Tp - 1
       ops.cell_fwd_train(xh_dc[t], sw.dec_class, c_prev, c[t], h32[t],
                          None if (cfg.use_gnn or last) else xh_dc[t + 1], g[t], h, w, n)
-      ops.head_class_fwd(h32[t], sw.head_class, logits[t], ids[t], None if last else We,
-                         None if last else be, None if last else xh_dc[t + 1], h, w, n, planes=P)
+      head(h32[t], sw.head_class, logits[t], ids[t], None if last else We, None if last else be,
+           None if last else xh_dc[t + 1], h, w, n, planes=P)
     S.update(xh_dc=xh_dc, c_dc=c, g_dc=g, h32_dc=h32, logits=logits, ids=ids, first_ids=first_ids,
-             first_map=first_map, We_pad=We_pad, labels2_t=labels2_t, mix=mix)
+             first_map=first_map, We_pad=We_pad, labels2_t=labels2_t, mix=mix, dense_fb=dense_fb)
     # ---- regression encoder
     xh = xs("xh_er", T, sw.enc_reg.cpad); c = st("c_er", T); g = gt("g_er", T)
     xh_dr = xs("xh_dr", Tp, sw.dec_reg.cpad)
@@ -188,7 +198,7 @@ class TrainEngine(ConvRNNEngine):
     ops.cell_wgrad_direct(dg, xh, cg.dwp, h, w, n)     # MN-major operands: no transposed copies
     return dxh, out_dc
 
-  def _backward_scale(self, i, S, feeds, convs, means, dconv, loss_out, cw, rw):
+  def _backward_scale(self, i, S, feeds, convs, means, dconv, loss_out, cw, rw, fg=None):
     cfg, dev = self.cfg, self.device
     n, h, w = S["n"], S["h"], S["w"]
     sw = self.scales[i]
@@ -201,13 +211,28 @@ class TrainEngine(ConvRNNEngine):
       v.zero()
     dh = self._one(("dh", i, n), lambda: ops.alloc_state(n, h, w, dev))
     # ---- losses and their gradients (Model.build_loss :988-1027)
-    lab = feeds["grid_pred_labels"][i].to(torch.int32).t().contiguous()          # [Tp,N]
+    lab_in = feeds["grid_pred_labels"][i]
+    soft = lab_in.dim() > 2                                                        # [N,Tp,h,w,1] label maps
+    if soft:
+      lab = lab_in.float().reshape(n, Tp, h * w).transpose(0, 1).contiguous()   # [Tp,N,HW]
+    else:
+      lab = lab_in.to(torch.int32).t().contiguous()                              # [Tp,N]
     tgt = feeds["grid_pred_regress"][i].float().transpose(0, 1).reshape(Tp, n, h * w, 2).contiguous()
     dlogits = self._one(("dlogits", i, n), lambda: torch.empty_like(S["logits"]))
     doffs = self._one(("doffs", i, n), lambda: torch.empty_like(S["offs"]))
     mix = S["mix"]
-    if mix is None:
+    assert mix is None or not (soft or fg is not None), "soft labels / masked regression with SimAug's mixup"
+    if mix is None and not soft and fg is None:
       ops.loss_fwd_bwd(S["logits"], lab, dlogits, cw, S["offs"], tgt, doffs, rw, loss_out)
+    elif mix is None:
+      if soft:
+        ops.soft_ce_fwd_bwd(S["logits"], lab, dlogits, cw, loss_out)
+      else:
+        ops.loss_fwd_bwd(S["logits"], lab, dlogits, cw, None, None, None, 0.0, loss_out)
+      if fg is not None:                    # (fg count [1] fp64, weight): mean over the foreground of the whole batch
+        ops.masked_huber_fwd_bwd(S["offs"], tgt, doffs, lab, fg[0], fg[1], loss_out)
+      else:
+        ops.loss_fwd_bwd(None, None, None, 0.0, S["offs"], tgt, doffs, rw, loss_out)
     else:
       # mixed labels (SimAug/code/pred_models.py:1371-1405): softmax CE against beta one_hot(l1) + (1-beta) one_hot(l2)
       # = beta CE(l1) + (1-beta) CE(l2), optionally times the per-sample focal weight (double_weighting)
@@ -242,6 +267,9 @@ class TrainEngine(ConvRNNEngine):
         dWe_pad = torch.zeros_like(S["We_pad"])
         ops.emb_bwd(dxh, None, S["first_map"], S["We_pad"], be, dWe_pad, G[nm["emb_class"][1]], None, False, h, w, n)
         G[nm["emb_class"][0]] += dWe_pad[:, :, :1]
+      elif t > 0 and S["dense_fb"]:         # input = logits[t-1]: its gradient joins dlogits[t-1] before head_bwd reads it
+        ops.emb_bwd(dxh, None, S["logits"][t - 1], We, be, G[nm["emb_class"][0]], G[nm["emb_class"][1]],
+                    dlogits[t - 1], True, h, w, n)
       else:
         ops.emb_bwd(dxh, ids_prev, None, We, be, G[nm["emb_class"][0]], G[nm["emb_class"][1]], None, False, h, w, n)
       gout = dxh[:, sw.dec_class.cxp:].contiguous()
@@ -292,7 +320,20 @@ class TrainEngine(ConvRNNEngine):
                             accumulate=True)
 
   # ------------------------------------------------------------------ public
-  def loss_and_grads(self, feeds, loss_scale=1.0, zero=True, dscene_out=None, cls_weight=None, reg_weight=None):
+  def fg_counts(self, feeds):
+    """Foreground size K of the masked regression loss per scale (fp64 [scales] on the device, no host sync): the
+    cells whose label is > 0 of the soft maps, or the in-range label cells of sparse labels."""
+    cfg = self.cfg
+    K = torch.zeros((len(cfg.scene_grids),), dtype=torch.float64, device=self.device)
+    for i, (h, w) in enumerate(cfg.scene_grids):
+      if cfg.use_grids[i]:
+        lab = feeds["grid_pred_labels"][i]
+        lab = lab.float().contiguous() if lab.dim() > 2 else lab.to(torch.int32).contiguous()
+        ops.fg_count(lab, h * w, K[i:i + 1])
+    return K
+
+  def loss_and_grads(self, feeds, loss_scale=1.0, zero=True, dscene_out=None, cls_weight=None, reg_weight=None,
+                     fg_count=None):
     """Forward + loss + backward.  feeds additionally needs grid_pred_labels[i] int32 [N,Tp] and
     grid_pred_regress[i] fp32 [N,Tp,h,w,2].  Returns (losses fp32 tensor [2*scales] on device in
     the reference's order cls_0, reg_0, cls_1, ..., wd_loss tensor); gradients are ADDED into
@@ -305,7 +346,10 @@ class TrainEngine(ConvRNNEngine):
     feeds["mixup"] (optional; SimAug multiview_exp 3, SimAug/code/pred_models.py:616-638, :1371-1405) =
     dict(beta, obs_labels2[i] int [N,T], pred_labels2[i] int [N,Tp], focal fp32 [N] or None): the observed class
     maps (encoder input and the decoder's first input) and the loss labels become beta * view 1 + (1 - beta) * view 2,
-    the per-sample classification losses are weighted by `focal`."""
+    the per-sample classification losses are weighted by `focal`.
+    grid_pred_labels[i] may be fp32 label maps [N,Tp,h,w,1] (--use_soft_grid_class).  Under cfg.mask_grid_regression
+    the regression loss is divided by fg_count[i] (fg_counts of the whole batch this call is part of; loss_scale then
+    does not apply to it), or by this call's own count when fg_count is None."""
     cfg, dev = self.cfg, self.device
     cls_w = cfg.grid_loss_weight if cls_weight is None else cls_weight
     reg_w = cfg.grid_reg_loss_weight if reg_weight is None else reg_weight
@@ -317,12 +361,22 @@ class TrainEngine(ConvRNNEngine):
     used = [i for i in range(len(cfg.scene_grids)) if cfg.use_grids[i]]
     loss_out = torch.zeros((len(cfg.scene_grids), 2), dtype=torch.float32, device=dev)
     dconv = [torch.zeros_like(c) for c in convs]
+    fg = None
+    mask = getattr(cfg, "mask_grid_regression", False)
+    assert fg_count is None or mask, "fg_count is the denominator of the masked regression loss (mask_grid_regression)"
+    if mask:
+      if fg_count is None:
+        fg_count, fg_w = self.fg_counts(feeds), reg_w * loss_scale
+      else:
+        fg_w = reg_w
     self.last_logits = {}      # scale -> class logits [Tp,N,HW] of this call's train-mode forward (engine buffers)
     for i in used:
       S = self._forward_scale(i, feeds, convs, means)
       self.last_logits[i] = S["logits"]
+      if fg_count is not None:
+        fg = (fg_count[i:i + 1], fg_w)
       self._backward_scale(i, S, feeds, convs, means, dconv, loss_out[i],
-                           cls_w * loss_scale, reg_w * loss_scale)
+                           cls_w * loss_scale, reg_w * loss_scale, fg)
     # scene CNN backward: conv_k -> conv_{k-1} chain (code/pred_models.py:155-165)
     ins = [scene_feat] + convs[:-1]
     for k in range(len(convs) - 1, -1, -1):
@@ -361,12 +415,15 @@ class TrainEngine(ConvRNNEngine):
         raise ValueError("Optimizer not implemented: %r" % (opt,))      # :1681
     self._repack()
 
-  def loss_and_grads_chunked(self, feeds, micro_batch):
+  def loss_and_grads_chunked(self, feeds, micro_batch, fg_count=None):
     """loss_and_grads over a batch larger than the activation store allows: gradient
-    accumulation over contiguous chunks (identical result - every loss is a batch mean)."""
+    accumulation over contiguous chunks (identical result - every loss is a batch mean; the masked regression loss,
+    whose foreground differs per chunk, divides every chunk by the foreground count of the whole batch)."""
     n = feeds["obs_scene"].shape[0]
+    if fg_count is None and getattr(self.cfg, "mask_grid_regression", False):
+      fg_count = self.fg_counts(feeds)
     if not micro_batch or n <= micro_batch:
-      return self.loss_and_grads(feeds)
+      return self.loss_and_grads(feeds, fg_count=fg_count)
     assert n % micro_batch == 0, "batch must be a multiple of the micro batch"
     total, wd = None, None
     for lo in range(0, n, micro_batch):
@@ -380,15 +437,24 @@ class TrainEngine(ConvRNNEngine):
         part["mixup"] = dict(beta=mx["beta"], obs_labels2=[None if a is None else a[sl] for a in mx["obs_labels2"]],
                              pred_labels2=[None if a is None else a[sl] for a in mx["pred_labels2"]],
                              focal=None if mx.get("focal") is None else mx["focal"][sl])
-      losses, wd = self.loss_and_grads(part, loss_scale=micro_batch / float(n), zero=(lo == 0))
+      losses, wd = self.loss_and_grads(part, loss_scale=micro_batch / float(n), zero=(lo == 0), fg_count=fg_count)
       total = losses if total is None else total + losses
     return total, wd
 
   def train_step(self, feeds, lr, dist=None, micro_batch=0):
-    losses, wd = self.loss_and_grads_chunked(feeds, micro_batch)
     world = 1
     if dist is not None and dist.is_initialized() and dist.get_world_size() > 1:
       world = dist.get_world_size()
+    fg_count = None
+    if getattr(self.cfg, "mask_grid_regression", False):
+      fg_count = self.fg_counts(feeds)
+      if world > 1:
+        # the gradients are summed over ranks and scaled by 1/world: dividing by K_all / world makes that sum the
+        # mean over the foreground of the global batch
+        dist.all_reduce(fg_count)
+        fg_count /= world
+    losses, wd = self.loss_and_grads_chunked(feeds, micro_batch, fg_count)
+    if world > 1:
       ev = getattr(self, "allreduce_events", None)   # bench.py: CUDA events around the collective
       if ev is not None:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
