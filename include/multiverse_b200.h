@@ -14,8 +14,10 @@
  *   - return 0 on success, non-zero on error; mvb_last_error() returns a thread-local message.
  *   - activations use the library's "halo" layout: a grid of H x W cells is stored as
  *     S = (H+1)*(W+1) rows per sample, row = y*(W+1)+x, the extra column/row are zeros that
- *     the library never writes.  "planes" are the P bf16 summands of an fp32 value
- *     (v = p0 + p1 (+ p2)); a plane tensor is [P][rows][cpad] bf16.
+ *     the library never writes.  Operands are stored in one of two formats, selected by a `planes`
+ *     argument: planes == 2 ("bf16x2") stores an fp32 value as two bf16 summands (v = p0 + p1) in a
+ *     plane tensor [2][rows][cpad] bf16; planes == MVB_PLANES_F16F8 selects the inference format
+ *     described at mvb_pack_cell_weights.  Any other value is refused.
  *   - NS is the number of sample rows (batch, or batch*beam); fp32 state tensors are
  *     [NS*S, 256]; the hidden size is fixed at 256 (enc/dec_hidden_size of every published config).
  */
@@ -45,7 +47,7 @@ int mvb_cell_cpad(int cx);
 
 /* Pack a TF ConvLSTM `kernel` [3,3,cx+256,1024] (HWIO; gate order i,j,f,o) and `biases` [1024]
  * (host layout of the TF variables, but resident on the device) into
- *   w_planes   bf16 [P][1024][9*cpad]   (row = tile*256 + gate*64 + ch%64, K-major)
+ *   w_planes   bf16 [2][1024][9*cpad]   (row = tile*256 + gate*64 + ch%64, K-major)
  *   bias_packed fp32 [1024]             (same row order).
  * comp != 0 (needs planes == 2 and 4*cx <= roundup(cx,32)): "compensated x block" for inputs of
  * large magnitude (the regression encoder's raw pixel offsets, pred_models.py:232): the zero
@@ -68,17 +70,18 @@ int mvb_pack_cell_weights(const float* kernel, const float* biases, void* w_plan
 /* Which cell kernel the calling process launched last: planes * 2 + (1 if the CTA-pair / weight-multicast
  * variant ran), -1 before the first launch.  Lets tests assert that the variant they mean to check ran. */
 int mvb_cell_last_variant(void);
-/* Bit mask of the cell kernel variants launched since the last call with reset != 0: bit (f * 2 + pair), f = 0, 1, 2
- * for 1, 2, 3 bf16 planes and 3 for MVB_PLANES_F16F8; pair = the CTA-pair (cluster of two) variant. */
+/* Bit mask of the cell kernel variants launched since the last call with reset != 0: bit (f * 2 + pair), f = 0 for
+ * planes == 2 and 1 for MVB_PLANES_F16F8; pair = the CTA-pair (cluster of two) variant. */
 long long mvb_cell_variants_seen(int reset);
 
 /* One cell step over NS sample rows:  (c_in, xh) -> (c_out, h).
- *   xh_planes  bf16 [P][NS*S][cpad]: concat([x (cx, zero-padded to roundup(cx,32)), h (256)])
+ *   xh_planes  bf16 [2][NS*S][cpad]: concat([x (cx, zero-padded to roundup(cx,32)), h (256)])
  *   c_in       fp32 [*,256] or NULL (zero state); row_map int32 [NS] (source sample row of c_in
  *              for each sample row - the beam search's parent gather, pred_models.py:611-623) or NULL
  *   c_out      fp32 [NS*S,256];  h32_out fp32 [NS*S,256] or NULL
  *   hp_out     bf16 planes of h written at channel offset ch_off_out of rows with pitch cpad_out
  *              (the h block of the NEXT step's xh), plane stride hp_plane_stride elements; or NULL
+ *   planes     format of xh_planes and w_planes | (format of hp_out << 8) when the two differ
  * Semantics: g = conv3x3_SAME(concat[x,h]) + biases; i,j,f,o = split(g);
  *   c' = sigmoid(f+forget_bias)*c + sigmoid(i)*tanh(j);  h' = tanh(c')*sigmoid(o). */
 int mvb_convlstm_cell_fwd(const void* xh_planes, const void* w_planes, const float* bias_packed,
@@ -149,31 +152,22 @@ int mvb_convlstm_cell_fwd_train(const void* xh_planes, const void* w_planes,
                                 int ch_off_out, float* gates_out, int64_t NS, int H, int W, int cpad,
                                 int planes, float forget_bias, void* stream);
 /* Pointwise LSTM backward: (dh_t, dc_t (or NULL = 0), gates_t, c_{t-1} (or NULL = 0), c_t) ->
- * dg_planes bf16 [P][NS*S][1024] (pre-activation gate gradients; halo rows are never written and
- * must be zero), dc_prev fp32, dbias_packed[1024] += column sums. */
+ * dg_planes bf16 [2][NS*S][1024] (pre-activation gate gradients; halo rows are never written and
+ * must be zero), dc_prev fp32, dbias_packed[1024] += column sums.  The backward entry points take
+ * planes == 2 only. */
 int mvb_lstm_gates_bwd(const float* gates, const float* c_prev, const float* c_new, const float* dh,
                        const float* dc_in, void* dg_planes, int64_t plane_stride, float* dc_prev,
                        float* dbias_packed, int64_t NS, int H, int W, int planes, void* stream);
-/* bf16 planes [P][R][C] -> [P][taps][C][Rp] (Rp >= R, multiple of 8): K-major operands of the wgrad
- * GEMM.  taps == 1: plain transpose (dG).  taps == 9: one copy per 3x3 tap with the tap's halo-row
- * shift (dy-1)*(W+1)+(dx-1) applied (xh) - TMA inner coordinates must be 16-byte aligned, so the
- * shift cannot be done by the GEMM along its contiguous K axis. */
-int mvb_transpose_planes(const void* src, void* dst, int64_t R, int C, int64_t Rp, int planes,
-                         int taps, int W, void* stream);
-/* TF kernel [3,3,cx+256,1024] -> dgrad operand planes bf16 [P][cpad][9*1024]. */
+/* TF kernel [3,3,cx+256,1024] -> dgrad operand planes bf16 [2][cpad][9*1024]. */
 int mvb_pack_cell_weights_dgrad(const float* kernel, void* wd_planes, int cx, int planes,
                                 void* stream);
 /* dxh fp32 [NS*S, cpad] = conv3x3^T(dG, W): gradient w.r.t. concat([x, h]) of the step; the h block
  * (columns [cpad-256, cpad)) always, the x block only if need_dx (the regression encoder's input is data). */
 int mvb_cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, int64_t NS, int H,
                    int W, int cpad, int planes, int need_dx, void* stream);
-/* dw_packed fp32 [1024][9*cpad] += dG^T x im2col(xh): weight gradient of the step.  dgT_planes
- * [P][1024][Rp] and xhT_planes [P][9][cpad][Rp] come from mvb_transpose_planes (taps 1 / 9). */
-int mvb_cell_wgrad(const void* dgT_planes, const void* xhT_planes, float* dw_packed, int64_t NS,
-                   int H, int W, int cpad, int64_t Rp, int planes, void* stream);
-/* Same result without the transposed copies: both operands are read MN-major straight from the
- * row-major planes (dG [P][NS*S][1024], xh [P][NS*S][cpad]); the tap is a row shift of the TMA box.
- * dw_packed: fp32 [mvb_cell_wgrad_slabs(cpad)][1024][9*cpad], accumulated (+=). */
+/* dw_packed += dG^T x im2col(xh): weight gradient of the step.  Both operands are read MN-major
+ * straight from the row-major planes (dG [2][NS*S][1024], xh [2][NS*S][cpad]); the tap is a row
+ * shift of the TMA box.  dw_packed: fp32 [mvb_cell_wgrad_slabs(cpad)][1024][9*cpad], accumulated (+=). */
 int mvb_cell_wgrad_direct(const void* dg_planes, const void* xh_planes, float* dw_packed, int64_t NS,
                           int H, int W, int cpad, int planes, void* stream);
 /* packed accumulators -> gradients of the TF variables kernel [3,3,cx+256,1024], biases [1024]
@@ -182,7 +176,7 @@ int mvb_unpack_cell_wgrad(const float* dw_packed, const float* dbias_packed, flo
                           float* dbiases, int cx, int comp, int accumulate, int slabs, void* stream);
 /* Number of fp32 slabs [1024][9*cpad] mvb_cell_wgrad_direct accumulates into (its K split: every
  * (tile, k-split) work item owns one slab region, so no atomics); dw_packed must hold that many,
- * zero-initialised, and mvb_unpack_cell_wgrad sums them (slabs = 1 for mvb_cell_wgrad). */
+ * zero-initialised, and mvb_unpack_cell_wgrad sums them. */
 int mvb_cell_wgrad_slabs(int cpad);
 
 /* ---- a12: loss (Model.build_loss, pred_models.py:961-1040) --------------------------------
@@ -285,7 +279,7 @@ int mvb_head_class_fwd(const float* h32, const float* Wo, float* logits_out, int
                        void* stream);
 /* Class head of the training-mode decoder without --train_w_onehot (:426-435): as mvb_head_class_fwd, but
  * the x block receives tanh(conv3x3(logits, We[3,3,1,E]) + be) - the embedded logits map itself, not the one-hot
- * of its arg-max.  planes 1-3 only (a training format). */
+ * of its arg-max.  planes == 2 only (a training format). */
 int mvb_head_class_fwd_dense(const float* h32, const float* Wo, float* logits_out, int32_t* ids_out,
                              const float* We, const float* be, int E, void* xh_next, int64_t plane_stride, int cpad,
                              int64_t NS, int H, int W, int planes, void* stream);

@@ -39,10 +39,8 @@ SIGNATURES = {
     "mvb_convlstm_cell_fwd_train": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp, _i64, _i, _i,
                                     _i, _i, _f, _vp],
     "mvb_lstm_gates_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _i64, _i, _i, _i, _vp],
-    "mvb_transpose_planes": [_vp, _vp, _i64, _i, _i64, _i, _i, _i, _vp],
     "mvb_pack_cell_weights_dgrad": [_vp, _vp, _i, _i, _vp],
     "mvb_cell_dgrad": [_vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _vp],
-    "mvb_cell_wgrad": [_vp, _vp, _vp, _i64, _i, _i, _i, _i64, _i, _vp],
     "mvb_cell_wgrad_direct": [_vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp],
     "mvb_unpack_cell_wgrad": [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp],
     "mvb_cell_wgrad_slabs": [_i],

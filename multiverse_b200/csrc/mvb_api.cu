@@ -112,7 +112,7 @@ static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s)
 extern "C" {
 
 const char* mvb_last_error(void) { return get_error(); }
-int mvb_abi_version(void) { return 12; }
+int mvb_abi_version(void) { return 13; }
 int mvb_cell_last_variant(void) { return cell_last_variant(); }
 long long mvb_cell_variants_seen(int reset) { return (long long)cell_variants_seen(reset); }
 long long mvb_launch_count(void) { return g_launches; }
@@ -198,10 +198,6 @@ int mvb_lstm_gates_bwd(const float* gates, const float* c_prev, const float* c_n
   return lstm_gates_bwd(gates, c_prev, c_new, dh, dc_in, dg_planes, plane_stride, dc_prev,
                         dbias_packed, NS, H, W, planes, S(stream));
 }
-int mvb_transpose_planes(const void* src, void* dst, int64_t R, int C, int64_t Rp, int planes,
-                         int taps, int W, void* stream) {
-  return transpose_planes(src, dst, R, C, Rp, planes, taps, W + 1, S(stream));
-}
 int mvb_pack_cell_weights_dgrad(const float* kernel, void* wd_planes, int cx, int planes,
                                 void* stream) {
   return pack_cell_weights_dgrad(kernel, wd_planes, cx, planes, S(stream));
@@ -209,10 +205,6 @@ int mvb_pack_cell_weights_dgrad(const float* kernel, void* wd_planes, int cx, in
 int mvb_cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, int64_t NS, int H,
                    int W, int cpad, int planes, int need_dx, void* stream) {
   return cell_dgrad(dg_planes, wd_planes, dxh, NS, H, W, cpad, planes, need_dx, S(stream));
-}
-int mvb_cell_wgrad(const void* dgT_planes, const void* xhT_planes, float* dw_packed, int64_t NS,
-                   int H, int W, int cpad, int64_t Rp, int planes, void* stream) {
-  return cell_wgrad(dgT_planes, xhT_planes, dw_packed, NS, H, W, cpad, Rp, planes, S(stream));
 }
 int mvb_cell_wgrad_direct(const void* dg_planes, const void* xh_planes, float* dw_packed, int64_t NS,
                           int H, int W, int cpad, int planes, void* stream) {

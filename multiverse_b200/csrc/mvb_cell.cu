@@ -9,10 +9,10 @@
 //     G[R, 1024] = A[R, 9*Cpad] * Bt[1024, 9*Cpad]^T
 // over the halo layout (mvb_common.cuh): the A k-block for tap t / channel chunk q is
 // the rows [m0+shift(t), +128) x channels [64q, +64) of the activation matrix, read in place from one TMA-loaded
-// stage per chunk, so the 3x3 im2col never exists in memory.  fp32 parity on bf16 tensor cores comes
-// from operand planes: x = x0+x1(+x2) with every plane bf16 (mvb::split_planes), and
-// the products a_i*b_j with i+j < P are all accumulated into the same fp32 accumulator
-// (P=2 -> 3 MMAs, error ~2^-17; P=3 -> 6 MMAs, ~2^-24; P=1 -> plain bf16).
+// stage per chunk, so the 3x3 im2col never exists in memory.  fp32 parity on 16-bit tensor cores comes from one of
+// two operand formats (mvb_common.cuh): bf16x2, x = x0 + x1 with both planes bf16 (mvb::split_planes), whose products
+// a0*b0 + a0*b1 + a1*b0 (3 MMAs, error ~2^-17) go into the same fp32 accumulator; or f16f8, an fp16 pass and an e4m3
+// cross-term pass at twice the rate (2 bf16-pass equivalents) at the same accuracy.
 // Output columns are gate-interleaved (tile of 256 = 4 gates x 64 channels) so every
 // thread holds i,j,f,o of its channels in its accumulator registers and emits (c', h') directly - the gate
 // pre-activations never reach HBM.
@@ -43,14 +43,16 @@ constexpr uint32_t SW128_SBO = 8 * ROW_BYTES;      // 1024 B between 8-row group
 // Shared-memory rings.  The TMA unit writes about one box row per clock into shared memory whatever the row's width,
 // so the stages are made of full 128-byte rows and no activation row is loaded once per tap:
 //   B ring: slots of 256 rows x 128 B = 64 channels of ONE plane of the weight tile (SWIZZLE_128B): per (chunk,
-//           tap) P slots (bf16 planes) or 2 (f16f8: the fp16 plane, then both e4m3 planes interleaved in one row).
+//           tap) 2 slots (bf16x2: one per weight plane), or one per pass (f16f8: the fp16 plane, then both e4m3 planes
+//           interleaved in one row).
 //   A ring: one stage per 64-channel chunk: rows [m0 - (Wp+1), m0 + 128 + (Wp+1)) of every activation plane,
 //           rounded up to a multiple of 8 rows (RA8).  The nine taps of the chunk read THE SAME stage through wgmma
 //           descriptors that start (dy Wp + dx) rows into it (see make_smem_desc).
-template <int P> struct CellCfg {
+struct CellCfg {
   static constexpr int A_STAGES = 2;
   static constexpr int MAX_RA8 = 256;           // TMA box limit: 128 + 2 (W + 2) <= 256  ->  W <= 62
-  static constexpr int a_stage_bytes(int ra8) { return P * ra8 * ROW_BYTES; }
+  // both formats hold the bytes of two bf16 planes (f16f8 loads one half per pass)
+  static constexpr int a_stage_bytes(int ra8) { return kBf16Planes * ra8 * ROW_BYTES; }
   static constexpr int b_slots(int ra8) {       // 4 slots when they fit beside the A ring, else 3
     return (4 * B_SLOT_BYTES + A_STAGES * a_stage_bytes(ra8) + 2048 <= 227 * 1024) ? 4 : 3;
   }
@@ -84,13 +86,10 @@ struct CellParams {
   const float* xr_in;       // [NS, H, W, 2] fp32 NHWC (no halo), or nullptr
   const float* xr_W;        // [9 taps * 2 channels][1024] fp32, packed column order
   int order;                // work order, see work_index()
-  int abl;                  // debug ablations (MVB_CELL_ABL; results are then WRONG): 1 skip the fp8 MMAs, 2 skip the
-                            // 16-bit MMAs, 4 skip the epilogue's math and stores, 8 the issuer does not wait for operand
-                            // data, 16 the producer loads nothing (use with 8)
   float* preact_out;        // [R, 1024] raw accumulators (packed column order) instead of the state update: first stage of
                             // the fan-out step (fanout_children_kernel turns every parent row into its K children)
-  int hp_mixed;             // hp_out is written in the f16f8 format (else P bf16 planes)
-  __nv_bfloat16* hp_out;    // [P][R][cpad_out] plane base or nullptr
+  int hp_mixed;             // hp_out is written in the f16f8 format (else bf16x2 planes)
+  __nv_bfloat16* hp_out;    // [2][R][cpad_out] plane base or nullptr
   long long hp_plane_stride;  // elements between planes of hp_out
   int cpad_out;             // row pitch of hp_out (elements)
   int ch_off_out;           // channel offset of the h block inside hp_out rows
@@ -129,7 +128,7 @@ struct EpiRow {
 __device__ __forceinline__ EpiRow epi_row(const CellParams& prm, const Grid& g, long long row) {
   EpiRow r;
   r.row = row; r.src_row = row; r.psmp = 0; r.py = 0; r.px = 0; r.xfb = nullptr; r.xft = nullptr;
-  r.valid = row < prm.R && !(prm.abl & 4);
+  r.valid = row < prm.R;
   if (!r.valid) return r;
   const long long smp = row / g.S;
   const int rem = (int)(row - smp * g.S);
@@ -163,7 +162,7 @@ __device__ __forceinline__ EpiRow epi_row(const CellParams& prm, const Grid& g, 
 
 // The epilogue of one row and two adjacent packed columns j, j + 1 of every gate (a[gate][e] = accumulators of
 // column gate * 64 + j + e of N tile nt): state update and every requested output.
-template <int P, int FMT>
+template <int FMT>
 __device__ __forceinline__ void epi_pair(const CellParams& prm, const Grid& g, const EpiRow& r, int nt, int j,
                                          const float (&a)[4][2]) {
   const int col = nt * BLOCK_N + j;             // packed column of gate 0
@@ -236,11 +235,11 @@ __device__ __forceinline__ void epi_pair(const CellParams& prm, const Grid& g, c
     *reinterpret_cast<uint16_t*>(b8 + f8_off(c, 0, prm.cpad_out)) = (uint16_t)e0;
     *reinterpret_cast<uint16_t*>(b8 + f8_off(c, 1, prm.cpad_out)) = (uint16_t)e1;
   } else if (prm.hp_out) {
-    __nv_bfloat16 p0[P], p1[P];
-    split_planes<P>(o[0].h, p0);
-    split_planes<P>(o[1].h, p1);
+    __nv_bfloat16 p0[kBf16Planes], p1[kBf16Planes];
+    split_planes(o[0].h, p0);
+    split_planes(o[1].h, p1);
 #pragma unroll
-    for (int p = 0; p < P; ++p)
+    for (int p = 0; p < kBf16Planes; ++p)
       *reinterpret_cast<uint32_t*>(prm.hp_out + p * prm.hp_plane_stride + r.row * prm.cpad_out + prm.ch_off_out + ch) =
           pack_bf16x2(p0[p], p1[p]);
   }
@@ -248,18 +247,17 @@ __device__ __forceinline__ void epi_pair(const CellParams& prm, const Grid& g, c
 
 // MC = true: clusters of two CTAs work on two M tiles of the same N tile in lock step; each loads half of every B
 // (weight) tile and TMA-multicasts it to both, so the L2 -> shared-memory traffic per CTA and stage drops from
-// 48 KB to 32 KB (P = 2).  A slot may be refilled once the MMA warpgroups of BOTH CTAs have consumed it (empty
+// 48 KB to 32 KB (bf16x2).  A slot may be refilled once the MMA warpgroups of BOTH CTAs have consumed it (empty
 // barrier count 4: two warpgroups per CTA arrive on their own and on the peer's barrier).
-// FMT = 1: f16f8 operands (P must be 2: same stage bytes).  tmA / tmB then describe the fp16 regions (one
+// FMT = 1: f16f8 operands (FMT = 0: bf16x2).  tmA / tmB then describe the fp16 regions (one
 // "plane") and tmA8 / tmB8 the two fp8 planes; per 64-channel chunk and tap each warpgroup sends four e4m3 MMAs
 // (K = 32 each) and four fp16 MMAs (K = 16 each) into the same accumulator: 2 bf16-pass equivalents instead of 3.
-template <int P, bool MC, int FMT>
+template <bool MC, int FMT>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmA8, const __grid_constant__ CUtensorMap tmB8,
                 const CellParams prm) {
-  static_assert(FMT == 0 || P == 2, "the f16f8 format occupies the bytes of two bf16 planes");
-  using Cfg = CellCfg<P>;
+  using Cfg = CellCfg;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
@@ -287,7 +285,7 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   // with a short internal sum (about 14 significant bits of the accumulator), so they run while the accumulator holds
   // only their own small sum (~2^-11 of the result); the fp16 MMAs, exact in fp32, then add the main products.
   constexpr int NPASS = FMT ? 2 : 1;
-  constexpr int NS = FMT ? 1 : P;              // B slots per (pass, chunk, tap)
+  constexpr int NS = FMT ? 1 : kBf16Planes;    // B slots per (pass, chunk, tap)
   const long long num_m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
   // work index w -> (m tile, n tile).  MC: the pair shares w; rank r takes m tile 2*(w / N_TILES) + r.
   const uint32_t rank = MC ? cluster_ctarank() : 0u;
@@ -324,7 +322,6 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         // chunk-major K order: the x block - whose terms can be orders of magnitude larger than the h terms (raw
         // pixel offsets in the regression encoder) - is accumulated first, so the small h products are never added
         // onto a large transient partial sum.
-        if (prm.abl & 16) continue;
         for (int pass = 0; pass < NPASS; ++pass)
         for (int q = q_begin; q < NQ; ++q) {
           const int c16 = q == 0 ? 0 : cxp + (q - 1) * CHUNK;              // 16-bit channel coordinate
@@ -360,7 +357,6 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     const int c = wg - 1;
     const bool leader = (threadIdx.x & 127) == 0;          // arrives on the barriers for the warpgroup
     constexpr uint32_t kHi = smem_desc_hi(SW128_SBO, SW128_LAYOUT);
-    const bool do16 = !(prm.abl & 2), do8 = !(prm.abl & 1), wait_data = !(prm.abl & 8);
     const uint32_t a_plane_lo = (uint32_t)(ra8 * ROW_BYTES) >> 4;
     const uint32_t a_wg_lo = (uint32_t)(64 * c) * (ROW_BYTES >> 4);      // this warpgroup's 64 rows of the A tile
     int slot = 0, astage = 0; uint32_t phase = 0, aphase = 0;
@@ -391,25 +387,26 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       for (int pass = 0; pass < NPASS; ++pass)
       for (int q = q_begin; q < NQ; ++q) {
         const bool f8 = FMT == 1 && pass == 0;
-        if (wait_data) mbar_wait(&afull_bar[astage], aphase);
+        mbar_wait(&afull_bar[astage], aphase);
         const uint32_t sa_lo = (smem_u32(smem_a + astage * a_stage_bytes) >> 4) + a_wg_lo;
         for (int tap = 0; tap < 9; ++tap) {
           // the tap's A tile: the stage's rows starting (dy-1) Wp + (dx-1) + (Wp+1) = dy Wp + dx rows in
           const uint32_t a_lo = sa_lo + (uint32_t)((tap / 3) * g.Wp + (tap % 3)) * (ROW_BYTES >> 4);
 #pragma unroll
           for (int sl = 0; sl < NS; ++sl) {
-            if (wait_data) mbar_wait(&full_bar[slot], phase);
+            mbar_wait(&full_bar[slot], phase);
             const uint32_t b_lo = smem_u32(smem + slot * B_SLOT_BYTES) >> 4;
             wgmma_fence_regs(acc);
             wgmma_fence();
             if (q > 0) {
               // ---- h chunk: 64 channels = 4 K16 steps per 16-bit plane pair, 4 K32 steps over the two e4m3 planes ----
               if (f8) {
-                if (do8) for (int k = 0; k < 4; ++k) mma8(a_lo + 2 * k, b_lo + 2 * k);    // [e0 (64 B) | e1 (64 B)]
-              } else if (do16) {
-                // B plane sl against the A planes pa with pa + sl < P (f16f8: the fp16 planes, P - sl = 1)
+                for (int k = 0; k < 4; ++k) mma8(a_lo + 2 * k, b_lo + 2 * k);    // [e0 (64 B) | e1 (64 B)]
+              } else {
+                // bf16x2: B plane 0 against A planes 0 and 1, B plane 1 against A plane 0 (a0b0 + a1b0 + a0b1);
+                // f16f8: the fp16 planes
 #pragma unroll
-                for (int pa = 0; pa < (FMT ? 1 : P - sl); ++pa)
+                for (int pa = 0; pa < (FMT ? 1 : kBf16Planes - sl); ++pa)
 #pragma unroll
                   for (int k = 0; k < 4; ++k) mma16(a_lo + pa * a_plane_lo + 2 * k, b_lo + 2 * k);
               }
@@ -418,13 +415,13 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
               const int ks16 = cxp / MMA_K, ks8 = cxp / 32;
               const uint32_t poff = (uint32_t)cxp >> 4;              // e1 sits cxp bytes after e0 in an fp8 row
               if (f8) {
-                for (int pk = 0; pk < 2 * ks8 && do8; ++pk) {
+                for (int pk = 0; pk < 2 * ks8; ++pk) {
                   const uint32_t o = (pk / ks8) * poff + (pk % ks8) * 2;
                   mma8(a_lo + o, b_lo + o);
                 }
               } else {
-                for (int pa = 0; pa < (FMT ? 1 : P - sl); ++pa)
-                  for (int k = 0; k < ks16 && do16; ++k) mma16(a_lo + pa * a_plane_lo + 2 * k, b_lo + 2 * k);
+                for (int pa = 0; pa < (FMT ? 1 : kBf16Planes - sl); ++pa)
+                  for (int k = 0; k < ks16; ++k) mma16(a_lo + pa * a_plane_lo + 2 * k, b_lo + 2 * k);
               }
             }
             wgmma_commit();
@@ -441,10 +438,6 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       release();
-      if (fresh) {                          // no MMA ran (debug ablations): the accumulator is zero
-#pragma unroll
-        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-      }
       // ===================== epilogue =====================
       // thread (warp w of the warpgroup, lane l) holds rows 16 w + l / 4 (+ 8) and columns 8 i + 2 (l % 4) (+ 1);
       // column gate * 64 + j of the N tile is gate `gate` of channel j: each thread owns all four gates of its channels
@@ -461,7 +454,7 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             a[gt][0] = acc[4 * (8 * gt + ip) + 2 * hr];
             a[gt][1] = acc[4 * (8 * gt + ip) + 2 * hr + 1];
           }
-          epi_pair<P, FMT>(prm, g, r, nt, 8 * ip + 2 * (lane & 3), a);
+          epi_pair<FMT>(prm, g, r, nt, 8 * ip + 2 * (lane & 3), a);
         }
       }
     }
@@ -548,11 +541,10 @@ fanout_children_kernel(const float* __restrict__ acc, const float* __restrict__ 
 
 // ----------------------------------------------------------------------------------
 // weight packing:  TF kernel [3,3,Cx+256,1024] (HWIO, gate order i,j,f,o) + biases
-//   -> planes bf16 [P][1024][9*cpad]  (row = tile*256 + gate*64 + j,  k = tap*cpad + kc)
+//   -> planes bf16 [2][1024][9*cpad]  (row = tile*256 + gate*64 + j,  k = tap*cpad + kc)
 //   -> bias fp32 [1024] in the same row order
 // kc < cx: input channel kc;  cx <= kc < cxp: zero;  kc >= cxp: hidden channel kc-cxp.
 // ----------------------------------------------------------------------------------
-template <int P>
 __global__ void pack_weights_kernel(const float* __restrict__ kernel, const float* __restrict__ biases,
                                     __nv_bfloat16* __restrict__ wp, float* __restrict__ bias_packed,
                                     int cx, int cxp, int cpad, int comp) {
@@ -570,22 +562,19 @@ __global__ void pack_weights_kernel(const float* __restrict__ kernel, const floa
     else if (!comp) { if (kcn < cx) cin = kcn; }
     else if (kcn < 4 * cx) { blk = kcn / cx; cin = kcn - blk * cx; }
     const float v = (cin >= 0) ? kernel[((long long)tap * (cx + kHidden) + cin) * kGates + col] : 0.f;
-    __nv_bfloat16 pl[P];
-    split_planes<P>(v, pl);
-    if (comp && kcn < cxp && P == 2) {
-      // compensated x block (see nhwc_to_planes_comp): [W | W | W-w0-w1 | w1]
+    __nv_bfloat16 pl[kBf16Planes];
+    split_planes(v, pl);
+    if (comp && kcn < cxp) {
+      // compensated x block (see nhwc_to_planes_kernel): [W | W | W-w0-w1 | w1]
       if (blk == 2) {
-        float r = v;
-#pragma unroll
-        for (int p = 0; p < P; ++p) r -= __bfloat162float(pl[p]);
-        split_planes<P>(r, pl);
+        split_planes((v - __bfloat162float(pl[0])) - __bfloat162float(pl[1]), pl);
       } else if (blk == 3) {
-        pl[0] = pl[P - 1];
-        pl[P - 1] = __float2bfloat16_rn(0.f);
+        pl[0] = pl[1];
+        pl[1] = __float2bfloat16_rn(0.f);
       }
     }
-#pragma unroll
-    for (int p = 0; p < P; ++p) wp[(long long)p * total + i] = pl[p];
+    wp[i] = pl[0];
+    wp[total + i] = pl[1];
     if (k == 0) bias_packed[n] = biases[col];
   }
 }
@@ -724,17 +713,16 @@ int cell_xfold_tables(const float* kernel, const float* biases, const float* We,
 
 // variant of the last launch_cell() of this process: planes code * 2 + multicast (tests assert which kernel ran)
 static int g_last_variant = -1;
-static unsigned long long g_variants_seen = 0;      // bit (format index * 2 + pair): formats 1, 2, 3 planes, f16f8
+static unsigned long long g_variants_seen = 0;      // bit (format * 2 + pair): format 0 bf16x2, 1 f16f8
 int cell_last_variant() { return g_last_variant; }
 unsigned long long cell_variants_seen(int reset) {
   const unsigned long long v = g_variants_seen;
   if (reset) g_variants_seen = 0;
   return v;
 }
-static void note_variant(int planes, int pair) {
-  g_last_variant = planes * 2 + pair;
-  const int fi = planes == kPlanesF16F8 ? 3 : planes - 1;
-  g_variants_seen |= 1ull << (fi * 2 + pair);
+static void note_variant(int fmt, int pair) {
+  g_last_variant = (fmt ? kPlanesF16F8 : kBf16Planes) * 2 + pair;
+  g_variants_seen |= 1ull << (fmt * 2 + pair);
 }
 
 struct CellMaps { CUtensorMap A, B, Bh, A8, B8, B8h; };
@@ -751,16 +739,16 @@ static int pick_order(int forced, long long units, long long ctas) {
   return (strided < back_to_back && units < 4 * ctas) ? 0 : 1;
 }
 
-template <int P, int FMT>
+template <int FMT>
 static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms, bool multicast, cudaStream_t stream) {
-  using Cfg = CellCfg<P>;
+  using Cfg = CellCfg;
   CellParams prm = prm_in;
   static SmemOptIn opt_plain, opt_mc;
   const int ra8 = (BLOCK_M + 2 * (prm.W + 2) + 7) & ~7;
   const int smem_bytes = Cfg::smem_bytes(ra8);
   MVB_REQUIRE(ra8 <= Cfg::MAX_RA8 && smem_bytes <= 227 * 1024, "cell_fwd: grid width W=%d too large (A stage of %d rows, %d B shared memory)", prm.W, ra8, smem_bytes);
-  MVB_CHECK_CUDA(smem_opt_in(opt_plain, cell_fwd_kernel<P, false, FMT>, smem_bytes));
-  MVB_CHECK_CUDA(smem_opt_in(opt_mc, cell_fwd_kernel<P, true, FMT>, smem_bytes));
+  MVB_CHECK_CUDA(smem_opt_in(opt_plain, cell_fwd_kernel<false, FMT>, smem_bytes));
+  MVB_CHECK_CUDA(smem_opt_in(opt_mc, cell_fwd_kernel<true, FMT>, smem_bytes));
   const long long m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
   if (multicast && m_tiles >= 2 * (long long)num_sms) {
     prm.order = pick_order(prm_in.order, (m_tiles + 1) / 2, num_sms / 2);
@@ -771,18 +759,18 @@ static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    MVB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, cell_fwd_kernel<P, true, FMT>, tm.A, tm.Bh, tm.A8, tm.B8h, prm));
+    MVB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, cell_fwd_kernel<true, FMT>, tm.A, tm.Bh, tm.A8, tm.B8h, prm));
     count_launch(1);
-    note_variant(FMT ? kPlanesF16F8 : P, 1);
+    note_variant(FMT, 1);
     return MVB_OK;
   }
   const long long num_tiles = m_tiles * N_TILES;
   const int grid = (int)(num_tiles < num_sms ? num_tiles : num_sms);
   prm.order = pick_order(prm_in.order, m_tiles, grid);
-  cell_fwd_kernel<P, false, FMT><<<grid, NUM_THREADS, smem_bytes, stream>>>(tm.A, tm.B, tm.A8, tm.B8, prm);
+  cell_fwd_kernel<false, FMT><<<grid, NUM_THREADS, smem_bytes, stream>>>(tm.A, tm.B, tm.A8, tm.B8, prm);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
-  note_variant(FMT ? kPlanesF16F8 : P, 0);
+  note_variant(FMT, 0);
   return MVB_OK;
 }
 
@@ -795,9 +783,9 @@ int cell_fwd(const void* xh_planes, const void* w_planes, const float* bias, con
   // planes = format of the inputs and weights | (format of hp_out << 8), the latter only when it differs
   const int P_out = (P >> 8) ? (P >> 8) : (P & 0xFF);
   P &= 0xFF;
+  MVB_REQUIRE(valid_planes(P) && valid_planes(P_out), "cell_fwd: planes P=%d (output planes %d) not 2 or %d", P, P_out,
+              kPlanesF16F8);
   const bool mixed = P == kPlanesF16F8;
-  MVB_REQUIRE(P_out == P || P_out == kPlanesF16F8 || (mixed && P_out == 2), "cell_fwd: output planes %d with input planes %d", P_out, P);
-  MVB_REQUIRE((P >= 1 && P <= 3) || mixed, "cell_fwd: planes P=%d not in {1,2,3,%d}", P, kPlanesF16F8);
   MVB_REQUIRE(!mixed || !gates_out || fanout > 1, "cell_fwd: the f16f8 format is an inference format (no gates_out)");
   MVB_REQUIRE(fanout <= 1 || (xf_B && xf_T2 && xf_ids && gates_out && c_in && h32_out && !row_map && !hp_out),
               "cell_fwd: fanout=%d needs the x-fold tables, c_in, h32_out, a [R,1024] fp32 workspace and no row_map / hp_out", fanout);
@@ -812,7 +800,7 @@ int cell_fwd(const void* xh_planes, const void* w_planes, const float* bias, con
   // weight-tile multicast across CTA pairs is on by default (MVB_CELL_MULTICAST=0 turns it off for A/B runs)
   static const bool multicast = [] { const char* e = getenv("MVB_CELL_MULTICAST"); return !(e && e[0] == '0'); }();
   CellMaps tm;
-  const int P16 = mixed ? 1 : P;      // 16-bit "planes" the A / B maps describe
+  const int P16 = mixed ? 1 : kBf16Planes;      // 16-bit "planes" the A / B maps describe
   const uint32_t ra8 = (uint32_t)((BLOCK_M + 2 * (W + 2) + 7) & ~7);      // rows of an A stage (see CellCfg)
   MVB_REQUIRE(ra8 <= 256, "cell_fwd: grid width W=%d too large for the halo'd A stage (%u rows > 256)", W, ra8);
   int rc = encode_tmap_3d_bf16(&tm.A, xh_planes, (uint64_t)cpad, (uint64_t)R, (uint64_t)P16,
@@ -850,8 +838,6 @@ int cell_fwd(const void* xh_planes, const void* w_planes, const float* bias, con
   // work order: chosen per launch in launch_cell (MVB_CELL_ORDER=0|1 forces one)
   static const int order = [] { const char* e = getenv("MVB_CELL_ORDER"); return e ? atoi(e) : -1; }();
   prm.order = order;
-  static const int abl = [] { const char* e = getenv("MVB_CELL_ABL"); return e ? atoi(e) : 0; }();
-  prm.abl = (abl & 16) ? (abl | 8) : abl;      // "load nothing" without "do not wait for data" would hang the issuer
   if (xf_B) {
     MVB_REQUIRE(xf_T2 && xf_ids && H >= 3 && W >= 3, "cell_fwd: x-fold needs its tables, ids and a grid of at least 3x3");
     prm.skip_x = 1;
@@ -874,12 +860,7 @@ int cell_fwd(const void* xh_planes, const void* w_planes, const float* bias, con
   int dev = 0, num_sms = 0;
   MVB_CHECK_CUDA(cudaGetDevice(&dev));
   MVB_CHECK_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-  switch (P) {
-    case 1: rc = launch_cell<1, 0>(tm, prm, num_sms, multicast, stream); break;
-    case 2: rc = launch_cell<2, 0>(tm, prm, num_sms, multicast, stream); break;
-    case kPlanesF16F8: rc = launch_cell<2, 1>(tm, prm, num_sms, multicast, stream); break;
-    default: rc = launch_cell<3, 0>(tm, prm, num_sms, multicast, stream); break;
-  }
+  rc = mixed ? launch_cell<1>(tm, prm, num_sms, multicast, stream) : launch_cell<0>(tm, prm, num_sms, multicast, stream);
   if (rc || fanout <= 1) return rc;
   // fan-out stage 2: every parent row -> its K children (c_out / h32_out hold NS * fanout sample rows)
   const long long warps = NS * H * W;
@@ -956,8 +937,7 @@ __global__ void pack_weights_f16f8_kernel(const float* __restrict__ kernel, cons
 
 int pack_cell_weights(const float* kernel, const float* biases, void* w_planes, float* bias_packed,
                       int cx, int P, int comp, cudaStream_t stream) {
-  MVB_REQUIRE((P >= 1 && P <= 3) || P == kPlanesF16F8, "pack_cell_weights: planes P=%d not in {1,2,3,%d}", P,
-              kPlanesF16F8);
+  MVB_REQUIRE(valid_planes(P), "pack_cell_weights: planes P=%d not 2 or %d", P, kPlanesF16F8);
   MVB_REQUIRE(cx >= 1, "pack_cell_weights: cx=%d", cx);
   const int cxp = (cx + XPAD - 1) / XPAD * XPAD;
   const int cpad = cxp + kHidden;
@@ -973,14 +953,9 @@ int pack_cell_weights(const float* kernel, const float* biases, void* w_planes, 
     count_launch(2);
     return MVB_OK;
   }
-  MVB_REQUIRE(!comp || (P == 2 && 4 * cx <= cxp), "pack_cell_weights: compensated x block needs planes=2 and 4*cx <= %d", cxp);
-  __nv_bfloat16* wp = reinterpret_cast<__nv_bfloat16*>(w_planes);
-  const int threads = 256, blocks = 1184;
-  switch (P) {
-    case 1: pack_weights_kernel<1><<<blocks, threads, 0, stream>>>(kernel, biases, wp, bias_packed, cx, cxp, cpad, comp); break;
-    case 2: pack_weights_kernel<2><<<blocks, threads, 0, stream>>>(kernel, biases, wp, bias_packed, cx, cxp, cpad, comp); break;
-    default: pack_weights_kernel<3><<<blocks, threads, 0, stream>>>(kernel, biases, wp, bias_packed, cx, cxp, cpad, comp); break;
-  }
+  MVB_REQUIRE(!comp || 4 * cx <= cxp, "pack_cell_weights: compensated x block needs 4*cx <= %d", cxp);
+  pack_weights_kernel<<<1184, 256, 0, stream>>>(kernel, biases, reinterpret_cast<__nv_bfloat16*>(w_planes), bias_packed,
+                                                cx, cxp, cpad, comp);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;

@@ -68,16 +68,14 @@ __host__ __device__ inline Grid make_grid(int H, int W) {
 }
 
 // ----------------------------------------------------------------------------------
-// bf16 plane splitting:  v = p0 + p1 (+ p2) + O(2^-9P |v|)
+// "bf16x2" operand format (planes code kBf16Planes): v = p0 + p1 + O(2^-18 |v|), both planes bf16; the product
+// of two such operands is accumulated as a0*b0 + a0*b1 + a1*b0 (a1*b1, 2^-18 of the result, is dropped).
+// A plane tensor is [2][rows][cpad] bf16.
 // ----------------------------------------------------------------------------------
-template <int P>
-__device__ __forceinline__ void split_planes(float v, __nv_bfloat16 (&out)[P]) {
-  float r = v;
-#pragma unroll
-  for (int p = 0; p < P; ++p) {
-    out[p] = __float2bfloat16_rn(r);
-    r -= __bfloat162float(out[p]);
-  }
+constexpr int kBf16Planes = 2;
+__device__ __forceinline__ void split_planes(float v, __nv_bfloat16 (&out)[kBf16Planes]) {
+  out[0] = __float2bfloat16_rn(v);
+  out[1] = __float2bfloat16_rn(v - __bfloat162float(out[0]));
 }
 
 // ----------------------------------------------------------------------------------
@@ -95,6 +93,9 @@ __device__ __forceinline__ void split_planes(float v, __nv_bfloat16 (&out)[P]) {
 // ----------------------------------------------------------------------------------
 constexpr int kPlanesF16F8 = 16;
 constexpr float kF8ResidualScale = 4096.f;   // 2^12: residual of an fp16 rounding, brought into e4m3's range
+
+// the `planes` codes of the two operand formats; kernels that serve both take FMT = 0 (bf16x2) or 1 (f16f8)
+inline bool valid_planes(int P) { return P == kBf16Planes || P == kPlanesF16F8; }
 
 // byte offset inside an fp8 row of channel c, plane p
 __host__ __device__ __forceinline__ int f8_off(int c, int p, int cpad) {

@@ -13,7 +13,7 @@
 // cell, and the centre-left dot product is the previous step's centre-right one.  Per cell: 7 dot
 // products + 3 norms reduced by warp shuffles, a <=9-way softmax, 72 FMAs of weighted sum, and the
 // result is written straight as the bf16 operand planes of the next cell step.
-// HBM-bound by design: 4*HW*(256+64) bytes read, 2*P*HW*256 written per sample row.
+// HBM-bound by design: 4*HW*(256+64) bytes read, 4*HW*256 written per sample row (either operand format).
 #include "mvb_common.cuh"
 #include "mvb_kernels.h"
 
@@ -69,8 +69,8 @@ __device__ __forceinline__ void gnn_norms(GnnCol& c) {
   for (int r = 0; r < 3; ++r) c.inv[r] = rsqrtf(fmaxf(c.n[r], 1e-12f));
 }
 
-// MIX: the output is written in the f16f8 operand format (mvb_common.cuh) instead of P bf16 planes
-template <int P, bool MIX = false>
+// FMT = 1: the output is written in the f16f8 operand format (mvb_common.cuh), else as bf16x2 planes
+template <int FMT>
 __global__ void __launch_bounds__(GNN_WARPS * 32)
 gnn_kernel(const float* __restrict__ h32, const int* __restrict__ row_map,
            const float* __restrict__ scene_mean, int beam, __nv_bfloat16* __restrict__ hp_out,
@@ -149,20 +149,20 @@ gnn_kernel(const float* __restrict__ h32, const int* __restrict__ row_map,
     }
     const float o[8] = {o2[0].x, o2[0].y, o2[1].x, o2[1].y, o2[2].x, o2[2].y, o2[3].x, o2[3].y};
     const long long orow = s * g.S + (long long)y * g.Wp + x;
-    if constexpr (MIX) {
+    if constexpr (FMT) {
       store_f16f8_x8(hp_out, plane_stride, orow, ch_off + lane * 8, cpad_out, o);
     } else {
-      uint32_t pk[P][4];
+      uint32_t pk[kBf16Planes][4];
 #pragma unroll
       for (int v = 0; v < 4; ++v) {
-        __nv_bfloat16 a[P], b[P];
-        split_planes<P>(o[2 * v], a);
-        split_planes<P>(o[2 * v + 1], b);
+        __nv_bfloat16 a[kBf16Planes], b[kBf16Planes];
+        split_planes(o[2 * v], a);
+        split_planes(o[2 * v + 1], b);
 #pragma unroll
-        for (int p = 0; p < P; ++p) pk[p][v] = pack_bf16x2(a[p], b[p]);
+        for (int p = 0; p < kBf16Planes; ++p) pk[p][v] = pack_bf16x2(a[p], b[p]);
       }
 #pragma unroll
-      for (int p = 0; p < P; ++p) {
+      for (int p = 0; p < kBf16Planes; ++p) {
         uint4* po = reinterpret_cast<uint4*>(hp_out + p * plane_stride + orow * cpad_out + ch_off + lane * 8);
         *po = make_uint4(pk[p][0], pk[p][1], pk[p][2], pk[p][3]);
       }
@@ -214,11 +214,11 @@ __device__ __forceinline__ void dot_acc(float2& acc, const float4& a, const floa
   acc = ffma2(hi2(a), hi2(b), acc);
 }
 
-// 4 consecutive channels of one row into the operand buffer (bf16 planes or f16f8)
-template <int P, bool MIX>
+// 4 consecutive channels of one row into the operand buffer (FMT = 0: bf16x2 planes, 1: f16f8)
+template <int FMT>
 __device__ __forceinline__ void store_operand_x4(__nv_bfloat16* hp_out, long long plane_stride, long long row,
                                                  int ch, int cpad, const float (&v)[4]) {
-  if constexpr (MIX) {
+  if constexpr (FMT) {
     uint32_t hw[2], b0 = 0u, b1 = 0u;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -232,22 +232,22 @@ __device__ __forceinline__ void store_operand_x4(__nv_bfloat16* hp_out, long lon
     *reinterpret_cast<uint32_t*>(b8 + f8_off(ch, 0, cpad)) = b0;
     *reinterpret_cast<uint32_t*>(b8 + f8_off(ch, 1, cpad)) = b1;
   } else {
-    uint32_t pk[P][2];
+    uint32_t pk[kBf16Planes][2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      __nv_bfloat16 a[P], b[P];
-      split_planes<P>(v[2 * i], a);
-      split_planes<P>(v[2 * i + 1], b);
+      __nv_bfloat16 a[kBf16Planes], b[kBf16Planes];
+      split_planes(v[2 * i], a);
+      split_planes(v[2 * i + 1], b);
 #pragma unroll
-      for (int q = 0; q < P; ++q) pk[q][i] = pack_bf16x2(a[q], b[q]);
+      for (int q = 0; q < kBf16Planes; ++q) pk[q][i] = pack_bf16x2(a[q], b[q]);
     }
 #pragma unroll
-    for (int q = 0; q < P; ++q)
+    for (int q = 0; q < kBf16Planes; ++q)
       *reinterpret_cast<uint2*>(hp_out + q * plane_stride + row * cpad + ch) = make_uint2(pk[q][0], pk[q][1]);
   }
 }
 
-template <int P, bool MIX>
+template <int FMT>
 __global__ void __launch_bounds__(GT)
 gnn_rows_kernel(const float* __restrict__ h32, const int* __restrict__ row_map,
                 const float* __restrict__ scene_mean, int beam, __nv_bfloat16* __restrict__ hp_out,
@@ -412,8 +412,8 @@ gnn_rows_kernel(const float* __restrict__ h32, const int* __restrict__ row_map,
         const long long orow = s * g.S + (long long)y * g.Wp + xb + c;
         const float lo[4] = {o[c][0].x, o[c][0].y, o[c][1].x, o[c][1].y};
         const float hi[4] = {o[c][2].x, o[c][2].y, o[c][3].x, o[c][3].y};
-        store_operand_x4<P, MIX>(hp_out, plane_stride, orow, ch_off + 4 * lane, cpad_out, lo);
-        store_operand_x4<P, MIX>(hp_out, plane_stride, orow, ch_off + 128 + 4 * lane, cpad_out, hi);
+        store_operand_x4<FMT>(hp_out, plane_stride, orow, ch_off + 4 * lane, cpad_out, lo);
+        store_operand_x4<FMT>(hp_out, plane_stride, orow, ch_off + 128 + 4 * lane, cpad_out, hi);
       }
     }
   };
@@ -448,42 +448,28 @@ gnn_rows_kernel(const float* __restrict__ h32, const int* __restrict__ row_map,
 int gnn_attend_fwd(const float* h32, const int* row_map, const float* scene_mean, int beam,
                    void* hp_out, long long hp_plane_stride, int cpad_out, int ch_off_out,
                    long long NS, int H, int W, int P, cudaStream_t stream) {
-  MVB_REQUIRE((P >= 1 && P <= 3) || P == kPlanesF16F8, "gnn_attend_fwd: planes P=%d", P);
+  MVB_REQUIRE(valid_planes(P), "gnn_attend_fwd: planes P=%d not 2 or %d", P, kPlanesF16F8);
   MVB_REQUIRE(h32 && hp_out && NS > 0 && beam >= 1, "gnn_attend_fwd: bad args");
   MVB_REQUIRE(cpad_out % 8 == 0 && ch_off_out % 8 == 0, "gnn_attend_fwd: pitch/offset must be multiples of 8");
   const Grid g = make_grid(H, W);
   __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(hp_out);
-  // shared-memory ring formulation when a ring of image rows fits (W <= 42); MVB_GNN_ROWS=0 forces the
-  // warp-per-image-row kernel (A/B measurements)
-  static const bool rows_off = [] { const char* e = getenv("MVB_GNN_ROWS"); return e && e[0] == '0'; }();
+  const bool f16f8 = P == kPlanesF16F8;
+  // shared-memory ring formulation when a ring of image rows fits (W <= 42), else the warp-per-image-row kernel
   const size_t smem = gnn_rows_smem(W);
-  if (!rows_off && smem <= 220 * 1024 && ch_off_out % 4 == 0 && NS < (1ll << 31)) {
-#define MVB_GNN_ROWS_LAUNCH(PP, MM)                                                                             \
-    do {                                                                                                        \
-      MVB_CHECK_CUDA(cudaFuncSetAttribute(gnn_rows_kernel<PP, MM>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                          (int)smem));                                                          \
-      gnn_rows_kernel<PP, MM><<<(unsigned)NS, GT, smem, stream>>>(h32, row_map, scene_mean, beam, d,            \
-                                                                   hp_plane_stride, cpad_out, ch_off_out, g);   \
-    } while (0)
-    switch (P) {
-      case 1: MVB_GNN_ROWS_LAUNCH(1, false); break;
-      case 2: MVB_GNN_ROWS_LAUNCH(2, false); break;
-      case kPlanesF16F8: MVB_GNN_ROWS_LAUNCH(2, true); break;
-      default: MVB_GNN_ROWS_LAUNCH(3, false); break;
-    }
-#undef MVB_GNN_ROWS_LAUNCH
+  if (smem <= 220 * 1024 && ch_off_out % 4 == 0 && NS < (1ll << 31)) {
+    auto kernel = f16f8 ? gnn_rows_kernel<1> : gnn_rows_kernel<0>;
+    MVB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<(unsigned)NS, GT, smem, stream>>>(h32, row_map, scene_mean, beam, d, hp_plane_stride, cpad_out,
+                                               ch_off_out, g);
     MVB_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
     return MVB_OK;
   }
   const long long warps = NS * H;
   const unsigned blocks = (unsigned)((warps + GNN_WARPS - 1) / GNN_WARPS);
-  switch (P) {
-    case 1: gnn_kernel<1><<<blocks, GNN_WARPS * 32, 0, stream>>>(h32, row_map, scene_mean, beam, d, hp_plane_stride, cpad_out, ch_off_out, NS, g); break;
-    case 2: gnn_kernel<2><<<blocks, GNN_WARPS * 32, 0, stream>>>(h32, row_map, scene_mean, beam, d, hp_plane_stride, cpad_out, ch_off_out, NS, g); break;
-    case kPlanesF16F8: gnn_kernel<2, true><<<blocks, GNN_WARPS * 32, 0, stream>>>(h32, row_map, scene_mean, beam, d, hp_plane_stride, cpad_out, ch_off_out, NS, g); break;
-    default: gnn_kernel<3><<<blocks, GNN_WARPS * 32, 0, stream>>>(h32, row_map, scene_mean, beam, d, hp_plane_stride, cpad_out, ch_off_out, NS, g); break;
-  }
+  auto kernel = f16f8 ? gnn_kernel<1> : gnn_kernel<0>;
+  kernel<<<blocks, GNN_WARPS * 32, 0, stream>>>(h32, row_map, scene_mean, beam, d, hp_plane_stride, cpad_out,
+                                               ch_off_out, NS, g);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;

@@ -21,7 +21,8 @@ constexpr int HEAD_THREADS = 256;
 
 // x block (channels [0,E)) of xh_next for one sample row.
 //   ONEHOT: input is one_hot(amax) (POUT == 1);  else the dense map `vals` [HW][POUT] in smem.
-template <int P, int POUT, bool ONEHOT = (POUT == 1)>
+//   FMT = 1: written in the f16f8 operand format, else as bf16x2 planes.
+template <int FMT, int POUT, bool ONEHOT = (POUT == 1)>
 __device__ __forceinline__ void emb_write(const float* __restrict__ vals, int amax,
                                           const float* __restrict__ We, const float* __restrict__ be,
                                           int E, __nv_bfloat16* __restrict__ xh, long long plane_stride,
@@ -57,31 +58,31 @@ __device__ __forceinline__ void emb_write(const float* __restrict__ vals, int am
           for (int ci = 0; ci < POUT; ++ci) v[c] = fmaf(in[ci], __ldg(We + (tap * POUT + ci) * E + e0 + c), v[c]);
       }
     }
-    if (P == kPlanesF16F8) {      // f16f8 operand format (mvb_common.cuh)
+    if (FMT) {      // f16f8 operand format (mvb_common.cuh)
 #pragma unroll
       for (int c = 0; c < 8; ++c) v[c] = tanhf(v[c]);
       store_f16f8_x8(xh, plane_stride, s * g.S + (long long)y * g.Wp + x, e0, cpad, v);
       continue;
     }
-    uint32_t pk[P][4];
+    uint32_t pk[kBf16Planes][4];
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-      __nv_bfloat16 a[P], b[P];
-      split_planes<P>(tanhf(v[2 * c]), a);
-      split_planes<P>(tanhf(v[2 * c + 1]), b);
+      __nv_bfloat16 a[kBf16Planes], b[kBf16Planes];
+      split_planes(tanhf(v[2 * c]), a);
+      split_planes(tanhf(v[2 * c + 1]), b);
 #pragma unroll
-      for (int q = 0; q < P; ++q) pk[q][c] = pack_bf16x2(a[q], b[q]);
+      for (int q = 0; q < kBf16Planes; ++q) pk[q][c] = pack_bf16x2(a[q], b[q]);
     }
     const long long row = s * g.S + (long long)y * g.Wp + x;
 #pragma unroll
-    for (int q = 0; q < P; ++q)
+    for (int q = 0; q < kBf16Planes; ++q)
       *reinterpret_cast<uint4*>(xh + q * plane_stride + row * cpad + e0) =
           make_uint4(pk[q][0], pk[q][1], pk[q][2], pk[q][3]);
   }
 }
 
 // DENSE_FB (POUT == 1 only): the feedback embeds the logits map itself, not one_hot(argmax)
-template <int P, int POUT, bool DENSE_FB = false>
+template <int FMT, int POUT, bool DENSE_FB = false>
 __global__ void __launch_bounds__(HEAD_THREADS)
 head_kernel(const float* __restrict__ h32, const float* __restrict__ Wo, float* __restrict__ out,
             int* __restrict__ ids_out, const float* __restrict__ We, const float* __restrict__ be,
@@ -223,18 +224,18 @@ head_kernel(const float* __restrict__ h32, const float* __restrict__ Wo, float* 
     __syncthreads();
   }
   // phase 4: embedded feedback input of the next cell step
-  if (xh_next) emb_write<P, POUT, POUT == 1 && !DENSE_FB>(o_s, amax, We, be, E, xh_next, plane_stride, cpad, s, g);
+  if (xh_next) emb_write<FMT, POUT, POUT == 1 && !DENSE_FB>(o_s, amax, We, be, E, xh_next, plane_stride, cpad, s, g);
 }
 
-template <int P>
+template <int FMT>
 __global__ void __launch_bounds__(HEAD_THREADS)
 emb_onehot_kernel(const int* __restrict__ ids, const float* __restrict__ We, const float* __restrict__ be,
                   int E, __nv_bfloat16* __restrict__ xh_next, long long plane_stride, int cpad, Grid g) {
   const long long s = blockIdx.x;
-  emb_write<P, 1>(nullptr, ids[s], We, be, E, xh_next, plane_stride, cpad, s, g);
+  emb_write<FMT, 1>(nullptr, ids[s], We, be, E, xh_next, plane_stride, cpad, s, g);
 }
 
-template <int P>
+template <int FMT>
 __global__ void __launch_bounds__(HEAD_THREADS)
 emb_dense_kernel(const float* __restrict__ x, const float* __restrict__ We, const float* __restrict__ be,
                  int E, __nv_bfloat16* __restrict__ xh_next, long long plane_stride, int cpad, Grid g) {
@@ -243,10 +244,10 @@ emb_dense_kernel(const float* __restrict__ x, const float* __restrict__ We, cons
   const int hw = g.H * g.W;
   for (int i = threadIdx.x; i < hw * 2; i += blockDim.x) sm[i] = x[s * hw * 2 + i];
   __syncthreads();
-  emb_write<P, 2>(sm, 0, We, be, E, xh_next, plane_stride, cpad, s, g);
+  emb_write<FMT, 2>(sm, 0, We, be, E, xh_next, plane_stride, cpad, s, g);
 }
 
-template <int P, int POUT, bool DENSE_FB = false>
+template <int FMT, int POUT, bool DENSE_FB = false>
 static int launch_head(const float* h32, const float* Wo, float* out, int* ids_out, const float* We,
                        const float* be, int E, void* xh_next, long long plane_stride, int cpad,
                        long long NS, const Grid& g, cudaStream_t stream) {
@@ -254,9 +255,9 @@ static int launch_head(const float* h32, const float* Wo, float* out, int* ids_o
   static SmemOptIn opt;
   if (smem > 48 * 1024) {
     MVB_REQUIRE(smem <= 227 * 1024, "head_fwd: grid %dx%d needs %zu B shared memory", g.H, g.W, smem);
-    MVB_CHECK_CUDA(smem_opt_in(opt, head_kernel<P, POUT, DENSE_FB>, smem));
+    MVB_CHECK_CUDA(smem_opt_in(opt, head_kernel<FMT, POUT, DENSE_FB>, smem));
   }
-  head_kernel<P, POUT, DENSE_FB><<<(unsigned)NS, HEAD_THREADS, smem, stream>>>(
+  head_kernel<FMT, POUT, DENSE_FB><<<(unsigned)NS, HEAD_THREADS, smem, stream>>>(
       h32, Wo, out, ids_out, We, be, E, reinterpret_cast<__nv_bfloat16*>(xh_next), plane_stride, cpad, g);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
@@ -266,50 +267,40 @@ static int launch_head(const float* h32, const float* Wo, float* out, int* ids_o
 int head_fwd(const float* h32, const float* Wo, int Pout, float* out, int* ids_out, const float* We,
              const float* be, int E, void* xh_next, long long plane_stride, int cpad, long long NS,
              int H, int W, int P, cudaStream_t stream) {
-  MVB_REQUIRE((P >= 1 && P <= 3) || P == kPlanesF16F8, "head_fwd: planes P=%d", P);
+  MVB_REQUIRE(valid_planes(P), "head_fwd: planes P=%d not 2 or %d", P, kPlanesF16F8);
   MVB_REQUIRE(Pout == 1 || Pout == 2, "head_fwd: Pout=%d", Pout);
   MVB_REQUIRE(h32 && Wo && out && NS > 0, "head_fwd: bad args");
   if (xh_next) MVB_REQUIRE(We && be && E > 0 && E % 8 == 0 && E <= cpad - kHidden && cpad % 8 == 0,
                            "head_fwd: emb needs We/be and E (=%d) a multiple of 8 within the x block", E);
   const Grid g = make_grid(H, W);
-#define MVB_HEAD_CASE(PP, PO) \
-  if (P == PP && Pout == PO) return launch_head<PP, PO>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream);
-  MVB_HEAD_CASE(1, 1) MVB_HEAD_CASE(2, 1) MVB_HEAD_CASE(3, 1)
-  MVB_HEAD_CASE(1, 2) MVB_HEAD_CASE(2, 2) MVB_HEAD_CASE(3, 2)
-  MVB_HEAD_CASE(kPlanesF16F8, 1) MVB_HEAD_CASE(kPlanesF16F8, 2)
-#undef MVB_HEAD_CASE
-  return MVB_ERR_INVALID;
+  if (P == kPlanesF16F8)
+    return Pout == 1 ? launch_head<1, 1>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream)
+                     : launch_head<1, 2>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream);
+  return Pout == 1 ? launch_head<0, 1>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream)
+                   : launch_head<0, 2>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream);
 }
 
 int head_class_fwd_dense(const float* h32, const float* Wo, float* out, int* ids_out, const float* We,
                          const float* be, int E, void* xh_next, long long plane_stride, int cpad, long long NS,
                          int H, int W, int P, cudaStream_t stream) {
-  MVB_REQUIRE(P >= 1 && P <= 3, "head_class_fwd_dense: planes P=%d (training formats only)", P);
+  MVB_REQUIRE(P == kBf16Planes, "head_class_fwd_dense: planes P=%d must be 2 (a training format)", P);
   MVB_REQUIRE(h32 && Wo && out && NS > 0, "head_class_fwd_dense: bad args");
   if (xh_next) MVB_REQUIRE(We && be && E > 0 && E % 8 == 0 && E <= cpad - kHidden && cpad % 8 == 0,
                            "head_class_fwd_dense: emb needs We/be and E (=%d) a multiple of 8 within the x block", E);
   const Grid g = make_grid(H, W);
-  switch (P) {
-    case 1: return launch_head<1, 1, true>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream);
-    case 2: return launch_head<2, 1, true>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream);
-    default: return launch_head<3, 1, true>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream);
-  }
+  return launch_head<0, 1, true>(h32, Wo, out, ids_out, We, be, E, xh_next, plane_stride, cpad, NS, g, stream);
 }
 
 int emb_onehot_fwd(const int* ids, const float* We, const float* be, int E, void* xh_next,
                    long long plane_stride, int cpad, long long NS, int H, int W, int P,
                    cudaStream_t stream) {
-  MVB_REQUIRE((P >= 1 && P <= 3) || P == kPlanesF16F8, "emb_onehot_fwd: planes P=%d", P);
+  MVB_REQUIRE(valid_planes(P), "emb_onehot_fwd: planes P=%d not 2 or %d", P, kPlanesF16F8);
   MVB_REQUIRE(ids && We && be && xh_next && NS > 0 && E > 0 && E % 8 == 0 && E <= cpad - kHidden,
               "emb_onehot_fwd: bad args (E=%d)", E);
   const Grid g = make_grid(H, W);
   __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(xh_next);
-  switch (P) {
-    case 1: emb_onehot_kernel<1><<<(unsigned)NS, HEAD_THREADS, 0, stream>>>(ids, We, be, E, d, plane_stride, cpad, g); break;
-    case 2: emb_onehot_kernel<2><<<(unsigned)NS, HEAD_THREADS, 0, stream>>>(ids, We, be, E, d, plane_stride, cpad, g); break;
-    case kPlanesF16F8: emb_onehot_kernel<kPlanesF16F8><<<(unsigned)NS, HEAD_THREADS, 0, stream>>>(ids, We, be, E, d, plane_stride, cpad, g); break;
-    default: emb_onehot_kernel<3><<<(unsigned)NS, HEAD_THREADS, 0, stream>>>(ids, We, be, E, d, plane_stride, cpad, g); break;
-  }
+  if (P == kPlanesF16F8) emb_onehot_kernel<1><<<(unsigned)NS, HEAD_THREADS, 0, stream>>>(ids, We, be, E, d, plane_stride, cpad, g);
+  else emb_onehot_kernel<0><<<(unsigned)NS, HEAD_THREADS, 0, stream>>>(ids, We, be, E, d, plane_stride, cpad, g);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;
@@ -318,19 +309,15 @@ int emb_onehot_fwd(const int* ids, const float* We, const float* be, int E, void
 int emb_dense_fwd(const float* x, const float* We, const float* be, int E, void* xh_next,
                   long long plane_stride, int cpad, long long NS, int H, int W, int P,
                   cudaStream_t stream) {
-  MVB_REQUIRE((P >= 1 && P <= 3) || P == kPlanesF16F8, "emb_dense_fwd: planes P=%d", P);
+  MVB_REQUIRE(valid_planes(P), "emb_dense_fwd: planes P=%d not 2 or %d", P, kPlanesF16F8);
   MVB_REQUIRE(x && We && be && xh_next && NS > 0 && E > 0 && E % 8 == 0 && E <= cpad - kHidden,
               "emb_dense_fwd: bad args (E=%d)", E);
   const Grid g = make_grid(H, W);
   __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(xh_next);
   const size_t smem = sizeof(float) * (size_t)H * W * 2;
   MVB_REQUIRE(smem <= 48 * 1024, "emb_dense_fwd: grid too large");
-  switch (P) {
-    case 1: emb_dense_kernel<1><<<(unsigned)NS, HEAD_THREADS, smem, stream>>>(x, We, be, E, d, plane_stride, cpad, g); break;
-    case 2: emb_dense_kernel<2><<<(unsigned)NS, HEAD_THREADS, smem, stream>>>(x, We, be, E, d, plane_stride, cpad, g); break;
-    case kPlanesF16F8: emb_dense_kernel<kPlanesF16F8><<<(unsigned)NS, HEAD_THREADS, smem, stream>>>(x, We, be, E, d, plane_stride, cpad, g); break;
-    default: emb_dense_kernel<3><<<(unsigned)NS, HEAD_THREADS, smem, stream>>>(x, We, be, E, d, plane_stride, cpad, g); break;
-  }
+  if (P == kPlanesF16F8) emb_dense_kernel<1><<<(unsigned)NS, HEAD_THREADS, smem, stream>>>(x, We, be, E, d, plane_stride, cpad, g);
+  else emb_dense_kernel<0><<<(unsigned)NS, HEAD_THREADS, smem, stream>>>(x, We, be, E, d, plane_stride, cpad, g);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;

@@ -80,15 +80,11 @@ int beam_nll(const float* logits, const float* logprobs, const int* gt_idx, cons
 // mvb_train.cu
 int cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, long long NS, int H, int W,
                int cpad, int P, int need_x, cudaStream_t stream);
-int cell_wgrad(const void* dgT_planes, const void* xhT_planes, float* dwp, long long NS, int H, int W,
-               int cpad, long long Rp, int P, cudaStream_t stream);
 int cell_wgrad_mn(const void* dg_planes, const void* xh_planes, float* dwp, long long NS, int H, int W,
                   int cpad, int P, cudaStream_t stream);
 int lstm_gates_bwd(const float* gates, const float* c_prev, const float* c_new, const float* dh,
                    const float* dc_in, void* dg_planes, long long plane_stride, float* dc_prev,
                    float* dbias_packed, long long NS, int H, int W, int P, cudaStream_t stream);
-int transpose_planes(const void* src, void* dst, long long R, int C, long long Rp, int P, int taps,
-                     int Wp, cudaStream_t stream);
 int pack_cell_weights_dgrad(const float* kernel, void* wd_planes, int cx, int P, cudaStream_t stream);
 int unpack_cell_wgrad(const float* dwp, const float* dbias_packed, float* dkernel, float* dbiases,
                       int cx, int comp, int accumulate, int slabs, cudaStream_t stream);

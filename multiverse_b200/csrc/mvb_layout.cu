@@ -6,8 +6,8 @@
 
 namespace mvb {
 
-// One thread per (pixel, channel); channel fastest so reads and writes coalesce.
-template <int P>
+// One thread per (pixel, channel); channel fastest so reads and writes coalesce.  FMT = 1: f16f8 operand format.
+template <int FMT>
 __global__ void nhwc_to_planes_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst,
                                       long long plane_stride, int cpad, int ch_off, long long NS,
                                       Grid g, int C, int comp) {
@@ -22,32 +22,29 @@ __global__ void nhwc_to_planes_kernel(const float* __restrict__ src, __nv_bfloat
     const long long s = t / g.H;
     const long long row = s * g.S + (long long)y * g.Wp + x;
     const float v = src[i];
-    if (P == kPlanesF16F8) {      // f16f8 operand format (mvb_common.cuh)
+    if (FMT) {      // f16f8 operand format (mvb_common.cuh)
       store_f16f8(dst, plane_stride, row, ch_off + c, cpad, v);
       continue;
     }
-    __nv_bfloat16 pl[P];
-    split_planes<P>(v, pl);
+    __nv_bfloat16 pl[kBf16Planes];
+    split_planes(v, pl);
     __nv_bfloat16* d = dst + row * cpad + ch_off + c;
-#pragma unroll
-    for (int p = 0; p < P; ++p) d[p * plane_stride] = pl[p];
-    if (comp && P == 2) {
+    d[0] = pl[0];
+    d[plane_stride] = pl[1];
+    if (comp) {
       // Compensated x block for large-magnitude inputs (the regression encoder is fed raw pixel
       // offsets up to ~1.9e3, code/pred_models.py:232): the padded channels carry the terms the
       // 3-product plane scheme drops, so the MMA itself restores fp32-grade accuracy:
       //   A: [x | r=x-x0-x1 | x | x1]   B: [W | W | W-w0-w1 | w1]   (pack_weights_kernel)
-      float r = v;
-#pragma unroll
-      for (int p = 0; p < P; ++p) r -= __bfloat162float(pl[p]);
-      __nv_bfloat16 rp[P];
-      split_planes<P>(r, rp);
-#pragma unroll
-      for (int p = 0; p < P; ++p) {
-        d[p * plane_stride + C] = rp[p];
-        d[p * plane_stride + 2 * C] = pl[p];
-      }
-      d[3 * C] = pl[P - 1];
-      d[(P - 1) * plane_stride + 3 * C] = __float2bfloat16_rn(0.f);
+      const float r = (v - __bfloat162float(pl[0])) - __bfloat162float(pl[1]);
+      __nv_bfloat16 rp[kBf16Planes];
+      split_planes(r, rp);
+      d[C] = rp[0];
+      d[plane_stride + C] = rp[1];
+      d[2 * C] = pl[0];
+      d[plane_stride + 2 * C] = pl[1];
+      d[3 * C] = pl[1];
+      d[plane_stride + 3 * C] = __float2bfloat16_rn(0.f);
     }
   }
 }
@@ -73,7 +70,7 @@ __global__ void nhwc_halo_copy_kernel(const float* __restrict__ src, float* __re
 }
 
 // One block of 64 threads per sample row: thread c handles scene channel c.
-template <int P>
+template <int FMT>
 __global__ void enc_class_input_kernel(const float* __restrict__ scene_conv,
                                        const int* __restrict__ frame_idx,
                                        const int* __restrict__ label,
@@ -87,10 +84,12 @@ __global__ void enc_class_input_kernel(const float* __restrict__ scene_conv,
     const int pl = prev_label[s];
     if (pl >= 0 && pl < hw) {
       const long long row = s * g.S + (long long)(pl / g.W) * g.Wp + (pl % g.W);
-      if (P == kPlanesF16F8) store_f16f8(xh, plane_stride, row, c, cpad, 0.f);
-      else
-#pragma unroll
-      for (int p = 0; p < P; ++p) xh[p * plane_stride + row * cpad + c] = __float2bfloat16_rn(0.f);
+      if (FMT) {
+        store_f16f8(xh, plane_stride, row, c, cpad, 0.f);
+      } else {
+        xh[row * cpad + c] = __float2bfloat16_rn(0.f);
+        xh[plane_stride + row * cpad + c] = __float2bfloat16_rn(0.f);
+      }
     }
   }
   __syncthreads();  // same-pixel clear/set ordering inside the block
@@ -98,18 +97,18 @@ __global__ void enc_class_input_kernel(const float* __restrict__ scene_conv,
   if (lb >= 0 && lb < hw) {
     const long long row = s * g.S + (long long)(lb / g.W) * g.Wp + (lb % g.W);
     const float v = scene_conv[((long long)frame_idx[s] * hw + lb) * 64 + c];
-    if (P == kPlanesF16F8) { store_f16f8(xh, plane_stride, row, c, cpad, v); return; }
-    __nv_bfloat16 pl[P];
-    split_planes<P>(v, pl);
-#pragma unroll
-    for (int p = 0; p < P; ++p) xh[p * plane_stride + row * cpad + c] = pl[p];
+    if (FMT) { store_f16f8(xh, plane_stride, row, c, cpad, v); return; }
+    __nv_bfloat16 pl[kBf16Planes];
+    split_planes(v, pl);
+    xh[row * cpad + c] = pl[0];
+    xh[plane_stride + row * cpad + c] = pl[1];
   }
 }
 
 // SimAug multiview_exp 3 (SimAug/code/pred_models.py:616-638): the observed grid class is a mix of two one-hot maps,
 // beta * one_hot(label) + one_hot(label2) * (1 - beta), so two pixels of the x block carry scene features (one, with the
 // fp32 sum of the two weights, when both labels name the same cell).  The x block must be zero on entry.
-template <int P>
+template <int FMT>
 __global__ void enc_class_input_mix_kernel(const float* __restrict__ scene_conv, const int* __restrict__ frame_idx,
                                            const int* __restrict__ label, const int* __restrict__ label2, float beta,
                                            __nv_bfloat16* __restrict__ xh, long long plane_stride, int cpad, Grid g) {
@@ -122,11 +121,11 @@ __global__ void enc_class_input_mix_kernel(const float* __restrict__ scene_conv,
     if (lb < 0 || lb >= hw) return;
     const long long row = s * g.S + (long long)(lb / g.W) * g.Wp + (lb % g.W);
     const float v = scene_conv[((long long)frame_idx[s] * hw + lb) * 64 + c] * wgt;
-    if (P == kPlanesF16F8) { store_f16f8(xh, plane_stride, row, c, cpad, v); return; }
-    __nv_bfloat16 pl[P];
-    split_planes<P>(v, pl);
-#pragma unroll
-    for (int p = 0; p < P; ++p) xh[p * plane_stride + row * cpad + c] = pl[p];
+    if (FMT) { store_f16f8(xh, plane_stride, row, c, cpad, v); return; }
+    __nv_bfloat16 pl[kBf16Planes];
+    split_planes(v, pl);
+    xh[row * cpad + c] = pl[0];
+    xh[plane_stride + row * cpad + c] = pl[1];
   };
   if (l1 == l2) {
     put(l1, w1 + w2);
@@ -139,16 +138,12 @@ __global__ void enc_class_input_mix_kernel(const float* __restrict__ scene_conv,
 int enc_class_input_mix(const float* scene_conv, const int* frame_idx, const int* label, const int* label2, float beta,
                         void* xh_planes, long long plane_stride, int cpad, long long NS, int H, int W, int P,
                         cudaStream_t stream) {
-  MVB_REQUIRE((P >= 1 && P <= 3) || P == kPlanesF16F8, "enc_class_input_mix: planes P=%d", P);
+  MVB_REQUIRE(valid_planes(P), "enc_class_input_mix: planes P=%d not 2 or %d", P, kPlanesF16F8);
   MVB_REQUIRE(scene_conv && frame_idx && label && label2 && xh_planes && NS > 0, "enc_class_input_mix: bad args");
   const Grid g = make_grid(H, W);
   __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(xh_planes);
-  switch (P) {
-    case 1: enc_class_input_mix_kernel<1><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, label2, beta, d, plane_stride, cpad, g); break;
-    case 2: enc_class_input_mix_kernel<2><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, label2, beta, d, plane_stride, cpad, g); break;
-    case kPlanesF16F8: enc_class_input_mix_kernel<kPlanesF16F8><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, label2, beta, d, plane_stride, cpad, g); break;
-    default: enc_class_input_mix_kernel<3><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, label2, beta, d, plane_stride, cpad, g); break;
-  }
+  if (P == kPlanesF16F8) enc_class_input_mix_kernel<1><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, label2, beta, d, plane_stride, cpad, g);
+  else enc_class_input_mix_kernel<0><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, label2, beta, d, plane_stride, cpad, g);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;
@@ -156,20 +151,16 @@ int enc_class_input_mix(const float* scene_conv, const int* frame_idx, const int
 
 int nhwc_to_planes(const float* src, void* dst_planes, long long plane_stride, int cpad, int ch_off,
                    long long NS, int H, int W, int C, int P, int comp, cudaStream_t stream) {
-  MVB_REQUIRE((P >= 1 && P <= 3) || P == kPlanesF16F8, "nhwc_to_planes: planes P=%d", P);
+  MVB_REQUIRE(valid_planes(P), "nhwc_to_planes: planes P=%d not 2 or %d", P, kPlanesF16F8);
   MVB_REQUIRE(src && dst_planes && NS > 0 && C > 0 && ch_off + C <= cpad, "nhwc_to_planes: bad args");
-  MVB_REQUIRE(!comp || (P == 2 && ch_off + 4 * C <= cpad - kHidden), "nhwc_to_planes: compensated block needs planes=2 and 4*C inside the x block");
+  MVB_REQUIRE(!comp || (P == kBf16Planes && ch_off + 4 * C <= cpad - kHidden), "nhwc_to_planes: compensated block needs planes=2 and 4*C inside the x block");
   const Grid g = make_grid(H, W);
   const long long total = NS * H * W * C;
   const int threads = 256;
   const int blocks = (int)((total + threads - 1) / threads < sm_count() * 16 ? (total + threads - 1) / threads : sm_count() * 16);
   __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst_planes);
-  switch (P) {
-    case 1: nhwc_to_planes_kernel<1><<<blocks, threads, 0, stream>>>(src, d, plane_stride, cpad, ch_off, NS, g, C, comp); break;
-    case 2: nhwc_to_planes_kernel<2><<<blocks, threads, 0, stream>>>(src, d, plane_stride, cpad, ch_off, NS, g, C, comp); break;
-    case kPlanesF16F8: nhwc_to_planes_kernel<kPlanesF16F8><<<blocks, threads, 0, stream>>>(src, d, plane_stride, cpad, ch_off, NS, g, C, 0); break;
-    default: nhwc_to_planes_kernel<3><<<blocks, threads, 0, stream>>>(src, d, plane_stride, cpad, ch_off, NS, g, C, comp); break;
-  }
+  if (P == kPlanesF16F8) nhwc_to_planes_kernel<1><<<blocks, threads, 0, stream>>>(src, d, plane_stride, cpad, ch_off, NS, g, C, 0);
+  else nhwc_to_planes_kernel<0><<<blocks, threads, 0, stream>>>(src, d, plane_stride, cpad, ch_off, NS, g, C, comp);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;
@@ -228,16 +219,12 @@ int nhwc_halo_copy(const float* src, float* dst, long long NS, int H, int W, int
 int enc_class_input(const float* scene_conv, const int* frame_idx, const int* label,
                     const int* prev_label, void* xh_planes, long long plane_stride, int cpad,
                     long long NS, int H, int W, int P, cudaStream_t stream) {
-  MVB_REQUIRE((P >= 1 && P <= 3) || P == kPlanesF16F8, "enc_class_input: planes P=%d", P);
+  MVB_REQUIRE(valid_planes(P), "enc_class_input: planes P=%d not 2 or %d", P, kPlanesF16F8);
   MVB_REQUIRE(scene_conv && frame_idx && label && xh_planes && NS > 0, "enc_class_input: bad args");
   const Grid g = make_grid(H, W);
   __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(xh_planes);
-  switch (P) {
-    case 1: enc_class_input_kernel<1><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, prev_label, d, plane_stride, cpad, g); break;
-    case 2: enc_class_input_kernel<2><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, prev_label, d, plane_stride, cpad, g); break;
-    case kPlanesF16F8: enc_class_input_kernel<kPlanesF16F8><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, prev_label, d, plane_stride, cpad, g); break;
-    default: enc_class_input_kernel<3><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, prev_label, d, plane_stride, cpad, g); break;
-  }
+  if (P == kPlanesF16F8) enc_class_input_kernel<1><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, prev_label, d, plane_stride, cpad, g);
+  else enc_class_input_kernel<0><<<(unsigned)NS, 64, 0, stream>>>(scene_conv, frame_idx, label, prev_label, d, plane_stride, cpad, g);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;

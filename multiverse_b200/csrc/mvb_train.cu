@@ -7,12 +7,14 @@
 //                    = one wgmma implicit GEMM  [R, 9*1024] x [9*1024, cpad]   (same halo trick
 //                    as the forward: a tap is a constant row shift of the dG matrix)
 //   cell wgrad       dW[tap, c, g] = sum_r xh[r + shift(tap), c] * dG[r, g]
-//                    = wgmma GEMM  dG^T [1024, R] x xh^T_tap [cpad, R]^T over 9 tap-shifted
-//                    transposes of the activations; 8 x 18 output tiles, each CTA looping over all R rows (K)
-//                    and adding into the fp32 dW accumulator
-// Both GEMMs use the forward kernel's operand-plane scheme (P bf16 planes, products i+j<P) and
-// the same TMA / mbarrier pipeline with register accumulators.  dgrad tiles: two N tiles of cpad/2 when the x
-// block is needed, one N = 256 tile (h block only) when it is not (regression encoder).
+//                    = wgmma GEMM  dG^T [1024, R] x xh_tap [R, cpad] with K = the halo rows: both operands are
+//                    read MN-major straight from the row-major planes (dG [2][R][1024], xh [2][R][cpad]) and the
+//                    tap is a row shift of the TMA box, so no transposed copy exists.  Work items = 8 M tiles of 128
+//                    gate columns x N tiles of (tap, channel) units x k-splits; every (tile, k-split) adds into its
+//                    own fp32 slab of dW, which unpack_cell_wgrad sums (no atomics).
+// Both GEMMs use the forward kernel's bf16x2 operand format (products a0*b0 + a0*b1 + a1*b0) and the same
+// TMA / mbarrier pipeline with register accumulators.  dgrad tiles: two N tiles of cpad/2 when the x block is
+// needed, one N = 256 tile (h block only) when it is not (regression encoder).
 // Algorithmic FLOPs: dgrad = wgrad = forward (2*R*9*cpad*1024 each).
 #include "mvb_common.cuh"
 #include "mvb_kernels.h"
@@ -30,17 +32,17 @@ constexpr int G_B_PLANE = G_MAX_BN * G_BLOCK_K * 2;    // 16 KB (smaller N tiles
 constexpr uint32_t G_SW64_LAYOUT = kSwizzle64B;
 constexpr uint32_t G_SW64_SBO = 512;
 
-enum { MODE_DGRAD = 0, MODE_WGRAD = 1, MODE_WGRAD_MN = 2 };
+enum { MODE_DGRAD = 0, MODE_WGRAD_MN = 1 };
 
-template <int P> struct GemmCfg {
-  static constexpr int A_BYTES = P * G_A_PLANE;
-  static constexpr int STAGE_BYTES = A_BYTES + P * G_B_PLANE;
+struct GemmCfg {
+  static constexpr int A_BYTES = kBf16Planes * G_A_PLANE;
+  static constexpr int STAGE_BYTES = A_BYTES + kBf16Planes * G_B_PLANE;
   static constexpr int STAGES = (227 * 1024 - 2048) / STAGE_BYTES > 8 ? 8 : (227 * 1024 - 2048) / STAGE_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 };
 
 struct GemmParams {
-  float* out;          // dgrad: [R, cpad] fp32;  wgrad: [1024, 9*cpad] fp32 accumulator (+=)
+  float* out;          // dgrad: [R, cpad] fp32;  wgrad: [ksplit][1024, 9*cpad] fp32 accumulator slabs (+=)
   long long R;         // halo rows
   int H, W;
   int cpad, bn;        // N tile
@@ -49,7 +51,7 @@ struct GemmParams {
   int num_kb;          // k-blocks per tile
   long long num_m_tiles;
   int num_n_tiles;
-  // MODE_WGRAD_MN: operands are read MN-major straight from the row-major activations
+  // wgrad: operands are read MN-major straight from the row-major activations
   int ubn, nb;         // channels / 32-channel blocks of one (tap, chunk) unit
   int n_per_tap;       // units per tap (cpad / ubn)
   int upt;             // units per N tile (bn = upt * ubn): two 96-wide units are paired into N = 192
@@ -59,11 +61,11 @@ struct GemmParams {
 };
 
 // BN = N tile (columns of the accumulator).  Warpgroup 0 loads; warpgroups 1 and 2 multiply and store 64 rows each.
-template <int P, int MODE, int BN>
+template <int MODE, int BN>
 __global__ void __launch_bounds__(G_THREADS, 1)
 pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const GemmParams prm) {
-  using Cfg = GemmCfg<P>;
+  using Cfg = GemmCfg;
   constexpr bool MN = MODE == MODE_WGRAD_MN;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -74,7 +76,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   const Grid g = make_grid(prm.H, prm.W);
   const long long num_tiles = prm.num_m_tiles * prm.num_n_tiles;
-  const uint32_t stage_tx = (uint32_t)(Cfg::A_BYTES + P * BN * G_BLOCK_K * 2);
+  const uint32_t stage_tx = (uint32_t)(Cfg::A_BYTES + kBf16Planes * BN * G_BLOCK_K * 2);
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA); prefetch_tmap(&tmB);
@@ -103,11 +105,6 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             tma_load_3d(sa, &tmA, &full_bar[stage], q * G_BLOCK_K, (int)(mt * G_BLOCK_M - shift), 0);
             tma_load_3d(sb, &tmB, &full_bar[stage], tap * kGates + q * G_BLOCK_K,
                         prm.need_x ? ntile * BN : prm.cxp, 0);
-          } else if (MODE == MODE_WGRAD) {
-            // A = dG^T[128 gate rows, 32 halo rows];  B = tap-shifted xh^T[tap][bn channels, 32 halo rows]
-            const int tap = ntile >> 1, half = ntile & 1;
-            tma_load_3d(sa, &tmA, &full_bar[stage], kb * G_BLOCK_K, (int)(mt * G_BLOCK_M), 0);
-            tma_load_3d(sb, &tmB, &full_bar[stage], kb * G_BLOCK_K, tap * prm.cpad + half * BN, 0);
           } else {
             // MN-major: A = dG[32 halo rows (K), 4 blocks of 32 gate columns]; B = `upt` units, each
             // xh[32 halo rows + shift(tap), nb blocks of 32 channels]; ntile = (unit group, k-split)
@@ -119,7 +116,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
               if (u >= prm.n_units) u = prm.n_units - 1;     // odd tail: duplicate, discarded by the epilogue
               const int tap = u / prm.n_per_tap, chunk = u - tap * prm.n_per_tap;
               const int shift = (tap / 3 - 1) * g.Wp + (tap % 3 - 1);
-              for (int p = 0; p < P; ++p)
+              for (int p = 0; p < kBf16Planes; ++p)
                 tma_load_4d(sb + p * (BN * 64) + j * (prm.ubn * 64), &tmB, &full_bar[stage], 0, k0 + shift,
                             chunk * prm.nb, p);
             }
@@ -147,28 +144,28 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
         const uint32_t sb = sa + Cfg::A_BYTES;
         uint32_t accumulate = kb == 0 ? 0u : 1u;
+        // the product of A plane pa and B plane pb over the k-block
+        auto product = [&](int pa, int pb) {
+#pragma unroll
+          for (int k = 0; k < G_BLOCK_K / G_MMA_K; ++k) {
+            uint64_t ad, bd;
+            if (MN) {
+              // one MMA consumes 16 K rows = two 8-row groups (sbo apart) of every 32-wide MN block
+              ad = make_smem_desc(sa + pa * G_A_PLANE + a_wg + k * 2 * prm.sbo, prm.sbo, G_SW64_LAYOUT, prm.lbo);
+              bd = make_smem_desc(sb + pb * b_plane + k * 2 * prm.sbo, prm.sbo, G_SW64_LAYOUT, prm.lbo);
+            } else {
+              ad = make_smem_desc(sa + pa * G_A_PLANE + a_wg + k * G_MMA_K * 2, G_SW64_SBO, G_SW64_LAYOUT);
+              bd = make_smem_desc(sb + pb * b_plane + k * G_MMA_K * 2, G_SW64_SBO, G_SW64_LAYOUT);
+            }
+            wgmma_bf16<BN, MN ? 1 : 0, MN ? 1 : 0>(acc, ad, bd, accumulate);
+            accumulate = 1u;
+          }
+        };
         wgmma_fence_regs(acc);
         wgmma_fence();
-#pragma unroll
-        for (int pa = 0; pa < P; ++pa) {
-#pragma unroll
-          for (int pb = 0; pb < P - pa; ++pb) {
-#pragma unroll
-            for (int k = 0; k < G_BLOCK_K / G_MMA_K; ++k) {
-              uint64_t ad, bd;
-              if (MN) {
-                // one MMA consumes 16 K rows = two 8-row groups (sbo apart) of every 32-wide MN block
-                ad = make_smem_desc(sa + pa * G_A_PLANE + a_wg + k * 2 * prm.sbo, prm.sbo, G_SW64_LAYOUT, prm.lbo);
-                bd = make_smem_desc(sb + pb * b_plane + k * 2 * prm.sbo, prm.sbo, G_SW64_LAYOUT, prm.lbo);
-              } else {
-                ad = make_smem_desc(sa + pa * G_A_PLANE + a_wg + k * G_MMA_K * 2, G_SW64_SBO, G_SW64_LAYOUT);
-                bd = make_smem_desc(sb + pb * b_plane + k * G_MMA_K * 2, G_SW64_SBO, G_SW64_LAYOUT);
-              }
-              wgmma_bf16<BN, MN ? 1 : 0, MN ? 1 : 0>(acc, ad, bd, accumulate);
-              accumulate = 1u;
-            }
-          }
-        }
+        product(0, 0);
+        product(0, 1);
+        product(1, 0);
         wgmma_commit();
         wgmma_fence_regs(acc);
         wgmma_wait<1>();                       // the previous k-block's MMAs have completed: refill its stage
@@ -194,10 +191,6 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             valid = (x < g.W) && (y < g.H);
           }
           dst = prm.out + row * prm.cpad + (prm.need_x ? ntile * BN : prm.cxp);
-        } else if (MODE == MODE_WGRAD) {
-          valid = row < kGates;
-          const int tap = ntile >> 1, half = ntile & 1;
-          dst = prm.out + row * (9LL * prm.cpad) + tap * prm.cpad + half * BN;
         } else {
           valid = row < kGates;
           dst = prm.out + (long long)(ntile % prm.ksplit) * kGates * 9LL * prm.cpad + row * (9LL * prm.cpad);
@@ -216,7 +209,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             d2 = reinterpret_cast<float2*>(dst + tap * prm.cpad + chunk * prm.ubn + (col - ju * prm.ubn));
           }
           float2 o = make_float2(acc[4 * i + 2 * hr], acc[4 * i + 2 * hr + 1]);
-          if (MODE != MODE_DGRAD) { const float2 old = *d2; o.x += old.x; o.y += old.y; }
+          if (MN) { const float2 old = *d2; o.x += old.x; o.y += old.y; }
           *d2 = o;
         }
       }
@@ -230,7 +223,6 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 //   dc_total = dc_in + dh*o*(1-tanh(c)^2);  dG = {di_pre, dj_pre, df_pre, do_pre};  dc_prev = dc_total*f
 // block = 32 channel groups (8 channels each) x 8 rows
 // ----------------------------------------------------------------------------------
-template <int P>
 __global__ void __launch_bounds__(256)
 lstm_bwd_kernel(const float* __restrict__ gates, const float* __restrict__ c_prev,
                 const float* __restrict__ c_new, const float* __restrict__ dh,
@@ -289,17 +281,17 @@ lstm_bwd_kernel(const float* __restrict__ gates, const float* __restrict__ c_pre
     dc4[1] = make_float4(dcp[4], dcp[5], dcp[6], dcp[7]);
 #pragma unroll
     for (int a = 0; a < 4; ++a) {
-      uint32_t pk[P][4];
+      uint32_t pk[kBf16Planes][4];
 #pragma unroll
       for (int v = 0; v < 4; ++v) {
-        __nv_bfloat16 x0[P], x1[P];
-        split_planes<P>(dgv[a][2 * v], x0);
-        split_planes<P>(dgv[a][2 * v + 1], x1);
+        __nv_bfloat16 x0[kBf16Planes], x1[kBf16Planes];
+        split_planes(dgv[a][2 * v], x0);
+        split_planes(dgv[a][2 * v + 1], x1);
 #pragma unroll
-        for (int q = 0; q < P; ++q) pk[q][v] = pack_bf16x2(x0[q], x1[q]);
+        for (int q = 0; q < kBf16Planes; ++q) pk[q][v] = pack_bf16x2(x0[q], x1[q]);
       }
 #pragma unroll
-      for (int q = 0; q < P; ++q)
+      for (int q = 0; q < kBf16Planes; ++q)
         *reinterpret_cast<uint4*>(dg_planes + q * plane_stride + row * kGates + colbase + a * 64) =
             make_uint4(pk[q][0], pk[q][1], pk[q][2], pk[q][3]);
     }
@@ -324,34 +316,7 @@ lstm_bwd_kernel(const float* __restrict__ gates, const float* __restrict__ c_pre
   }
 }
 
-// src [P][R][C] bf16 -> dst [P][T][C][Rp] bf16 (64x64 tiles through shared memory).
-// T == 1: plain transpose.  T == 9: one copy per 3x3 tap with the tap's row shift applied,
-// dst[p][tap][c][r] = src[p][r + shift(tap)][c] (zero outside) - TMA needs 16-byte aligned inner
-// coordinates, so the wgrad GEMM cannot shift along its contiguous K (= row) axis itself.
-__global__ void __launch_bounds__(256)
-transpose_planes_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat16* __restrict__ dst,
-                        long long R, int C, long long Rp, int taps, int Wp) {
-  __shared__ __nv_bfloat16 tile[64][66];
-  const int p = blockIdx.z / taps, tap = blockIdx.z % taps;
-  const long long shift = taps == 9 ? (long long)(tap / 3 - 1) * Wp + (tap % 3 - 1) : 0;
-  const long long r0 = (long long)blockIdx.x * 64;
-  const int c0 = blockIdx.y * 64;
-  const __nv_bfloat16* s = src + (long long)p * R * C;
-  __nv_bfloat16* d = dst + ((long long)p * taps + tap) * C * Rp;
-  for (int i = threadIdx.x; i < 64 * 64; i += 256) {
-    const int rr = i / 64, cc = i % 64;
-    const long long sr = r0 + rr + shift;
-    tile[rr][cc] = (sr >= 0 && sr < R && c0 + cc < C) ? s[sr * C + c0 + cc] : __float2bfloat16_rn(0.f);
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < 64 * 64; i += 256) {
-    const int cc = i / 64, rr = i % 64;
-    if (c0 + cc < C && r0 + rr < Rp) d[(long long)(c0 + cc) * Rp + r0 + rr] = tile[rr][cc];
-  }
-}
-
-// dgrad weights: Wd planes [P][cpad][9*1024], Wd[kc][tap*1024 + n_packed] = W_tf[tap][cin(kc)][col(n_packed)]
-template <int P>
+// dgrad weights: Wd planes [2][cpad][9*1024], Wd[kc][tap*1024 + n_packed] = W_tf[tap][cin(kc)][col(n_packed)]
 __global__ void pack_dgrad_kernel(const float* __restrict__ kernel, __nv_bfloat16* __restrict__ wd,
                                   int cx, int cxp, int cpad) {
   const long long ktot = 9LL * kGates;
@@ -367,10 +332,10 @@ __global__ void pack_dgrad_kernel(const float* __restrict__ kernel, __nv_bfloat1
     if (kc < cx) cin = kc;
     else if (kc >= cxp) cin = cx + (kc - cxp);
     const float v = (cin >= 0) ? kernel[((long long)tap * (cx + kHidden) + cin) * kGates + col] : 0.f;
-    __nv_bfloat16 pl[P];
-    split_planes<P>(v, pl);
-#pragma unroll
-    for (int p = 0; p < P; ++p) wd[(long long)p * total + i] = pl[p];
+    __nv_bfloat16 pl[kBf16Planes];
+    split_planes(v, pl);
+    wd[i] = pl[0];
+    wd[total + i] = pl[1];
   }
 }
 
@@ -399,32 +364,18 @@ __global__ void unpack_wgrad_kernel(const float* __restrict__ dwp, const float* 
   }
 }
 
-template <int P, int MODE, int BN>
-static int launch_pgemm_n(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& prm, int num_sms,
-                          cudaStream_t stream) {
-  using Cfg = GemmCfg<P>;
+template <int MODE, int BN>
+static int launch_pgemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& prm, int num_sms,
+                        cudaStream_t stream) {
+  using Cfg = GemmCfg;
   static SmemOptIn opt;
-  MVB_CHECK_CUDA(smem_opt_in(opt, pgemm_kernel<P, MODE, BN>, Cfg::SMEM_BYTES));
+  MVB_CHECK_CUDA(smem_opt_in(opt, pgemm_kernel<MODE, BN>, Cfg::SMEM_BYTES));
   const long long tiles = prm.num_m_tiles * prm.num_n_tiles;
   const int grid = (int)(tiles < num_sms ? tiles : num_sms);
-  pgemm_kernel<P, MODE, BN><<<grid, G_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, prm);
+  pgemm_kernel<MODE, BN><<<grid, G_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, prm);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;
-}
-
-// the N tiles the three GEMMs use: cpad / 2 (144, 160), 192 (two 96-wide units) and 256
-template <int P, int MODE>
-static int launch_pgemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& prm, int num_sms,
-                        cudaStream_t stream) {
-  switch (prm.bn) {
-    case 144: return launch_pgemm_n<P, MODE, 144>(tmA, tmB, prm, num_sms, stream);
-    case 160: return launch_pgemm_n<P, MODE, 160>(tmA, tmB, prm, num_sms, stream);
-    case 192: return launch_pgemm_n<P, MODE, 192>(tmA, tmB, prm, num_sms, stream);
-    case 256: return launch_pgemm_n<P, MODE, 256>(tmA, tmB, prm, num_sms, stream);
-    default: MVB_REQUIRE(false, "pgemm: N tile %d unsupported", prm.bn);
-  }
-  return MVB_ERR_INVALID;
 }
 
 static int num_sms_of_device(int* out) {
@@ -436,21 +387,21 @@ static int num_sms_of_device(int* out) {
 
 int cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, long long NS, int H, int W,
                int cpad, int P, int need_x, cudaStream_t stream) {
-  MVB_REQUIRE(P >= 1 && P <= 3, "cell_dgrad: planes P=%d", P);
+  MVB_REQUIRE(P == kBf16Planes, "cell_dgrad: planes P=%d must be 2 (the bf16x2 format)", P);
   MVB_REQUIRE(dg_planes && wd_planes && dxh && NS > 0, "cell_dgrad: bad args");
+  MVB_REQUIRE(cpad == 288 || cpad == 320, "cell_dgrad: cpad=%d unsupported", cpad);
   const int cxp = cpad - kHidden;
-  MVB_REQUIRE(cpad % 32 == 0 && cxp >= 32 && cxp <= 256 && cxp % 16 == 0, "cell_dgrad: cpad=%d unsupported", cpad);
   const Grid g = make_grid(H, W);
   const long long R = NS * g.S;
   CUtensorMap tmA, tmB;
-  int rc = encode_tmap_3d_bf16(&tmA, dg_planes, kGates, (uint64_t)R, P, kGates * 2ull, (uint64_t)R * kGates * 2,
-                               G_BLOCK_K, G_BLOCK_M, P, 64);
+  int rc = encode_tmap_3d_bf16(&tmA, dg_planes, kGates, (uint64_t)R, kBf16Planes, kGates * 2ull,
+                               (uint64_t)R * kGates * 2, G_BLOCK_K, G_BLOCK_M, kBf16Planes, 64);
   if (rc) return rc;
   const uint64_t ktot = 9ull * kGates;
   // with the x block: two N tiles of cpad/2 (144 / 160); h only: one N tile of 256
   const int bn = need_x ? cpad / 2 : 256;
-  MVB_REQUIRE(bn % 16 == 0, "cell_dgrad: cpad=%d unsupported", cpad);
-  rc = encode_tmap_3d_bf16(&tmB, wd_planes, ktot, (uint64_t)cpad, P, ktot * 2, ktot * cpad * 2, G_BLOCK_K, bn, P, 64);
+  rc = encode_tmap_3d_bf16(&tmB, wd_planes, ktot, (uint64_t)cpad, kBf16Planes, ktot * 2, ktot * cpad * 2, G_BLOCK_K,
+                           bn, kBf16Planes, 64);
   if (rc) return rc;
   GemmParams prm = {};
   prm.out = dxh; prm.R = R; prm.H = H; prm.W = W; prm.cpad = cpad; prm.bn = bn; prm.cxp = cxp; prm.need_x = need_x;
@@ -459,45 +410,16 @@ int cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, long lo
   prm.num_n_tiles = need_x ? 2 : 1;
   int sms = 0;
   if ((rc = num_sms_of_device(&sms))) return rc;
-  switch (P) {
-    case 1: return launch_pgemm<1, MODE_DGRAD>(tmA, tmB, prm, sms, stream);
-    case 2: return launch_pgemm<2, MODE_DGRAD>(tmA, tmB, prm, sms, stream);
-    default: return launch_pgemm<3, MODE_DGRAD>(tmA, tmB, prm, sms, stream);
-  }
-}
-
-int cell_wgrad(const void* dgT_planes, const void* xhT_planes, float* dwp, long long NS, int H, int W,
-               int cpad, long long Rp, int P, cudaStream_t stream) {
-  MVB_REQUIRE(P >= 1 && P <= 3, "cell_wgrad: planes P=%d", P);
-  MVB_REQUIRE(dgT_planes && xhT_planes && dwp && NS > 0, "cell_wgrad: bad args");
-  MVB_REQUIRE(cpad % 32 == 0 && (cpad / 2) % 16 == 0 && cpad / 2 <= G_MAX_BN, "cell_wgrad: cpad=%d unsupported", cpad);
-  const Grid g = make_grid(H, W);
-  const long long R = NS * g.S;
-  MVB_REQUIRE(Rp >= R && Rp % 8 == 0, "cell_wgrad: Rp=%lld must be >= R and a multiple of 8", Rp);
-  CUtensorMap tmA, tmB;
-  int rc = encode_tmap_3d_bf16(&tmA, dgT_planes, (uint64_t)R, kGates, P, (uint64_t)Rp * 2, (uint64_t)Rp * kGates * 2,
-                               G_BLOCK_K, G_BLOCK_M, P, 64);
-  if (rc) return rc;
-  rc = encode_tmap_3d_bf16(&tmB, xhT_planes, (uint64_t)R, 9ull * cpad, P, (uint64_t)Rp * 2, (uint64_t)Rp * cpad * 18,
-                           G_BLOCK_K, cpad / 2, P, 64);
-  if (rc) return rc;
-  GemmParams prm = {};
-  prm.out = dwp; prm.R = R; prm.H = H; prm.W = W; prm.cpad = cpad; prm.bn = cpad / 2;
-  prm.num_kb = (int)((R + G_BLOCK_K - 1) / G_BLOCK_K); prm.num_m_tiles = kGates / G_BLOCK_M; prm.num_n_tiles = 18;
-  int sms = 0;
-  if ((rc = num_sms_of_device(&sms))) return rc;
-  switch (P) {
-    case 1: return launch_pgemm<1, MODE_WGRAD>(tmA, tmB, prm, sms, stream);
-    case 2: return launch_pgemm<2, MODE_WGRAD>(tmA, tmB, prm, sms, stream);
-    default: return launch_pgemm<3, MODE_WGRAD>(tmA, tmB, prm, sms, stream);
-  }
+  if (!need_x) return launch_pgemm<MODE_DGRAD, 256>(tmA, tmB, prm, sms, stream);
+  return cpad == 288 ? launch_pgemm<MODE_DGRAD, 144>(tmA, tmB, prm, sms, stream)
+                     : launch_pgemm<MODE_DGRAD, 160>(tmA, tmB, prm, sms, stream);
 }
 
 int cell_wgrad_mn_slabs(int cpad) { return cpad == 288 ? 5 : 2; }
 
 int cell_wgrad_mn(const void* dg_planes, const void* xh_planes, float* dwp, long long NS, int H, int W,
                   int cpad, int P, cudaStream_t stream) {
-  MVB_REQUIRE(P >= 1 && P <= 3, "cell_wgrad_mn: planes P=%d", P);
+  MVB_REQUIRE(P == kBf16Planes, "cell_wgrad_mn: planes P=%d must be 2 (the bf16x2 format)", P);
   MVB_REQUIRE(dg_planes && xh_planes && dwp && NS > 0, "cell_wgrad_mn: bad args");
   MVB_REQUIRE(cpad == 288 || cpad == 320, "cell_wgrad_mn: cpad=%d unsupported", cpad);
   const Grid g = make_grid(H, W);
@@ -509,14 +431,14 @@ int cell_wgrad_mn(const void* dg_planes, const void* xh_planes, float* dwp, long
   prm.nb = prm.ubn / 32; prm.n_per_tap = cpad / prm.ubn; prm.n_units = 9 * prm.n_per_tap;
   CUtensorMap tmA, tmB;
   {
-    const uint64_t dims[4] = {32, (uint64_t)R, kGates / 32, (uint64_t)P};
+    const uint64_t dims[4] = {32, (uint64_t)R, kGates / 32, (uint64_t)kBf16Planes};
     const uint64_t st[3] = {kGates * 2ull, 64, (uint64_t)R * kGates * 2};
-    const uint32_t box[4] = {32, G_BLOCK_K, 4, (uint32_t)P};      // 128 gate columns per CTA tile
+    const uint32_t box[4] = {32, G_BLOCK_K, 4, (uint32_t)kBf16Planes};      // 128 gate columns per CTA tile
     int rc = encode_tmap_4d_bf16(&tmA, dg_planes, dims, st, box, 64);
     if (rc) return rc;
   }
   {
-    const uint64_t dims[4] = {32, (uint64_t)R, (uint64_t)cpad / 32, (uint64_t)P};
+    const uint64_t dims[4] = {32, (uint64_t)R, (uint64_t)cpad / 32, (uint64_t)kBf16Planes};
     const uint64_t st[3] = {(uint64_t)cpad * 2, 64, (uint64_t)R * cpad * 2};
     const uint32_t box[4] = {32, G_BLOCK_K, (uint32_t)prm.nb, 1};
     int rc = encode_tmap_4d_bf16(&tmB, xh_planes, dims, st, box, 64);
@@ -535,52 +457,33 @@ int cell_wgrad_mn(const void* dg_planes, const void* xh_planes, float* dwp, long
   int sms = 0;
   int rc = num_sms_of_device(&sms);
   if (rc) return rc;
-  switch (P) {
-    case 1: return launch_pgemm<1, MODE_WGRAD_MN>(tmA, tmB, prm, sms, stream);
-    case 2: return launch_pgemm<2, MODE_WGRAD_MN>(tmA, tmB, prm, sms, stream);
-    default: return launch_pgemm<3, MODE_WGRAD_MN>(tmA, tmB, prm, sms, stream);
-  }
+  // N tile: two 96-wide units (cpad 288) or one 160-wide unit (cpad 320)
+  return prm.bn == 192 ? launch_pgemm<MODE_WGRAD_MN, 192>(tmA, tmB, prm, sms, stream)
+                       : launch_pgemm<MODE_WGRAD_MN, 160>(tmA, tmB, prm, sms, stream);
 }
 
 int lstm_gates_bwd(const float* gates, const float* c_prev, const float* c_new, const float* dh,
                    const float* dc_in, void* dg_planes, long long plane_stride, float* dc_prev,
                    float* dbias_packed, long long NS, int H, int W, int P, cudaStream_t stream) {
-  MVB_REQUIRE(P >= 1 && P <= 3, "lstm_gates_bwd: planes P=%d", P);
+  MVB_REQUIRE(P == kBf16Planes, "lstm_gates_bwd: planes P=%d must be 2 (the bf16x2 format)", P);
   MVB_REQUIRE(gates && c_new && dh && dg_planes && dc_prev && dbias_packed && NS > 0, "lstm_gates_bwd: bad args");
   const Grid g = make_grid(H, W);
   const long long pix = NS * H * W;
   const int blocks = (int)((pix + 7) / 8 < sm_count() * 8 ? (pix + 7) / 8 : sm_count() * 8);
   __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dg_planes);
-  switch (P) {
-    case 1: lstm_bwd_kernel<1><<<blocks, 256, 0, stream>>>(gates, c_prev, c_new, dh, dc_in, d, plane_stride, dc_prev, dbias_packed, NS, g); break;
-    case 2: lstm_bwd_kernel<2><<<blocks, 256, 0, stream>>>(gates, c_prev, c_new, dh, dc_in, d, plane_stride, dc_prev, dbias_packed, NS, g); break;
-    default: lstm_bwd_kernel<3><<<blocks, 256, 0, stream>>>(gates, c_prev, c_new, dh, dc_in, d, plane_stride, dc_prev, dbias_packed, NS, g); break;
-  }
-  MVB_CHECK_CUDA(cudaGetLastError());
-  count_launch(1);
-  return MVB_OK;
-}
-
-int transpose_planes(const void* src, void* dst, long long R, int C, long long Rp, int P, int taps,
-                     int Wp, cudaStream_t stream) {
-  MVB_REQUIRE(src && dst && R > 0 && C > 0 && Rp >= R && P >= 1 && (taps == 1 || taps == 9), "transpose_planes: bad args");
-  dim3 grid((unsigned)((Rp + 63) / 64), (unsigned)((C + 63) / 64), (unsigned)(P * taps));
-  transpose_planes_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(src),
-                                                    reinterpret_cast<__nv_bfloat16*>(dst), R, C, Rp, taps, Wp);
+  lstm_bwd_kernel<<<blocks, 256, 0, stream>>>(gates, c_prev, c_new, dh, dc_in, d, plane_stride, dc_prev, dbias_packed,
+                                              NS, g);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;
 }
 
 int pack_cell_weights_dgrad(const float* kernel, void* wd_planes, int cx, int P, cudaStream_t stream) {
-  MVB_REQUIRE(P >= 1 && P <= 3 && kernel && wd_planes && cx >= 1, "pack_cell_weights_dgrad: bad args");
+  MVB_REQUIRE(P == kBf16Planes, "pack_cell_weights_dgrad: planes P=%d must be 2 (the bf16x2 format)", P);
+  MVB_REQUIRE(kernel && wd_planes && cx >= 1, "pack_cell_weights_dgrad: bad args");
   const int cxp = (cx + 31) / 32 * 32, cpad = cxp + kHidden;
   __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(wd_planes);
-  switch (P) {
-    case 1: pack_dgrad_kernel<1><<<1184, 256, 0, stream>>>(kernel, d, cx, cxp, cpad); break;
-    case 2: pack_dgrad_kernel<2><<<1184, 256, 0, stream>>>(kernel, d, cx, cxp, cpad); break;
-    default: pack_dgrad_kernel<3><<<1184, 256, 0, stream>>>(kernel, d, cx, cxp, cpad); break;
-  }
+  pack_dgrad_kernel<<<1184, 256, 0, stream>>>(kernel, d, cx, cxp, cpad);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;

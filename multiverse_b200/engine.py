@@ -20,8 +20,6 @@ the next GNN / cell launch reads its state through.
 """
 from __future__ import annotations
 
-import os
-
 import torch
 
 from . import ops
@@ -86,19 +84,19 @@ class ConvRNNEngine(object):
   GRAPH_CACHE = 4             # captured forward graphs kept per engine
   ALLOW_F16F8 = True          # TrainEngine: False (its packed weights also feed the bf16 backward GEMMs)
 
-  def __init__(self, cfg, weights, device=None, planes=None):
+  def __init__(self, cfg, weights, device=None, planes=ops.PLANES_BF16X2):
+    assert planes == ops.PLANES_BF16X2, \
+        "planes=%r: the engines run the bf16x2 operand format (planes=2), with f16f8 where inference allows" % (planes,)
     self.cfg = cfg
     self.device = device or torch.device("cuda", torch.cuda.current_device())
-    self.planes = planes or ops.DEFAULT_PLANES
+    self.planes = planes
     # The class decoder's cell reads only what the graph attention writes (its one-hot input is folded into table
-    # look-ups), so that producer/consumer pair switches to the f16f8 operand format as a unit; MVB_F16F8=0 keeps
-    # bf16 planes everywhere (A/B runs and the round-1 numbers).
-    self.fast_class = (self.ALLOW_F16F8 and bool(cfg.use_gnn) and self.planes == 2 and
-                       os.environ.get("MVB_F16F8", "1") != "0")
+    # look-ups), so that producer/consumer pair switches to the f16f8 operand format as a unit.
+    self.fast_class = self.ALLOW_F16F8 and bool(cfg.use_gnn)
     self.class_planes = ops.PLANES_F16F8 if self.fast_class else self.planes
     # class encoder and regression decoder (inputs in (-1,1): tanh outputs) use the same format; the regression
     # ENCODER keeps bf16 planes: its raw pixel offsets (+-1.9e3) need the compensated x block.
-    self.fast = self.ALLOW_F16F8 and self.planes == 2 and os.environ.get("MVB_F16F8", "1") != "0"
+    self.fast = self.ALLOW_F16F8
     self.fast_planes = ops.PLANES_F16F8 if self.fast else self.planes
     assert cfg.enc_hidden_size == ops.HIDDEN and cfg.dec_hidden_size == ops.HIDDEN, \
         "the kernels are specialised for hidden size 256 (every published config)"
@@ -202,7 +200,7 @@ class ConvRNNEngine(object):
     xh = self._xh("enc_class", n, h, w, sw.enc_class.cpad, self.fast_planes)
     c = [self._state("enc_c0", n, h, w), self._state("enc_c1", n, h, w)]
     h32 = self._state("enc_h32", n, h, w)
-    if sw.enc_class_xs is not None and os.environ.get("MVB_ENC_XSPARSE", "1") != "0":
+    if sw.enc_class_xs is not None:
       # (one table per scale: the chains of different scales run concurrently under forward_graph)
       table = self._buf(("enc_class_xtab", n, h, w), lambda: torch.empty((n, 9, 4 * ops.HIDDEN), dtype=torch.float32,
                                                                   device=self.device))
@@ -239,7 +237,7 @@ class ConvRNNEngine(object):
     h, w = self.cfg.scene_grids[i]
     t_len, n = obs_reg_t.shape[0], obs_reg_t.shape[1]
     sw = self.scales[i]
-    if sw.enc_reg_fast is not None and os.environ.get("MVB_REG_XDENSE", "1") != "0":
+    if sw.enc_reg_fast is not None:
       pk = sw.enc_reg_fast
       xh = self._xh("enc_reg_f", n, h, w, pk.cpad, ops.PLANES_F16F8)
       c = [self._state("encr_c0", n, h, w), self._state("encr_c1", n, h, w)]

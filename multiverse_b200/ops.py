@@ -8,15 +8,16 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
 
 import torch
 
 from . import _lib
 
 HIDDEN = 256
-DEFAULT_PLANES = int(os.environ.get("MVB_PLANES", "2"))
-PLANES_F16F8 = 16    # MVB_PLANES_F16F8: one fp16 + two e4m3 planes in the bytes of two bf16 planes (inference)
+# the two operand formats (`planes` codes): two bf16 summands, and MVB_PLANES_F16F8, one fp16 + two e4m3 planes in the
+# bytes of two bf16 planes (inference)
+PLANES_BF16X2 = 2
+PLANES_F16F8 = 16
 
 
 def planes_of(t):
@@ -27,7 +28,7 @@ def planes_of(t):
 def cell_variants_seen(reset=False):
   """Set of (planes, pair) cell-kernel variants launched since the last reset."""
   m = int(_lib.load().mvb_cell_variants_seen(int(bool(reset))))
-  return {((1, 2, 3, PLANES_F16F8)[b // 2], bool(b % 2)) for b in range(8) if m >> b & 1}
+  return {((PLANES_BF16X2, PLANES_F16F8)[b // 2], bool(b % 2)) for b in range(4) if m >> b & 1}
 
 
 def cell_last_variant():
@@ -66,15 +67,14 @@ def reset_launch_count():
 class PackedCell(object):
   """Device-resident packed weights of one ConvLSTM cell (see mvb_pack_cell_weights)."""
 
-  def __init__(self, kernel, biases, planes=None, comp=False):
-    planes = planes or DEFAULT_PLANES
+  def __init__(self, kernel, biases, planes=PLANES_BF16X2, comp=False):
     assert kernel.dim() == 4 and kernel.shape[0] == 3 and kernel.shape[1] == 3
     assert kernel.shape[3] == 4 * HIDDEN
     self.cx = int(kernel.shape[2]) - HIDDEN
     self.cxp = (self.cx + 31) // 32 * 32
     self.cpad = self.cxp + HIDDEN
     self.planes = planes
-    self.comp = bool(comp) and planes == 2 and 4 * self.cx <= self.cxp
+    self.comp = bool(comp) and planes == PLANES_BF16X2 and 4 * self.cx <= self.cxp
     kernel = kernel.detach().to(torch.float32).contiguous()
     biases = biases.detach().to(torch.float32).contiguous()
     if planes == PLANES_F16F8:
@@ -96,12 +96,12 @@ def _planes_arg(packed, xh_next):
 
 
 def alloc_xh(ns, h, w, cpad, planes, device):
-  """Zeroed operand planes [P, R, cpad]; halo cells and channel padding must stay zero."""
+  """Zeroed operand planes [2, R, cpad] (either format: the same bytes); halo cells and channel padding must stay
+  zero."""
+  t = torch.zeros((2, halo_rows(ns, h, w), cpad), dtype=torch.bfloat16, device=device)
   if planes == PLANES_F16F8:
-    t = torch.zeros((2, halo_rows(ns, h, w), cpad), dtype=torch.bfloat16, device=device)   # same bytes
     t.mvb_planes = PLANES_F16F8
-    return t
-  return torch.zeros((planes, halo_rows(ns, h, w), cpad), dtype=torch.bfloat16, device=device)
+  return t
 
 
 def operand_values(xh):
@@ -280,33 +280,33 @@ def gnn_attend_fwd(h32, scene_mean, xh_next, h, w, ns, beam=1, row_map=None):
             planes_of(xh_next), _stream())
 
 
-def head_class_fwd(h32, Wo, logits_out, ids_out, We, be, xh_next, h, w, ns, planes=None):
+def head_class_fwd(h32, Wo, logits_out, ids_out, We, be, xh_next, h, w, ns, planes=PLANES_BF16X2):
   e = 0 if We is None else We.shape[3]
   if xh_next is not None:
     stride, cpad, planes = xh_next.stride(0), xh_next.shape[2], planes_of(xh_next)
   else:
-    stride, cpad, planes = 0, 0, planes or DEFAULT_PLANES
+    stride, cpad = 0, 0
   _lib.call("mvb_head_class_fwd", _p(h32), _p(Wo), _p(logits_out), _p(ids_out), _p(We), _p(be), e,
             _p(xh_next), stride, cpad, ns, h, w, planes, _stream())
 
 
-def head_class_fwd_dense(h32, Wo, logits_out, ids_out, We, be, xh_next, h, w, ns, planes=None):
+def head_class_fwd_dense(h32, Wo, logits_out, ids_out, We, be, xh_next, h, w, ns, planes=PLANES_BF16X2):
   """head_class_fwd whose feedback embeds the logits map itself (training without --train_w_onehot)."""
   e = 0 if We is None else We.shape[3]
   if xh_next is not None:
     stride, cpad, planes = xh_next.stride(0), xh_next.shape[2], planes_of(xh_next)
   else:
-    stride, cpad, planes = 0, 0, planes or DEFAULT_PLANES
+    stride, cpad = 0, 0
   _lib.call("mvb_head_class_fwd_dense", _p(h32), _p(Wo), _p(logits_out), _p(ids_out), _p(We), _p(be), e,
             _p(xh_next), stride, cpad, ns, h, w, planes, _stream())
 
 
-def head_reg_fwd(h32, Wo, off_out, We, be, xh_next, h, w, ns, planes=None):
+def head_reg_fwd(h32, Wo, off_out, We, be, xh_next, h, w, ns, planes=PLANES_BF16X2):
   e = 0 if We is None else We.shape[3]
   if xh_next is not None:
     stride, cpad, planes = xh_next.stride(0), xh_next.shape[2], planes_of(xh_next)
   else:
-    stride, cpad, planes = 0, 0, planes or DEFAULT_PLANES
+    stride, cpad = 0, 0
   _lib.call("mvb_head_reg_fwd", _p(h32), _p(Wo), _p(off_out), _p(We), _p(be), e, _p(xh_next),
             stride, cpad, ns, h, w, planes, _stream())
 
@@ -364,20 +364,9 @@ def lstm_gates_bwd(gates, c_prev, c_new, dh, dc_in, dg_planes, dc_prev, dbias_pa
             dg_planes.shape[0], _stream())
 
 
-def transpose_planes(src, dst, taps=1, w=0):
-  """src [P,R,C] -> dst [P,C,Rp] (taps=1) or [P,9,C,Rp] (taps=9, tap-shifted copies)."""
-  p, r, c = src.shape
-  _lib.call("mvb_transpose_planes", _p(src), _p(dst), r, c, dst.shape[-1], p, taps, w, _stream())
-
-
 def cell_dgrad(dg_planes, wd, dxh, h, w, ns, need_dx=True):
   _lib.call("mvb_cell_dgrad", _p(dg_planes), _p(wd), _p(dxh), ns, h, w, dxh.shape[1],
             dg_planes.shape[0], int(need_dx), _stream())
-
-
-def cell_wgrad(dgT, xhT, dw_packed, h, w, ns):
-  _lib.call("mvb_cell_wgrad", _p(dgT), _p(xhT), _p(dw_packed), ns, h, w, xhT.shape[2],
-            xhT.shape[3], dgT.shape[0], _stream())
 
 
 def cell_wgrad_direct(dg_planes, xh, dw_packed, h, w, ns):

@@ -47,7 +47,7 @@ class TrainEngine(ConvRNNEngine):
   update."""
   ALLOW_F16F8 = False
 
-  def __init__(self, cfg, weights, device=None, planes=None):
+  def __init__(self, cfg, weights, device=None, planes=ops.PLANES_BF16X2):
     super(TrainEngine, self).__init__(cfg, weights, device, planes)
     assert not cfg.use_beam_search, "beam search is inference-only (code/pred_models.py:261)"
     dev = self.device

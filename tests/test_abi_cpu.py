@@ -64,6 +64,39 @@ def test_argument_validation_needs_no_gpu(lib):
   assert rc != 0 and b"beam_step" in lib.mvb_last_error()
 
 
+def planes_entry_points():
+  """name -> parameter names of every header function that takes a `planes` argument."""
+  src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "multiverse_b200.h")).read(), flags=re.S)
+  out = {}
+  for name, params in re.findall(r"\bint\s+(mvb_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", src):
+    names = [p.split()[-1].lstrip("*") for p in params.split(",")]
+    if "planes" in names:
+      out[name] = names
+  return out
+
+
+@pytest.mark.parametrize("planes", [1, 3, 2 | 3 << 8])
+def test_only_two_operand_formats(lib, planes):
+  """planes 2 (bf16x2) and MVB_PLANES_F16F8 are the only operand formats: any other code - including an output format
+  of 3 planes in the `planes | out << 8` form of the cell entry points - is refused before any CUDA call."""
+  eps = planes_entry_points()
+  assert len(eps) == 20 and "mvb_convlstm_cell_fwd" in eps and "mvb_cell_wgrad_direct" in eps
+  from multiverse_b200 import _lib
+  for name, params in sorted(eps.items()):
+    if planes >> 8 and not name.startswith("mvb_convlstm_cell_fwd"):
+      continue
+    args = []
+    for pname, ty in zip(params, _lib.SIGNATURES[name]):
+      if pname == "planes":
+        args.append(planes)
+      elif ty is ctypes.c_void_p:      # never dereferenced: the call must return first
+        args.append(None if pname == "stream" else ctypes.c_void_p(256))
+      else:
+        args.append(ty(1))
+    rc = getattr(lib, name)(*args)
+    assert rc != 0 and b"planes" in lib.mvb_last_error(), (name, lib.mvb_last_error())
+
+
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):
   from multiverse_b200 import _lib
   monkeypatch.setattr(_lib, "_lib", None)

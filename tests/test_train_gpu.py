@@ -33,7 +33,7 @@ def T(a, dev):
 
 
 @pytest.mark.parametrize("name", ["dec_cx32", "enc_class_cx64", "tile_edge", "enc_reg_cx2"])
-def test_cell_backward_matches_autograd(dev, name):
+def test_cell_backward_with_direct_wgrad_matches_autograd(dev, name):
   from multiverse_b200 import ops
   d = cases.cell_case(name)
   ns, h, w, cx = d["x"].shape
@@ -72,27 +72,27 @@ def test_cell_backward_matches_autograd(dev, name):
   assert rel(dxh_v[..., pk.cxp:], t["h"].grad.numpy()) < GTOL
   if not comp:
     assert rel(dxh_v[..., :cx], t["x"].grad.numpy()) < GTOL
-  # wgrad
-  Rp = (R + 7) // 8 * 8
-  dgT = torch.zeros((planes, 1024, Rp), dtype=torch.bfloat16, device=dev)
-  xhT = torch.zeros((planes, 9, pk.cpad, Rp), dtype=torch.bfloat16, device=dev)
-  ops.transpose_planes(dg, dgT); ops.transpose_planes(xh, xhT, taps=9, w=w)
-  assert torch.equal(xhT[:, 4, :, :R].transpose(1, 2).contiguous(), xh)
-  assert torch.equal(dgT[:, :, :R].transpose(1, 2).contiguous(), dg)
-  dwp = torch.zeros((1024, 9 * pk.cpad), device=dev)
-  ops.cell_wgrad(dgT, xhT, dwp, h, w, ns)
-  ops.cell_wgrad(dgT, xhT, dwp, h, w, ns)          # accumulates: twice -> 2x
+  # wgrad: MN-major operands straight from the row-major planes; a second run accumulates to exactly 2x
+  dwp = torch.zeros((ops.wgrad_slabs(pk.cpad), 1024, 9 * pk.cpad), device=dev)
+  ops.cell_wgrad_direct(dg, xh, dwp, h, w, ns)
+  dwp1 = dwp.clone()
+  ops.cell_wgrad_direct(dg, xh, dwp, h, w, ns)
+  assert torch.equal(dwp, 2 * dwp1)
   dk = torch.empty((3, 3, cx + 256, 1024), device=dev); db = torch.empty((1024,), device=dev)
   ops.unpack_cell_wgrad(dwp, dbp, dk, db, cx, comp=pk.comp)
   assert rel(0.5 * dk.cpu().numpy(), t["kernel"].grad.numpy()) < GTOL
   assert rel(db.cpu().numpy(), t["biases"].grad.numpy()) < GTOL
-  # the production path: MN-major operands straight from the row-major planes (no transposes)
-  dwp2 = torch.zeros((ops.wgrad_slabs(pk.cpad), 1024, 9 * pk.cpad), device=dev)
-  ops.cell_wgrad_direct(dg, xh, dwp2, h, w, ns)
-  assert rel(dwp2.sum(0).cpu().numpy(), 0.5 * dwp.cpu().numpy()) < 1e-5
-  dk2 = torch.empty_like(dk); db2 = torch.empty_like(db)
-  ops.unpack_cell_wgrad(dwp2, dbp, dk2, db2, cx, comp=pk.comp)
-  assert rel(dk2.cpu().numpy(), t["kernel"].grad.numpy()) < GTOL
+  # the same bf16 planes the kernel multiplies, in fp64: a0b0 + a0b1 + a1b0 per tap shift of the activation rows
+  ref = torch.zeros((1024, 9 * pk.cpad), dtype=torch.float64, device=dev)
+  for tap in range(9):
+    shift = (tap // 3 - 1) * (w + 1) + (tap % 3 - 1)
+    xs = torch.zeros((2, R, pk.cpad), dtype=torch.float64, device=dev)
+    lo, hi = max(0, -shift), min(R, R - shift)
+    xs[:, lo:hi] = xh[:, lo + shift:hi + shift].double()
+    ref[:, tap * pk.cpad:(tap + 1) * pk.cpad] = sum(dg[a].double().t() @ xs[b] for a, b in ((0, 0), (0, 1), (1, 0)))
+  err = rel(dwp1.sum(0).double().cpu().numpy(), ref.cpu().numpy())
+  print("cell %s: wgrad against the fp64 product of its bf16 planes: rel err %.2e" % (name, err))
+  assert err < 1e-5
 
 
 def test_loss_kernel(dev):

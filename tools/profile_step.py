@@ -12,7 +12,6 @@ from multiverse_b200.engine import ConvRNNEngine
 ap = argparse.ArgumentParser()
 ap.add_argument("--workload", default="c4")
 ap.add_argument("--global-batch", type=int, default=128)
-ap.add_argument("--planes", type=int, default=2)
 a = ap.parse_args()
 wl = bench.WORKLOADS[a.workload]
 cfg = synthetic.make_config(batch_size=a.global_batch, **wl["cfg"])
@@ -22,7 +21,7 @@ f = synthetic.make_feeds(cfg, a.global_batch)
 g = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(dev)
 feeds = dict(scene_feat=g(f["scene_feat"]), obs_scene=g(f["obs_scene"]),
              grid_obs_labels=[g(x) for x in f["grid_obs_labels"]], grid_obs_regress=[g(x) for x in f["grid_obs_regress"]])
-eng = ConvRNNEngine(cfg, {k: torch.from_numpy(v) for k, v in w.items()}, dev, a.planes)
+eng = ConvRNNEngine(cfg, {k: torch.from_numpy(v) for k, v in w.items()}, dev)
 for _ in range(2):
   eng.forward(feeds)
 torch.cuda.synchronize()
