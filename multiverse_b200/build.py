@@ -74,15 +74,31 @@ def _up_to_date(stamp=None):
 
 
 def _build_locked(force, verbose):
-  srcs = sources()
   stamp = _current_stamp()
   if not force and _up_to_date(stamp):
     return LIB
+  _compile_and_link(LIB, OBJ, NVCC_FLAGS, verbose)
+  with open(os.path.join(OBJ, "stamp"), "w") as f:
+    f.write(stamp)
+  return LIB
+
+
+def build_variant(out_dir, defines=(), verbose=False):
+  """Compile the library with extra preprocessor definitions (e.g. MVB_CELL_PROBE, the cell kernel's phase profile)
+  into out_dir/libmultiverse_b200.so, leaving the in-tree library alone.  Returns the library's path."""
+  os.makedirs(out_dir, exist_ok=True)
+  lib = os.path.join(out_dir, os.path.basename(LIB))
+  _compile_and_link(lib, out_dir, NVCC_FLAGS + ["-D" + d for d in defines], verbose)
+  return lib
+
+
+def _compile_and_link(lib, obj_dir, flags, verbose):
+  srcs = sources()
   nvcc = _nvcc()
 
   def compile_one(src):
-    obj = os.path.join(OBJ, os.path.basename(src)[:-3] + ".o")
-    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", src, "-o", obj]
+    obj = os.path.join(obj_dir, os.path.basename(src)[:-3] + ".o")
+    cmd = [nvcc] + flags + (["-Xptxas", "-v"] if verbose else []) + ["-c", src, "-o", obj]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
       raise RuntimeError("nvcc failed for %s:\n%s\n%s" % (src, r.stdout, r.stderr))
@@ -92,13 +108,10 @@ def _build_locked(force, verbose):
 
   with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
     objs = list(ex.map(compile_one, srcs))
-  cmd = [nvcc, "-shared", "-o", LIB] + objs + GENCODE + ["-lcudart_static", "-lpthread", "-ldl", "-lrt"]
+  cmd = [nvcc, "-shared", "-o", lib] + objs + GENCODE + ["-lcudart_static", "-lpthread", "-ldl", "-lrt"]
   r = subprocess.run(cmd, capture_output=True, text=True)
   if r.returncode != 0:
     raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))
-  with open(os.path.join(OBJ, "stamp"), "w") as f:
-    f.write(stamp)
-  return LIB
 
 
 if __name__ == "__main__":

@@ -48,18 +48,58 @@ constexpr uint32_t SW128_SBO = 8 * ROW_BYTES;      // 1024 B between 8-row group
 //   A ring: one stage per 64-channel chunk: rows [m0 - (Wp+1), m0 + 128 + (Wp+1)) of every activation plane,
 //           rounded up to a multiple of 8 rows (RA8).  The nine taps of the chunk read THE SAME stage through wgmma
 //           descriptors that start (dy Wp + dx) rows into it (see make_smem_desc).
+// Layout: [B slots][A stages][barriers: full, empty (kMaxBSlots each), afull, aempty (kMaxAStages each)].
+constexpr int kSmemLimit = 227 * 1024;
+constexpr int kSmemExtra = 1024 /*alignment*/ + 512 /*barriers*/;
+constexpr int kMaxBSlots = 8;
+constexpr int kMaxAStages = 4;
+static_assert((2 * kMaxBSlots + 2 * kMaxAStages) * 8 <= 512, "the barrier area holds every ring's barriers");
+
+struct CellRing {
+  int b_slots, a_stages, a_stage_bytes;
+  constexpr int smem_bytes() const { return b_slots * B_SLOT_BYTES + a_stages * a_stage_bytes + kSmemExtra; }
+};
+
+template <int FMT>
 struct CellCfg {
-  static constexpr int A_STAGES = 2;
   static constexpr int MAX_RA8 = 256;           // TMA box limit: 128 + 2 (W + 2) <= 256  ->  W <= 62
-  // both formats hold the bytes of two bf16 planes (f16f8 loads one half per pass)
-  static constexpr int a_stage_bytes(int ra8) { return kBf16Planes * ra8 * ROW_BYTES; }
-  static constexpr int b_slots(int ra8) {       // 4 slots when they fit beside the A ring, else 3
-    return (4 * B_SLOT_BYTES + A_STAGES * a_stage_bytes(ra8) + 2048 <= 227 * 1024) ? 4 : 3;
-  }
-  static constexpr int smem_bytes(int ra8) {
-    return b_slots(ra8) * B_SLOT_BYTES + A_STAGES * a_stage_bytes(ra8) + 1024 /*align*/ + 512 /*barriers*/;
+  static constexpr CellRing ring(int ra8) {
+    if (FMT == 0) {
+      // bf16x2: both planes of a chunk in one stage, two stages; 4 weight slots when they fit beside them, else 3
+      const int a = kBf16Planes * ra8 * ROW_BYTES;
+      return CellRing{(4 * B_SLOT_BYTES + 2 * a + 2048 <= kSmemLimit) ? 4 : 3, 2, a};
+    }
+    // f16f8: a pass loads one 128-byte row per A row (the fp16 plane, or both e4m3 planes interleaved), so a stage
+    // holds one plane.  As many weight slots as fit beside two stages (5 at every width up to 62), then a third
+    // stage where it still fits (W <= 21: 36x18, 18x9).
+    const int a = ra8 * ROW_BYTES;
+    int b = (kSmemLimit - kSmemExtra - 2 * a) / B_SLOT_BYTES;
+    if (b > kMaxBSlots) b = kMaxBSlots;
+    return CellRing{b, CellRing{b, 3, a}.smem_bytes() <= kSmemLimit ? 3 : 2, a};
   }
 };
+static_assert(CellCfg<1>::ring(168).b_slots == 5 && CellCfg<1>::ring(168).a_stages == 3, "36x18: 5 slots, 3 stages");
+static_assert(CellCfg<1>::ring(152).b_slots == 5 && CellCfg<1>::ring(152).a_stages == 3, "18x9: 5 slots, 3 stages");
+static_assert(CellCfg<1>::ring(200).b_slots == 5 && CellCfg<1>::ring(200).a_stages == 2, "18x32: 5 slots, 2 stages");
+static_assert(CellCfg<1>::ring(256).b_slots == 5 && CellCfg<1>::ring(256).a_stages == 2 &&
+              CellCfg<1>::ring(256).smem_bytes() <= kSmemLimit, "4x62: 5 slots, 2 stages");
+static_assert(CellCfg<0>::ring(168).b_slots == 4 && CellCfg<0>::ring(200).b_slots == 3, "bf16x2 rings unchanged");
+
+// Phase profile (built with -DMVB_CELL_PROBE only, tools/probe_cell_phases.py): clock64() cycles of every warpgroup's
+// first thread, summed over all CTAs of the launches since the last read.  The product build has none of it.
+enum CellProbePhase {
+  kProbeFullWait, kProbeAFullWait, kProbeMmaWait, kProbeEpilogue, kProbeConsumer,    // MMA warpgroups
+  kProbeEmptyWait, kProbeAEmptyWait, kProbeProducer,                                 // TMA producer thread
+  kProbeTiles, kProbePhases
+};
+#ifdef MVB_CELL_PROBE
+__device__ unsigned long long g_cell_probe[kProbePhases];
+#define CELL_PROBE(...) __VA_ARGS__
+#define CELL_PROBED(ph, ...) do { const long long t0_ = clock64(); __VA_ARGS__; probe[ph] += clock64() - t0_; } while (0)
+#else
+#define CELL_PROBE(...)
+#define CELL_PROBED(ph, ...) __VA_ARGS__
+#endif
 
 struct CellParams {
   const float* bias;        // [1024] packed (tile, gate, channel) order
@@ -86,6 +126,7 @@ struct CellParams {
   const float* xr_in;       // [NS, H, W, 2] fp32 NHWC (no halo), or nullptr
   const float* xr_W;        // [9 taps * 2 channels][1024] fp32, packed column order
   int order;                // work order, see work_index()
+  CellRing ring;            // shared-memory rings of this launch (CellCfg<FMT>::ring)
   float* preact_out;        // [R, 1024] raw accumulators (packed column order) instead of the state update: first stage of
                             // the fan-out step (fanout_children_kernel turns every parent row into its K children)
   int hp_mixed;             // hp_out is written in the f16f8 format (else bf16x2 planes)
@@ -160,22 +201,25 @@ __device__ __forceinline__ EpiRow epi_row(const CellParams& prm, const Grid& g, 
   return r;
 }
 
-// The epilogue of one row and two adjacent packed columns j, j + 1 of every gate (a[gate][e] = accumulators of
-// column gate * 64 + j + e of N tile nt): state update and every requested output.
+// c of the row's channels ch, ch + 1 from the previous step (zero state without c_in).  The epilogue fetches all of
+// its rows' c before the tile's last MMAs complete (the rows are scattered by row_map, so each is an HBM round trip).
+__device__ __forceinline__ float2 epi_cprev(const CellParams& prm, const EpiRow& r, int ch) {
+  return (prm.c_in && !prm.preact_out && r.valid)
+             ? __ldg(reinterpret_cast<const float2*>(prm.c_in + r.src_row * kHidden + ch)) : make_float2(0.f, 0.f);
+}
+
+// What the pre-activations of one row and two adjacent packed columns j, j + 1 of every gate add to the
+// accumulators: q = bias (or bias-folded table) + x-fold / sparse-x table row + dense x path, and the f16f8 column
+// scales.  Loaded for both rows of a column pair before either is stored (epi_pair), so that the loads of one row do
+// not wait for the stores of the other.
+struct EpiIn { float q[4][2], sc[4][2]; };
 template <int FMT>
-__device__ __forceinline__ void epi_pair(const CellParams& prm, const Grid& g, const EpiRow& r, int nt, int j,
-                                         const float (&a)[4][2]) {
+__device__ __forceinline__ EpiIn epi_inputs(const CellParams& prm, const Grid& g, const EpiRow& r, int nt, int j) {
+  EpiIn in = {};
+  if (prm.preact_out || !r.valid) return in;
   const int col = nt * BLOCK_N + j;             // packed column of gate 0
-  const int ch = nt * TILE_CH + j;              // hidden channel
-  if (prm.preact_out) {
-    float* gp = prm.preact_out + r.row * kGates + col;
-#pragma unroll
-    for (int gt = 0; gt < 4; ++gt) *reinterpret_cast<float2*>(gp + gt * TILE_CH) = make_float2(a[gt][0], a[gt][1]);
-    return;
-  }
-  // bias (or bias-folded table), + the x-fold / sparse-x table row of this cell, + the dense x path
   const float* bptr = (r.xfb ? r.xfb : prm.bias) + col;
-  float q[4][2];
+  float (&q)[4][2] = in.q;
 #pragma unroll
   for (int gt = 0; gt < 4; ++gt) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(bptr + gt * TILE_CH));
@@ -201,16 +245,32 @@ __device__ __forceinline__ void epi_pair(const CellParams& prm, const Grid& g, c
       }
     }
   }
-  float sc[4][2] = {};
   if (FMT == 1) {
 #pragma unroll
     for (int gt = 0; gt < 4; ++gt) {
       const float2 s2 = __ldg(reinterpret_cast<const float2*>(prm.col_scale + col + gt * TILE_CH));
-      sc[gt][0] = s2.x; sc[gt][1] = s2.y;
+      in.sc[gt][0] = s2.x; in.sc[gt][1] = s2.y;
     }
   }
-  float2 cprev = make_float2(0.f, 0.f);
-  if (prm.c_in) cprev = __ldg(reinterpret_cast<const float2*>(prm.c_in + r.src_row * kHidden + ch));
+  return in;
+}
+
+// The epilogue of one row and two adjacent packed columns j, j + 1 of every gate (a[gate][e] = accumulators of
+// column gate * 64 + j + e of N tile nt, cprev = epi_cprev of its channels, in = epi_inputs): state update and every
+// requested output.
+template <int FMT>
+__device__ __forceinline__ void epi_pair(const CellParams& prm, const EpiRow& r, int nt, int j, const float (&a)[4][2],
+                                         float2 cprev, const EpiIn& in) {
+  const int col = nt * BLOCK_N + j;             // packed column of gate 0
+  const int ch = nt * TILE_CH + j;              // hidden channel
+  if (prm.preact_out) {
+    float* gp = prm.preact_out + r.row * kGates + col;
+#pragma unroll
+    for (int gt = 0; gt < 4; ++gt) *reinterpret_cast<float2*>(gp + gt * TILE_CH) = make_float2(a[gt][0], a[gt][1]);
+    return;
+  }
+  const float (&q)[4][2] = in.q;
+  const float (&sc)[4][2] = in.sc;
   GateOut o[2];
 #pragma unroll
   for (int e = 0; e < 2; ++e)
@@ -257,19 +317,19 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmA8, const __grid_constant__ CUtensorMap tmB8,
                 const CellParams prm) {
-  using Cfg = CellCfg;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   const int ra8 = (BLOCK_M + 2 * (prm.W + 2) + 7) & ~7;     // rows of an A stage
-  const int a_stage_bytes = Cfg::a_stage_bytes(ra8);
+  const int a_stage_bytes = prm.ring.a_stage_bytes;
   const int a_load_bytes = FMT ? ra8 * ROW_BYTES : a_stage_bytes;     // f16f8: one plane per pass
-  const int b_slots = Cfg::b_slots(ra8);
+  const int b_slots = prm.ring.b_slots, a_stages = prm.ring.a_stages;
   uint8_t* smem_a = smem + b_slots * B_SLOT_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_a + Cfg::A_STAGES * a_stage_bytes);
-  uint64_t* empty_bar = full_bar + 8;
-  uint64_t* afull_bar = empty_bar + 8;
-  uint64_t* aempty_bar = afull_bar + Cfg::A_STAGES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_a + a_stages * a_stage_bytes);
+  uint64_t* empty_bar = full_bar + kMaxBSlots;
+  uint64_t* afull_bar = empty_bar + kMaxBSlots;
+  uint64_t* aempty_bar = afull_bar + kMaxAStages;
+  CELL_PROBE(long long probe[kProbePhases] = {};)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -304,8 +364,10 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     if (FMT == 1) { prefetch_tmap(&tmA8); prefetch_tmap(&tmB8); }
+#pragma unroll 1
     for (int s = 0; s < b_slots; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], MC ? 4 : 2); }
-    for (int s = 0; s < Cfg::A_STAGES; ++s) { mbar_init(&afull_bar[s], 1); mbar_init(&aempty_bar[s], 2); }
+#pragma unroll 1
+    for (int s = 0; s < a_stages; ++s) { mbar_init(&afull_bar[s], 1); mbar_init(&aempty_bar[s], 2); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -316,6 +378,7 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     if (warp == 0 && lane == 0) {
       // ===================== TMA producer =====================
       int slot = 0, astage = 0; uint32_t phase = 0, aphase = 0;
+      CELL_PROBE(const long long probe_t0 = clock64();)
       for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
         const long long m0 = tile_m0(t);
         const int n0 = (int)(t % N_TILES) * BLOCK_N;
@@ -327,16 +390,16 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           const int c16 = q == 0 ? 0 : cxp + (q - 1) * CHUNK;              // 16-bit channel coordinate
           const int c8 = q == 0 ? 0 : 2 * cxp + (q - 1) * 2 * CHUNK;       // fp8 byte coordinate
           const bool f8 = FMT == 1 && pass == 0;
-          mbar_wait(&aempty_bar[astage], aphase ^ 1);
+          CELL_PROBED(kProbeAEmptyWait, mbar_wait(&aempty_bar[astage], aphase ^ 1));
           uint8_t* sa = smem_a + astage * a_stage_bytes;
           mbar_expect_tx(&afull_bar[astage], a_load_bytes);
           if (f8) tma_load_3d(sa, &tmA8, &afull_bar[astage], c8, (int)(m0 - g.Wp - 1), 0);
           else tma_load_3d(sa, &tmA, &afull_bar[astage], c16, (int)(m0 - g.Wp - 1), 0);
-          if (++astage == Cfg::A_STAGES) { astage = 0; aphase ^= 1; }
+          if (++astage == a_stages) { astage = 0; aphase ^= 1; }
           for (int tap = 0; tap < 9; ++tap) {
 #pragma unroll
             for (int sl = 0; sl < NS; ++sl) {
-              mbar_wait(&empty_bar[slot], phase ^ 1);
+              CELL_PROBED(kProbeEmptyWait, mbar_wait(&empty_bar[slot], phase ^ 1));
               uint8_t* sb = smem + slot * B_SLOT_BYTES;
               mbar_expect_tx(&full_bar[slot], B_SLOT_BYTES);
               const CUtensorMap* tm = f8 ? &tmB8 : &tmB;
@@ -350,6 +413,11 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           }
         }
       }
+#ifdef MVB_CELL_PROBE
+      atomicAdd(&g_cell_probe[kProbeEmptyWait], (unsigned long long)probe[kProbeEmptyWait]);
+      atomicAdd(&g_cell_probe[kProbeAEmptyWait], (unsigned long long)probe[kProbeAEmptyWait]);
+      atomicAdd(&g_cell_probe[kProbeProducer], (unsigned long long)(clock64() - probe_t0));
+#endif
     }
   } else {
     regs_alloc<232>();
@@ -371,7 +439,9 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       }
       rel_slot = -1; rel_astage = -1;
     };
+    CELL_PROBE(const long long probe_t0 = clock64();)
     for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
+      CELL_PROBE(++probe[kProbeTiles];)
       const long long m0 = tile_m0(t);
       const int nt = (int)(t % N_TILES);
       uint32_t fresh = 1;                      // the tile's first MMA overwrites the accumulator
@@ -387,14 +457,14 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       for (int pass = 0; pass < NPASS; ++pass)
       for (int q = q_begin; q < NQ; ++q) {
         const bool f8 = FMT == 1 && pass == 0;
-        mbar_wait(&afull_bar[astage], aphase);
+        CELL_PROBED(kProbeAFullWait, mbar_wait(&afull_bar[astage], aphase));
         const uint32_t sa_lo = (smem_u32(smem_a + astage * a_stage_bytes) >> 4) + a_wg_lo;
         for (int tap = 0; tap < 9; ++tap) {
           // the tap's A tile: the stage's rows starting (dy-1) Wp + (dx-1) + (Wp+1) = dy Wp + dx rows in
           const uint32_t a_lo = sa_lo + (uint32_t)((tap / 3) * g.Wp + (tap % 3)) * (ROW_BYTES >> 4);
 #pragma unroll
           for (int sl = 0; sl < NS; ++sl) {
-            mbar_wait(&full_bar[slot], phase);
+            CELL_PROBED(kProbeFullWait, mbar_wait(&full_bar[slot], phase));
             const uint32_t b_lo = smem_u32(smem + slot * B_SLOT_BYTES) >> 4;
             wgmma_fence_regs(acc);
             wgmma_fence();
@@ -426,38 +496,63 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             }
             wgmma_commit();
             wgmma_fence_regs(acc);
-            wgmma_wait<1>();               // the previous batch has completed: its slot (and A stage) can be refilled
+            // the previous batch has completed: its slot (and A stage) can be refilled
+            CELL_PROBED(kProbeMmaWait, wgmma_wait<1>());
             release();
             rel_slot = slot;
             if (tap == 8 && sl == NS - 1) rel_astage = astage;     // this CTA's nine taps have consumed the A stage
             if (++slot == b_slots) { slot = 0; phase ^= 1; }
           }
         }
-        if (++astage == Cfg::A_STAGES) { astage = 0; aphase ^= 1; }
+        if (++astage == a_stages) { astage = 0; aphase ^= 1; }
       }
-      wgmma_wait<0>();
-      wgmma_fence_regs(acc);
-      release();
       // ===================== epilogue =====================
       // thread (warp w of the warpgroup, lane l) holds rows 16 w + l / 4 (+ 8) and columns 8 i + 2 (l % 4) (+ 1);
-      // column gate * 64 + j of the N tile is gate `gate` of channel j: each thread owns all four gates of its channels
+      // column gate * 64 + j of the N tile is gate `gate` of channel j: each thread owns all four gates of its channels.
+      // The rows' context and c are loaded while the last MMAs run, all at once rather than one pair after another's
+      // stores.
+      CELL_PROBE(const long long probe_e0 = clock64();)
       const long long rbase = m0 + 64 * c + 16 * (warp & 3) + (lane >> 2);
+      EpiRow rows[2];
+      float2 cprev[2][8];
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
-        const EpiRow r = epi_row(prm, g, rbase + 8 * hr);
-        if (!r.valid) continue;
+        rows[hr] = epi_row(prm, g, rbase + 8 * hr);
 #pragma unroll
-        for (int ip = 0; ip < 8; ++ip) {
+        for (int ip = 0; ip < 8; ++ip) cprev[hr][ip] = epi_cprev(prm, rows[hr], nt * TILE_CH + 8 * ip + 2 * (lane & 3));
+      }
+      CELL_PROBE(const long long probe_w0 = clock64();)
+      wgmma_wait<0>();
+      CELL_PROBE(const long long probe_w = clock64() - probe_w0; probe[kProbeMmaWait] += probe_w;)
+      wgmma_fence_regs(acc);
+      release();
+#pragma unroll
+      for (int ip = 0; ip < 8; ++ip) {
+        const int j = 8 * ip + 2 * (lane & 3);
+        EpiIn in[2];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) in[hr] = epi_inputs<FMT>(prm, g, rows[hr], nt, j);
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          if (!rows[hr].valid) continue;
           float a[4][2];
 #pragma unroll
           for (int gt = 0; gt < 4; ++gt) {
             a[gt][0] = acc[4 * (8 * gt + ip) + 2 * hr];
             a[gt][1] = acc[4 * (8 * gt + ip) + 2 * hr + 1];
           }
-          epi_pair<FMT>(prm, g, r, nt, 8 * ip + 2 * (lane & 3), a);
+          epi_pair<FMT>(prm, rows[hr], nt, j, a, cprev[hr][ip], in[hr]);
         }
       }
+      CELL_PROBE(probe[kProbeEpilogue] += clock64() - probe_e0 - probe_w;)
     }
+#ifdef MVB_CELL_PROBE
+    if (leader) {
+      for (int p = kProbeFullWait; p <= kProbeEpilogue; ++p) atomicAdd(&g_cell_probe[p], (unsigned long long)probe[p]);
+      atomicAdd(&g_cell_probe[kProbeConsumer], (unsigned long long)(clock64() - probe_t0));
+      atomicAdd(&g_cell_probe[kProbeTiles], (unsigned long long)probe[kProbeTiles]);
+    }
+#endif
   }
 
   __syncthreads();
@@ -725,6 +820,24 @@ static void note_variant(int fmt, int pair) {
   g_variants_seen |= 1ull << (fmt * 2 + pair);
 }
 
+#ifdef MVB_CELL_PROBE
+static CellRing g_probe_ring = {};
+// Phase profile of the cell launches since the last reset (probe build only, not part of the public header):
+// out[kProbePhases] in CellProbePhase order, then weight slots, A stages and A stage bytes of the last launch.
+extern "C" int mvb_cell_probe(unsigned long long* out, int reset) {
+  MVB_CHECK_CUDA(cudaDeviceSynchronize());
+  MVB_CHECK_CUDA(cudaMemcpyFromSymbol(out, g_cell_probe, sizeof(g_cell_probe)));
+  out[kProbePhases] = g_probe_ring.b_slots;
+  out[kProbePhases + 1] = g_probe_ring.a_stages;
+  out[kProbePhases + 2] = g_probe_ring.a_stage_bytes;
+  if (reset) {
+    const unsigned long long zero[kProbePhases] = {};
+    MVB_CHECK_CUDA(cudaMemcpyToSymbol(g_cell_probe, zero, sizeof(zero)));
+  }
+  return MVB_OK;
+}
+#endif
+
 struct CellMaps { CUtensorMap A, B, Bh, A8, B8, B8h; };
 
 // Work order of a launch (CellParams::order, work_index()).  1: the four N tiles of an M tile (pair) run back to back
@@ -741,12 +854,19 @@ static int pick_order(int forced, long long units, long long ctas) {
 
 template <int FMT>
 static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms, bool multicast, cudaStream_t stream) {
-  using Cfg = CellCfg;
   CellParams prm = prm_in;
   static SmemOptIn opt_plain, opt_mc;
+  // MVB_CELL_FORMAT_RINGS=0: f16f8 launches use the bf16x2 rings (two-plane A stages, 4 or 3 weight slots), the
+  // layout before the rings were sized per format, for A/B runs; the results are bit-identical either way
+  static const bool format_rings = [] { const char* e = getenv("MVB_CELL_FORMAT_RINGS"); return !(e && e[0] == '0'); }();
   const int ra8 = (BLOCK_M + 2 * (prm.W + 2) + 7) & ~7;
-  const int smem_bytes = Cfg::smem_bytes(ra8);
-  MVB_REQUIRE(ra8 <= Cfg::MAX_RA8 && smem_bytes <= 227 * 1024, "cell_fwd: grid width W=%d too large (A stage of %d rows, %d B shared memory)", prm.W, ra8, smem_bytes);
+  prm.ring = format_rings ? CellCfg<FMT>::ring(ra8) : CellCfg<0>::ring(ra8);
+  const int smem_bytes = prm.ring.smem_bytes();
+  MVB_REQUIRE(ra8 <= CellCfg<FMT>::MAX_RA8 && smem_bytes <= kSmemLimit && prm.ring.b_slots >= 2 &&
+              prm.ring.b_slots <= kMaxBSlots && prm.ring.a_stages >= 2 && prm.ring.a_stages <= kMaxAStages,
+              "cell_fwd: grid width W=%d too large (A stage of %d rows: %d weight slots, %d A stages, %d B shared memory)",
+              prm.W, ra8, prm.ring.b_slots, prm.ring.a_stages, smem_bytes);
+  CELL_PROBE(g_probe_ring = prm.ring;)
   MVB_CHECK_CUDA(smem_opt_in(opt_plain, cell_fwd_kernel<false, FMT>, smem_bytes));
   MVB_CHECK_CUDA(smem_opt_in(opt_mc, cell_fwd_kernel<true, FMT>, smem_bytes));
   const long long m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
