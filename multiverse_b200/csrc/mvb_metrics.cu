@@ -11,6 +11,13 @@
 
 namespace mvb {
 
+// dx^2 + dy^2 as numpy forms it: both squares rounded, then the add.  Written with explicit round-to-nearest
+// intrinsics because nvcc would otherwise contract it to dx*dx then fma(dy, dy, .), which differs from numpy in the
+// last bit whenever dy^2 is not exact in double (coordinates of unlike magnitude), and can flip a near-tie selection.
+__device__ __forceinline__ double sq_dist(double dx, double dy) {
+  return __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
+}
+
 // One warp per (trajectory n, ground-truth future g).
 //   pred [N,K,Tp,2] fp32, gt [N,G,Tg,2] fp32, gt_len [N,G] (0 = no such future; <= min(Tp,Tg))
 // The arithmetic is the reference's, in double like numpy on the float64 arrays it builds: per prediction k the
@@ -35,7 +42,7 @@ __global__ void min_ade_fde_kernel(const float* __restrict__ pred, const float* 
       double s = 0.0, last = 0.0;
       for (int t = 0; t < len; ++t) {
         const double dx = (double)g[2 * t] - (double)p[2 * t], dy = (double)g[2 * t + 1] - (double)p[2 * t + 1];
-        last = sqrt(dx * dx + dy * dy);
+        last = sqrt(sq_dist(dx, dy));
         s += last;
       }
       if (s < best_sum) { best_sum = s; best_k = k; }          // lanes scan k in increasing order: first index wins
@@ -56,7 +63,7 @@ __global__ void min_ade_fde_kernel(const float* __restrict__ pred, const float* 
     if (t < len) {
       const float* p = pred + ((n * K + best_k) * Tp) * 2;
       const double dx = (double)g[2 * t] - (double)p[2 * t], dy = (double)g[2 * t + 1] - (double)p[2 * t + 1];
-      d = sqrt(dx * dx + dy * dy);
+      d = sqrt(sq_dist(dx, dy));
     }
     ade_err[wid * Tg + t] = d;
   }
