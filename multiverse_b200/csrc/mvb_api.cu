@@ -130,9 +130,11 @@ int mvb_convlstm_cell_fwd(const void* xh_planes, const void* w_planes, const flo
                           void* hp_out, int64_t hp_plane_stride, int cpad_out, int ch_off_out,
                           int64_t NS, int H, int W, int cpad, int planes, float forget_bias,
                           void* stream) {
-  return cell_fwd(xh_planes, w_planes, bias_packed, c_in, row_map, c_out, h32_out, hp_out,
-                  hp_plane_stride, cpad_out, ch_off_out, NS, H, W, cpad, planes, forget_bias,
-                  nullptr, nullptr, nullptr, nullptr, 1, S(stream));
+  CellStep s{};
+  s.xh = xh_planes; s.w = w_planes; s.bias = bias_packed; s.c_in = c_in; s.row_map = row_map; s.c_out = c_out;
+  s.h32_out = h32_out; s.hp_out = hp_out; s.hp_plane_stride = hp_plane_stride; s.cpad_out = cpad_out;
+  s.ch_off_out = ch_off_out; s.NS = NS; s.H = H; s.W = W; s.cpad = cpad; s.planes = planes; s.forget_bias = forget_bias;
+  return cell_fwd(s, S(stream));
 }
 int mvb_cell_xfold_tables(const float* kernel, const float* biases, const float* We, const float* be,
                           int E, float* table_B, float* table_T2, void* stream) {
@@ -143,18 +145,23 @@ int mvb_convlstm_cell_fwd_onehot(const void* xh_planes, const void* w_planes, co
                                  const int32_t* row_map, float* c_out, float* h32_out, void* hp_out,
                                  int64_t hp_plane_stride, int cpad_out, int ch_off_out, int64_t NS, int H,
                                  int W, int cpad, int planes, float forget_bias, void* stream) {
-  return cell_fwd(xh_planes, w_planes, table_B, c_in, row_map, c_out, h32_out, hp_out, hp_plane_stride,
-                  cpad_out, ch_off_out, NS, H, W, cpad, planes, forget_bias, nullptr, table_B, table_T2, ids, 1,
-                  S(stream));
+  CellStep s{};
+  s.xh = xh_planes; s.w = w_planes; s.xf_B = table_B; s.xf_T2 = table_T2; s.xf_ids = ids; s.c_in = c_in;
+  s.row_map = row_map; s.c_out = c_out; s.h32_out = h32_out; s.hp_out = hp_out; s.hp_plane_stride = hp_plane_stride;
+  s.cpad_out = cpad_out; s.ch_off_out = ch_off_out; s.NS = NS; s.H = H; s.W = W; s.cpad = cpad; s.planes = planes;
+  s.forget_bias = forget_bias;
+  return cell_fwd(s, S(stream));
 }
 int mvb_convlstm_cell_fwd_xdense(const void* xh_planes, const void* w_planes, const float* bias_packed,
                                  const float* x_in, const float* x_weights, const float* c_in, float* c_out,
                                  float* h32_out, void* hp_out, int64_t hp_plane_stride, int cpad_out, int ch_off_out,
                                  int64_t NS, int H, int W, int cpad, int planes, float forget_bias, void* stream) {
   MVB_REQUIRE(x_in && x_weights, "mvb_convlstm_cell_fwd_xdense: null x input / weights");
-  return cell_fwd(xh_planes, w_planes, bias_packed, c_in, nullptr, c_out, h32_out, hp_out, hp_plane_stride, cpad_out,
-                  ch_off_out, NS, H, W, cpad, planes, forget_bias, nullptr, nullptr, nullptr, nullptr, 1, S(stream),
-                  x_in, x_weights);
+  CellStep s{};
+  s.xh = xh_planes; s.w = w_planes; s.bias = bias_packed; s.xr_in = x_in; s.xr_W = x_weights; s.c_in = c_in;
+  s.c_out = c_out; s.h32_out = h32_out; s.hp_out = hp_out; s.hp_plane_stride = hp_plane_stride; s.cpad_out = cpad_out;
+  s.ch_off_out = ch_off_out; s.NS = NS; s.H = H; s.W = W; s.cpad = cpad; s.planes = planes; s.forget_bias = forget_bias;
+  return cell_fwd(s, S(stream));
 }
 int mvb_cell_xdense_weights(const float* kernel_tf, float* x_weights, void* stream) {
   return cell_xdense_weights(kernel_tf, x_weights, S(stream));
@@ -164,9 +171,11 @@ int mvb_convlstm_cell_fwd_xsparse(const void* xh_planes, const void* w_planes, c
                                   float* h32_out, void* hp_out, int64_t hp_plane_stride, int cpad_out, int ch_off_out,
                                   int64_t NS, int H, int W, int cpad, int planes, float forget_bias, void* stream) {
   MVB_REQUIRE(x_table && label, "mvb_convlstm_cell_fwd_xsparse: null table / labels");
-  return cell_fwd(xh_planes, w_planes, bias_packed, c_in, nullptr, c_out, h32_out, hp_out, hp_plane_stride, cpad_out,
-                  ch_off_out, NS, H, W, cpad, planes, forget_bias, nullptr, nullptr, nullptr, nullptr, 1, S(stream),
-                  nullptr, nullptr, x_table, label);
+  CellStep s{};
+  s.xh = xh_planes; s.w = w_planes; s.bias = bias_packed; s.xs_tab = x_table; s.xs_label = label; s.c_in = c_in;
+  s.c_out = c_out; s.h32_out = h32_out; s.hp_out = hp_out; s.hp_plane_stride = hp_plane_stride; s.cpad_out = cpad_out;
+  s.ch_off_out = ch_off_out; s.NS = NS; s.H = H; s.W = W; s.cpad = cpad; s.planes = planes; s.forget_bias = forget_bias;
+  return cell_fwd(s, S(stream));
 }
 int mvb_cell_xsparse_weights(const float* kernel_tf, int cx, float* x_weights, void* stream) {
   return cell_xsparse_weights(kernel_tf, cx, x_weights, S(stream));
@@ -179,8 +188,11 @@ int mvb_convlstm_cell_fwd_onehot_fanout(const void* xh_planes, const void* w_pla
                                         const float* table_T2, const int32_t* ids, const float* c_in,
                                         float* c_out, float* h32_out, float* workspace, int64_t NS, int fanout, int H,
                                         int W, int cpad, int planes, float forget_bias, void* stream) {
-  return cell_fwd(xh_planes, w_planes, table_B, c_in, nullptr, c_out, h32_out, nullptr, 0, 0, 0, NS, H, W, cpad,
-                  planes, forget_bias, workspace, table_B, table_T2, ids, fanout, S(stream));
+  CellStep s{};
+  s.xh = xh_planes; s.w = w_planes; s.xf_B = table_B; s.xf_T2 = table_T2; s.xf_ids = ids; s.c_in = c_in;
+  s.c_out = c_out; s.h32_out = h32_out; s.fanout_ws = workspace; s.NS = NS; s.fanout = fanout; s.H = H; s.W = W;
+  s.cpad = cpad; s.planes = planes; s.forget_bias = forget_bias;
+  return cell_fwd(s, S(stream));
 }
 
 int mvb_convlstm_cell_fwd_train(const void* xh_planes, const void* w_planes,
@@ -188,9 +200,11 @@ int mvb_convlstm_cell_fwd_train(const void* xh_planes, const void* w_planes,
                                 float* h32_out, void* hp_out, int64_t hp_plane_stride, int cpad_out,
                                 int ch_off_out, float* gates_out, int64_t NS, int H, int W, int cpad,
                                 int planes, float forget_bias, void* stream) {
-  return cell_fwd(xh_planes, w_planes, bias_packed, c_in, nullptr, c_out, h32_out, hp_out,
-                  hp_plane_stride, cpad_out, ch_off_out, NS, H, W, cpad, planes, forget_bias,
-                  gates_out, nullptr, nullptr, nullptr, 1, S(stream));
+  CellStep s{};
+  s.xh = xh_planes; s.w = w_planes; s.bias = bias_packed; s.c_in = c_in; s.c_out = c_out; s.h32_out = h32_out;
+  s.hp_out = hp_out; s.hp_plane_stride = hp_plane_stride; s.cpad_out = cpad_out; s.ch_off_out = ch_off_out;
+  s.gates_out = gates_out; s.NS = NS; s.H = H; s.W = W; s.cpad = cpad; s.planes = planes; s.forget_bias = forget_bias;
+  return cell_fwd(s, S(stream));
 }
 int mvb_lstm_gates_bwd(const float* gates, const float* c_prev, const float* c_new, const float* dh,
                        const float* dc_in, void* dg_planes, int64_t plane_stride, float* dc_prev,

@@ -894,25 +894,24 @@ static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms
   return MVB_OK;
 }
 
-int cell_fwd(const void* xh_planes, const void* w_planes, const float* bias, const float* c_in,
-             const int* row_map, float* c_out, float* h32_out, void* hp_out, long long hp_plane_stride,
-             int cpad_out, int ch_off_out, long long NS, int H, int W, int cpad, int P,
-             float forget_bias, float* gates_out, const float* xf_B, const float* xf_T2, const int* xf_ids,
-             int fanout, cudaStream_t stream, const float* xr_in, const float* xr_W, const float* xs_tab,
-             const int* xs_label) {
-  // planes = format of the inputs and weights | (format of hp_out << 8), the latter only when it differs
-  const int P_out = (P >> 8) ? (P >> 8) : (P & 0xFF);
-  P &= 0xFF;
+int cell_fwd(const CellStep& s, cudaStream_t stream) {
+  const int P = s.planes & 0xFF, P_out = (s.planes >> 8) ? (s.planes >> 8) : P;
   MVB_REQUIRE(valid_planes(P) && valid_planes(P_out), "cell_fwd: planes P=%d (output planes %d) not 2 or %d", P, P_out,
               kPlanesF16F8);
-  const bool mixed = P == kPlanesF16F8;
-  MVB_REQUIRE(!mixed || !gates_out || fanout > 1, "cell_fwd: the f16f8 format is an inference format (no gates_out)");
-  MVB_REQUIRE(fanout <= 1 || (xf_B && xf_T2 && xf_ids && gates_out && c_in && h32_out && !row_map && !hp_out),
-              "cell_fwd: fanout=%d needs the x-fold tables, c_in, h32_out, a [R,1024] fp32 workspace and no row_map / hp_out", fanout);
+  const bool mixed = P == kPlanesF16F8, fan = s.fanout > 1;
+  const int x_sources = !!s.xf_B + !!s.xs_tab + !!s.xr_W;
+  const long long NS = s.NS; const int H = s.H, W = s.W, cpad = s.cpad;
+  MVB_REQUIRE(!mixed || !s.gates_out, "cell_fwd: the f16f8 format is an inference format (no gates_out)");
+  MVB_REQUIRE(x_sources <= 1, "cell_fwd: at most one x source (x-fold, sparse or dense x)");
+  MVB_REQUIRE(!s.row_map || !(s.xs_tab || s.xr_W), "cell_fwd: a row map goes with the x-fold tables or no x source");
+  MVB_REQUIRE(!fan || (s.xf_B && s.c_in && s.h32_out && s.fanout_ws && !s.row_map && !s.hp_out),
+              "cell_fwd: fanout=%d needs the x-fold tables, c_in, h32_out, a [R,1024] fp32 workspace and no row_map / hp_out", s.fanout);
+  MVB_REQUIRE(!s.xf_B || (s.xf_T2 && s.xf_ids && H >= 3 && W >= 3), "cell_fwd: x-fold needs its tables, ids and a grid of at least 3x3");
+  MVB_REQUIRE((!s.xs_tab || s.xs_label) && (!s.xr_W || s.xr_in), "cell_fwd: the sparse x path needs its labels, the dense one its input");
   MVB_REQUIRE(cpad == kHidden + XPAD || cpad == kHidden + 2 * XPAD, "cell_fwd: cpad=%d must be 288 or 320 (x block of 32 or 64 channels)", cpad);
   MVB_REQUIRE(NS > 0 && H > 0 && W > 0, "cell_fwd: bad sizes NS=%lld H=%d W=%d", NS, H, W);
-  MVB_REQUIRE(xh_planes && w_planes && bias && c_out, "cell_fwd: null pointer");
-  if (hp_out) MVB_REQUIRE(cpad_out % 8 == 0 && ch_off_out % 8 == 0, "cell_fwd: hp_out pitch/offset must be multiples of 8");
+  MVB_REQUIRE(s.xh && s.w && (s.bias || s.xf_B) && s.c_out, "cell_fwd: null pointer");
+  if (s.hp_out) MVB_REQUIRE(s.cpad_out % 8 == 0 && s.ch_off_out % 8 == 0, "cell_fwd: hp_out pitch/offset must be multiples of 8");
   const Grid g = make_grid(H, W);
   const long long R = NS * g.S;
   MVB_REQUIRE(R + 2LL * g.Wp + 256 < 0x7fffffffLL, "cell_fwd: too many rows (%lld) for int32 TMA coordinates", R);
@@ -923,14 +922,14 @@ int cell_fwd(const void* xh_planes, const void* w_planes, const float* bias, con
   const int P16 = mixed ? 1 : kBf16Planes;      // 16-bit "planes" the A / B maps describe
   const uint32_t ra8 = (uint32_t)((BLOCK_M + 2 * (W + 2) + 7) & ~7);      // rows of an A stage (see CellCfg)
   MVB_REQUIRE(ra8 <= 256, "cell_fwd: grid width W=%d too large for the halo'd A stage (%u rows > 256)", W, ra8);
-  int rc = encode_tmap_3d_bf16(&tm.A, xh_planes, (uint64_t)cpad, (uint64_t)R, (uint64_t)P16,
+  int rc = encode_tmap_3d_bf16(&tm.A, s.xh, (uint64_t)cpad, (uint64_t)R, (uint64_t)P16,
                                (uint64_t)cpad * 2, (uint64_t)R * cpad * 2, CHUNK, ra8, P16, 128);
   if (rc) return rc;
   const uint64_t ktot = 9ull * cpad;
-  rc = encode_tmap_3d_bf16(&tm.B, w_planes, ktot, (uint64_t)kGates, (uint64_t)P16, ktot * 2,
+  rc = encode_tmap_3d_bf16(&tm.B, s.w, ktot, (uint64_t)kGates, (uint64_t)P16, ktot * 2,
                            ktot * kGates * 2, CHUNK, BLOCK_N, 1, 128);          // one plane of a tile = one slot
   if (rc) return rc;
-  rc = encode_tmap_3d_bf16(&tm.Bh, w_planes, ktot, (uint64_t)kGates, (uint64_t)P16, ktot * 2,
+  rc = encode_tmap_3d_bf16(&tm.Bh, s.w, ktot, (uint64_t)kGates, (uint64_t)P16, ktot * 2,
                            ktot * kGates * 2, CHUNK, BLOCK_N / 2, 1, 128);      // half of it (CTA pairs)
   if (rc) return rc;
   tm.A8 = tm.A; tm.B8 = tm.B; tm.B8h = tm.Bh;
@@ -938,8 +937,8 @@ int cell_fwd(const void* xh_planes, const void* w_planes, const float* bias, con
   if (mixed) {
     // [fp16 region][fp8 region: rows of 2*cpad bytes, both e4m3 planes interleaved per chunk (f8_off)]
     // ([+ 1024 fp32 column scales] after the weights)
-    const uint8_t* a8 = reinterpret_cast<const uint8_t*>(xh_planes) + 2ull * R * cpad;
-    const uint8_t* b8 = reinterpret_cast<const uint8_t*>(w_planes) + 2ull * kGates * ktot;
+    const uint8_t* a8 = reinterpret_cast<const uint8_t*>(s.xh) + 2ull * R * cpad;
+    const uint8_t* b8 = reinterpret_cast<const uint8_t*>(s.w) + 2ull * kGates * ktot;
     rc = encode_tmap_3d_u8(&tm.A8, a8, 2ull * cpad, (uint64_t)R, 1, 2ull * cpad, 2ull * R * cpad, ROW_BYTES, ra8, 1, 128);
     if (rc) return rc;
     rc = encode_tmap_3d_u8(&tm.B8, b8, 2 * ktot, (uint64_t)kGates, 1, 2 * ktot, 2 * ktot * kGates, ROW_BYTES, BLOCK_N, 1, 128);
@@ -950,45 +949,30 @@ int cell_fwd(const void* xh_planes, const void* w_planes, const float* bias, con
   }
 
   CellParams prm;
-  prm.bias = bias; prm.col_scale = col_scale; prm.c_in = c_in; prm.row_map = row_map; prm.c_out = c_out; prm.h32_out = h32_out;
-  prm.gates_out = fanout > 1 ? nullptr : gates_out;
-  prm.preact_out = fanout > 1 ? gates_out : nullptr;      // fan-out: stage 1 stores the raw accumulators there
-  prm.xf_B = xf_B; prm.xf_T2 = xf_T2; prm.xf_ids = xf_ids;
-  prm.skip_x = 0;
+  prm.bias = s.bias; prm.col_scale = col_scale; prm.c_in = s.c_in; prm.row_map = s.row_map; prm.c_out = s.c_out;
+  prm.h32_out = s.h32_out; prm.gates_out = s.gates_out;
+  prm.preact_out = fan ? s.fanout_ws : nullptr;      // fan-out: stage 1 stores the raw accumulators there
+  prm.xf_B = s.xf_B; prm.xf_T2 = s.xf_T2; prm.xf_ids = s.xf_ids;
+  prm.xs_tab = s.xs_tab; prm.xs_label = s.xs_label; prm.xr_in = s.xr_in; prm.xr_W = s.xr_W;
+  prm.skip_x = x_sources;      // an x source replaces the x chunk of the K loop
   // work order: chosen per launch in launch_cell (MVB_CELL_ORDER=0|1 forces one)
   static const int order = [] { const char* e = getenv("MVB_CELL_ORDER"); return e ? atoi(e) : -1; }();
   prm.order = order;
-  if (xf_B) {
-    MVB_REQUIRE(xf_T2 && xf_ids && H >= 3 && W >= 3, "cell_fwd: x-fold needs its tables, ids and a grid of at least 3x3");
-    prm.skip_x = 1;
-  }
-  prm.xs_tab = xs_tab; prm.xs_label = xs_label;
-  if (xs_tab) {
-    MVB_REQUIRE(xs_label && !xf_B && !xr_W && !row_map && fanout <= 1, "cell_fwd: the sparse x path needs its labels and excludes x-fold, the dense x path, row maps and fan-out");
-    prm.skip_x = 1;
-  }
-  prm.xr_in = xr_in; prm.xr_W = xr_W;
-  if (xr_W) {
-    MVB_REQUIRE(xr_in && !xf_B && !row_map && fanout <= 1, "cell_fwd: the dense x path needs its input and excludes x-fold, row maps and fan-out");
-    prm.skip_x = 1;
-  }
   prm.hp_mixed = P_out == kPlanesF16F8;
-  prm.hp_out = reinterpret_cast<__nv_bfloat16*>(hp_out);
-  prm.hp_plane_stride = hp_plane_stride; prm.cpad_out = cpad_out; prm.ch_off_out = ch_off_out;
-  prm.R = R; prm.H = H; prm.W = W; prm.cpad = cpad; prm.forget_bias = forget_bias;
+  prm.hp_out = reinterpret_cast<__nv_bfloat16*>(s.hp_out);
+  prm.hp_plane_stride = s.hp_plane_stride; prm.cpad_out = s.cpad_out; prm.ch_off_out = s.ch_off_out;
+  prm.R = R; prm.H = H; prm.W = W; prm.cpad = cpad; prm.forget_bias = s.forget_bias;
 
   int dev = 0, num_sms = 0;
   MVB_CHECK_CUDA(cudaGetDevice(&dev));
   MVB_CHECK_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
   rc = mixed ? launch_cell<1>(tm, prm, num_sms, multicast, stream) : launch_cell<0>(tm, prm, num_sms, multicast, stream);
-  if (rc || fanout <= 1) return rc;
+  if (rc || !fan) return rc;
   // fan-out stage 2: every parent row -> its K children (c_out / h32_out hold NS * fanout sample rows)
-  const long long warps = NS * H * W;
-  const unsigned blocks = (unsigned)((warps * 32 + 255) / 256);
-  if (mixed) fanout_children_kernel<1><<<blocks, 256, 0, stream>>>(gates_out, col_scale, xf_B, xf_T2, xf_ids, c_in, c_out,
-                                                                    h32_out, NS, fanout, g, forget_bias);
-  else fanout_children_kernel<0><<<blocks, 256, 0, stream>>>(gates_out, col_scale, xf_B, xf_T2, xf_ids, c_in, c_out,
-                                                             h32_out, NS, fanout, g, forget_bias);
+  const unsigned blocks = (unsigned)((NS * H * W * 32 + 255) / 256);      // a warp per parent cell
+  auto children = mixed ? fanout_children_kernel<1> : fanout_children_kernel<0>;
+  children<<<blocks, 256, 0, stream>>>(s.fanout_ws, col_scale, s.xf_B, s.xf_T2, s.xf_ids, s.c_in, s.c_out, s.h32_out,
+                                       NS, s.fanout, g, s.forget_bias);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;

@@ -8,12 +8,25 @@ namespace mvb {
 void count_launch(int n);
 
 // mvb_cell.cu
-int cell_fwd(const void* xh_planes, const void* w_planes, const float* bias, const float* c_in,
-             const int* row_map, float* c_out, float* h32_out, void* hp_out,
-             long long hp_plane_stride, int cpad_out, int ch_off_out, long long NS, int H, int W,
-             int cpad, int P, float forget_bias, float* gates_out, const float* xf_B, const float* xf_T2,
-             const int* xf_ids, int fanout, cudaStream_t stream, const float* xr_in = nullptr,
-             const float* xr_W = nullptr, const float* xs_tab = nullptr, const int* xs_label = nullptr);
+// One ConvLSTM cell step.  Callers value-initialise it (`CellStep s{};`) and set the fields they use; a null pointer is
+// an input not read or an output not written.  At most one x source (x-fold, sparse, dense) replaces the x block.
+struct CellStep {
+  const void *xh, *w;             // operand planes [R, cpad] and packed weights (mvb_pack_cell_weights)
+  const float *bias, *c_in;       // [1024] packed (may be null with x-fold, whose tables fold it in); [R_src, 256]
+  const int* row_map;             // [NS] source sample row of c_in for each sample row (null: identity)
+  float *c_out, *h32_out;         // [R, 256]
+  void* hp_out;                   // operand planes whose h block receives h': plane stride, row pitch, channel offset
+  long long hp_plane_stride; int cpad_out, ch_off_out;
+  long long NS; int H, W, cpad;
+  int planes; float forget_bias;  // planes: format of xh and w | (format of hp_out << 8) when that differs
+  float* gates_out;               // [R, 1024] activated gates for the backward pass (bf16x2 only)
+  const float *xf_B, *xf_T2; const int* xf_ids;   // x-fold: tables [9][1024], [9][25][1024]; arg-max cells [NS]
+  const float* xs_tab; const int* xs_label;       // sparse x: table rows [NS, 9, 1024]; label cells [NS]
+  const float *xr_in, *xr_W;                      // dense x: raw input [NS, H, W, 2] fp32; weights [18][1024]
+  int fanout;                     // > 1: each x-fold row is the parent of `fanout` child rows of c_out / h32_out,
+  float* fanout_ws;               // through the parents' raw accumulators [R, 1024] fp32
+};
+int cell_fwd(const CellStep& s, cudaStream_t stream);
 int cell_xdense_weights(const float* kernel, float* out, cudaStream_t stream);
 int cell_xsparse_weights(const float* kernel, int cx, float* out, cudaStream_t stream);
 int cell_xsparse_table(const float* scene_conv, const int* frame_idx, const int* label, const float* Wx, float* tab,

@@ -107,7 +107,7 @@ class ConvRNNEngine(object):
         getattr(cfg.activation_func, "__name__", "") == "tanh", "kernels implement tanh"
     self.set_weights(weights)
     self._bufs = {}
-    self.cell_events = None   # set to [] to record (tag, cx, start, end) events per cell launch
+    self.cell_events = None   # set to [] to record (tag, (h, w, ns), start, end) events per cell launch
     self._graphs = {}         # forward_graph(): feed signature -> (CUDAGraph, static feeds, static outputs)
     self._graph_seen = set()  # signatures seen once (captured at their second occurrence)
 
@@ -148,35 +148,17 @@ class ConvRNNEngine(object):
   def _state(self, tag, ns, h, w):
     return self._buf((tag, ns, h, w), lambda: ops.alloc_state(ns, h, w, self.device))
 
-  def _cell(self, tag, *args, **kw):
-    """ops.cell_fwd, optionally bracketed by CUDA events on the launching stream (bench.py's
-    live roofline measurement of the dominant kernel)."""
+  def _cell(self, tag, shape, launch, *args, **kw):
+    """launch(*args, **kw): one cell launch of shape (h, w, ns).  With cell_events a list, it is bracketed by CUDA
+    events on the launching stream and (tag, shape, start, end) is appended (bench.py's live roofline measurement of
+    the dominant kernel)."""
     if self.cell_events is None:
-      return ops.cell_fwd(*args, **kw)
+      return launch(*args, **kw)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    ops.cell_fwd(*args, **kw)
+    launch(*args, **kw)
     e1.record()
-    self.cell_events.append((tag, (args[6], args[7], args[8]), e0, e1))   # (h, w, ns)
-
-  def _cell_onehot(self, tag, *args, **kw):
-    """ops.cell_fwd_onehot with the same optional event bracket."""
-    if self.cell_events is None:
-      return ops.cell_fwd_onehot(*args, **kw)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    ops.cell_fwd_onehot(*args, **kw)
-    e1.record()
-    self.cell_events.append((tag, (args[8], args[9], args[10]), e0, e1))   # (h, w, ns)
-
-  def _cell_fanout(self, tag, *args, **kw):
-    if self.cell_events is None:
-      return ops.cell_fwd_onehot_fanout(*args, **kw)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    ops.cell_fwd_onehot_fanout(*args, **kw)
-    e1.record()
-    self.cell_events.append((tag, (args[7], args[8], args[9]), e0, e1))   # (h, w, ns)
+    self.cell_events.append((tag, shape, e0, e1))
 
   # ------------------------------------------------------------------ pieces
   def scene_cnn(self, scene_feat, obs_scene):
@@ -209,15 +191,9 @@ class ConvRNNEngine(object):
         cur, nxt = xh[t % 2], xh[(t + 1) % 2]
         last = t == t_len - 1
         ops.cell_xsparse_table(scene_conv, obs_scene_t[t], labels_t[t], sw.enc_class_xs, table, h, w)
-        ev = None
-        if self.cell_events is not None:
-          ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
-          ev[0].record()
-        ops.cell_fwd_xsparse(cur, sw.enc_class, table, labels_t[t], None if t == 0 else c[t % 2], c[(t + 1) % 2],
-                             h32 if last else None, xh_out if last else nxt, h, w, n)
-        if ev is not None:
-          ev[1].record()
-          self.cell_events.append(("enc_class", (h, w, n), ev[0], ev[1]))
+        self._cell("enc_class", (h, w, n), ops.cell_fwd_xsparse, cur, sw.enc_class, table, labels_t[t],
+                   None if t == 0 else c[t % 2], c[(t + 1) % 2], h32 if last else None, xh_out if last else nxt,
+                   h, w, n)
       return c[t_len % 2], h32
     # a previous call left the label pixels of its last two steps in the x blocks: clear them
     for j in range(2):
@@ -228,8 +204,8 @@ class ConvRNNEngine(object):
       ops.enc_class_input(scene_conv, obs_scene_t[t], labels_t[t],
                           labels_t[t - 2] if t >= 2 else None, cur, h, w)
       last = t == t_len - 1
-      self._cell("enc_class", cur, sw.enc_class, None if t == 0 else c[t % 2], c[(t + 1) % 2],
-                   h32 if last else None, xh_out if last else nxt, h, w, n)
+      self._cell("enc_class", (h, w, n), ops.cell_fwd, cur, sw.enc_class, None if t == 0 else c[t % 2],
+                 c[(t + 1) % 2], h32 if last else None, xh_out if last else nxt, h, w, n)
     return c[t_len % 2], h32
 
   def encode_reg(self, i, obs_reg_t, xh_out):
@@ -246,16 +222,9 @@ class ConvRNNEngine(object):
       for t in range(t_len):
         cur, nxt = xh[t % 2], xh[(t + 1) % 2]
         last = t == t_len - 1
-        if self.cell_events is None:
-          ops.cell_fwd_xdense(cur, pk, sw.enc_reg_xd, obs_reg_t[t], None if t == 0 else c[t % 2], c[(t + 1) % 2],
-                              h32 if last else None, xh_out if last else nxt, h, w, n)
-        else:
-          e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-          e0.record()
-          ops.cell_fwd_xdense(cur, pk, sw.enc_reg_xd, obs_reg_t[t], None if t == 0 else c[t % 2], c[(t + 1) % 2],
-                              h32 if last else None, xh_out if last else nxt, h, w, n)
-          e1.record()
-          self.cell_events.append(("enc_reg", (h, w, n), e0, e1))
+        self._cell("enc_reg", (h, w, n), ops.cell_fwd_xdense, cur, pk, sw.enc_reg_xd, obs_reg_t[t],
+                   None if t == 0 else c[t % 2], c[(t + 1) % 2], h32 if last else None, xh_out if last else nxt,
+                   h, w, n)
       return c[t_len % 2], h32
     xh = self._xh("enc_reg", n, h, w, sw.enc_reg.cpad)
     c = [self._state("encr_c0", n, h, w), self._state("encr_c1", n, h, w)]
@@ -265,8 +234,8 @@ class ConvRNNEngine(object):
       cur, nxt = xh[t % 2], xh[(t + 1) % 2]
       ops.nhwc_to_planes(obs_reg_t[t], cur, 0, h, w, comp=sw.enc_reg.comp)
       last = t == t_len - 1
-      self._cell("enc_reg", cur, sw.enc_reg, None if t == 0 else c[t % 2], c[(t + 1) % 2],
-                   h32 if last else None, xh_out if last else nxt, h, w, n)
+      self._cell("enc_reg", (h, w, n), ops.cell_fwd, cur, sw.enc_reg, None if t == 0 else c[t % 2],
+                 c[(t + 1) % 2], h32 if last else None, xh_out if last else nxt, h, w, n)
     return c[t_len % 2], h32
 
   def decode_class_greedy(self, i, c_enc, h32_enc, first_ids, scene_mean, pred_len):
@@ -287,8 +256,8 @@ class ConvRNNEngine(object):
         ops.gnn_attend_fwd(h_src, scene_mean if self.gnn_scene_in_greedy else None, cur, h, w, n)
       # (no attention: the planes of the previous h already sit in cur's h block)
       # the embedded one_hot(ids_prev) input is folded into table look-ups: nobody writes the x block
-      self._cell_onehot("dec_class", cur, sw.dec_class, sw.dec_class_xf, ids_prev, c_src, c[(t + 1) % 2],
-                        h32, None if cfg.use_gnn else nxt, h, w, n)
+      self._cell("dec_class", (h, w, n), ops.cell_fwd_onehot, cur, sw.dec_class, sw.dec_class_xf, ids_prev, c_src,
+                 c[(t + 1) % 2], h32, None if cfg.use_gnn else nxt, h, w, n)
       c_src, h_src = c[(t + 1) % 2], h32
       ops.head_class_fwd(h32, sw.head_class, logits[t], ids[t], None, None, None, h, w, n,
                          planes=self.planes)
@@ -309,7 +278,7 @@ class ConvRNNEngine(object):
     c_src = c_enc
     for t in range(pred_len):
       cur, nxt = xh[t % 2], xh[(t + 1) % 2]
-      self._cell("dec_reg", cur, sw.dec_reg, c_src, c[(t + 1) % 2], h32, nxt, h, w, n)
+      self._cell("dec_reg", (h, w, n), ops.cell_fwd, cur, sw.dec_reg, c_src, c[(t + 1) % 2], h32, nxt, h, w, n)
       c_src = c[(t + 1) % 2]
       last = t == pred_len - 1
       ops.head_reg_fwd(h32, sw.head_reg, offs[t], None if last else We, None if last else be,
@@ -347,7 +316,8 @@ class ConvRNNEngine(object):
     h32_t0 = self._state("beam_h32_t0", n, h, w)
     logits_t0 = torch.empty((n, v), dtype=torch.float32, device=dev)
     ops.gnn_attend_fwd(h32_enc, scene_mean, xh1[0], h, w, n, beam=1, row_map=None)
-    self._cell_onehot("beam_t0", xh1[0], sw.dec_class, xf, first_ids.contiguous(), c_enc, c_t0, h32_t0, None, h, w, n)
+    self._cell("beam_t0", (h, w, n), ops.cell_fwd_onehot, xh1[0], sw.dec_class, xf, first_ids.contiguous(), c_enc,
+               c_t0, h32_t0, None, h, w, n)
     ops.head_class_fwd(h32_t0, sw.head_class, logits_t0, None, None, None, None, h, w, n, planes=self.planes)
     step_logits[0].copy_(logits_t0.unsqueeze(1).expand(n, b, v))
     h_src, c_src, cur_c = h32_t0, c_t0, 1
@@ -370,12 +340,12 @@ class ConvRNNEngine(object):
         ops.gnn_attend_fwd(h32_t0, scene_mean, xh1[1], h, w, n, beam=1, row_map=None)
         ws = self._buf(("beam_fanout_ws", n, h, w), lambda: torch.empty(
             (ops.halo_rows(n, h, w), 4 * ops.HIDDEN), dtype=torch.float32, device=dev))
-        self._cell_fanout("beam_fanout", xh1[1], sw.dec_class, xf, step_ids[0].view(-1), c_t0, c[1 - cur_c], h32,
-                          h, w, n, b, workspace=ws)
+        self._cell("beam_fanout", (h, w, n), ops.cell_fwd_onehot_fanout, xh1[1], sw.dec_class, xf,
+                   step_ids[0].view(-1), c_t0, c[1 - cur_c], h32, h, w, n, b, workspace=ws)
       else:
         ops.gnn_attend_fwd(h_src, scene_mean, nxt, h, w, ns, beam=b, row_map=row_map)
-        self._cell_onehot("beam", nxt, sw.dec_class, xf, step_ids[time - 1].view(-1), c_src, c[1 - cur_c], h32,
-                          None, h, w, ns, row_map=row_map)
+        self._cell("beam", (h, w, ns), ops.cell_fwd_onehot, nxt, sw.dec_class, xf, step_ids[time - 1].view(-1), c_src,
+                   c[1 - cur_c], h32, None, h, w, ns, row_map=row_map)
       cur_c = 1 - cur_c
       h_src, c_src = h32, c[cur_c]
     out_ids = torch.empty((n, b, pred_len), dtype=torch.int32, device=dev)

@@ -95,6 +95,15 @@ def _planes_arg(packed, xh_next):
   return packed.planes if po == packed.planes else packed.planes | (po << 8)
 
 
+def _hp_out(xh, packed, xh_next):
+  """Checks that `xh` is in the operand format of `packed`, and returns the h-output arguments of the cell entry
+  points: the planes xh_next whose h block receives h' (pointer, plane stride, row pitch, channel offset), or none."""
+  assert xh.shape[2] == packed.cpad and planes_of(xh) == packed.planes
+  if xh_next is None:
+    return None, 0, 0, 0
+  return _p(xh_next), xh_next.stride(0), xh_next.shape[2], xh_next.shape[2] - HIDDEN
+
+
 def alloc_xh(ns, h, w, cpad, planes, device):
   """Zeroed operand planes [2, R, cpad] (either format: the same bytes); halo cells and channel padding must stay
   zero."""
@@ -133,14 +142,9 @@ def cell_fwd(xh, packed, c_in, c_out, h32_out, xh_next, h, w, ns, row_map=None,
              forget_bias=1.0):
   """One ConvLSTM step.  xh_next: operand planes whose h block (channel offset = its cxp)
   receives the bf16 planes of h', or None."""
-  assert xh.shape[2] == packed.cpad and planes_of(xh) == packed.planes
-  if xh_next is not None:
-    stride, cpad_out, off = xh_next.stride(0), xh_next.shape[2], xh_next.shape[2] - HIDDEN
-  else:
-    stride, cpad_out, off = 0, 0, 0
-  _lib.call("mvb_convlstm_cell_fwd", _p(xh), _p(packed.w), _p(packed.bias), _p(c_in),
-            _p(row_map), _p(c_out), _p(h32_out), _p(xh_next), stride, cpad_out, off, ns, h, w,
-            packed.cpad, _planes_arg(packed, xh_next), float(forget_bias), _stream())
+  hp = _hp_out(xh, packed, xh_next)
+  _lib.call("mvb_convlstm_cell_fwd", _p(xh), _p(packed.w), _p(packed.bias), _p(c_in), _p(row_map), _p(c_out),
+            _p(h32_out), *hp, ns, h, w, packed.cpad, _planes_arg(packed, xh_next), float(forget_bias), _stream())
 
 
 class XDense(object):
@@ -155,15 +159,11 @@ class XDense(object):
 def cell_fwd_xdense(xh, packed, xdense, x_in, c_in, c_out, h32_out, xh_next, h, w, ns, forget_bias=1.0):
   """One ConvLSTM step of the regression encoder: h block of `xh` through the tensor cores, the raw 2-channel input
   x_in fp32 [ns,h,w,2] added in fp32 in the epilogue (mvb_convlstm_cell_fwd_xdense); the x block of xh is not read."""
-  assert xh.shape[2] == packed.cpad and planes_of(xh) == packed.planes
+  hp = _hp_out(xh, packed, xh_next)
   assert x_in.dtype == torch.float32 and x_in.is_contiguous() and x_in.numel() == ns * h * w * 2
-  if xh_next is not None:
-    stride, cpad_out, off = xh_next.stride(0), xh_next.shape[2], xh_next.shape[2] - HIDDEN
-  else:
-    stride, cpad_out, off = 0, 0, 0
   _lib.call("mvb_convlstm_cell_fwd_xdense", _p(xh), _p(packed.w), _p(packed.bias), _p(x_in), _p(xdense.W), _p(c_in),
-            _p(c_out), _p(h32_out), _p(xh_next), stride, cpad_out, off, ns, h, w, packed.cpad,
-            _planes_arg(packed, xh_next), float(forget_bias), _stream())
+            _p(c_out), _p(h32_out), *hp, ns, h, w, packed.cpad, _planes_arg(packed, xh_next), float(forget_bias),
+            _stream())
 
 
 class XSparse(object):
@@ -184,14 +184,10 @@ def cell_xsparse_table(scene_conv, frame_idx, label, xsparse, table, h, w):
 def cell_fwd_xsparse(xh, packed, table, label, c_in, c_out, h32_out, xh_next, h, w, ns, forget_bias=1.0):
   """One ConvLSTM step of the class encoder: h block of `xh` through the tensor cores, the one-cell scene-feature
   input added from `table` (cell_xsparse_table) in the epilogue; the x block of xh is not read."""
-  assert xh.shape[2] == packed.cpad and planes_of(xh) == packed.planes
-  if xh_next is not None:
-    stride, cpad_out, off = xh_next.stride(0), xh_next.shape[2], xh_next.shape[2] - HIDDEN
-  else:
-    stride, cpad_out, off = 0, 0, 0
+  hp = _hp_out(xh, packed, xh_next)
   _lib.call("mvb_convlstm_cell_fwd_xsparse", _p(xh), _p(packed.w), _p(packed.bias), _p(table), _p(label), _p(c_in),
-            _p(c_out), _p(h32_out), _p(xh_next), stride, cpad_out, off, ns, h, w, packed.cpad,
-            _planes_arg(packed, xh_next), float(forget_bias), _stream())
+            _p(c_out), _p(h32_out), *hp, ns, h, w, packed.cpad, _planes_arg(packed, xh_next), float(forget_bias),
+            _stream())
 
 
 class XFold(object):
@@ -209,14 +205,10 @@ class XFold(object):
 def cell_fwd_onehot(xh, packed, xf, ids, c_in, c_out, h32_out, xh_next, h, w, ns, row_map=None,
                     forget_bias=1.0):
   """Class-decoder step with the embedded one-hot input folded into table look-ups."""
-  assert xh.shape[2] == packed.cpad and planes_of(xh) == packed.planes
-  if xh_next is not None:
-    stride, cpad_out, off = xh_next.stride(0), xh_next.shape[2], xh_next.shape[2] - HIDDEN
-  else:
-    stride, cpad_out, off = 0, 0, 0
+  hp = _hp_out(xh, packed, xh_next)
   _lib.call("mvb_convlstm_cell_fwd_onehot", _p(xh), _p(packed.w), _p(xf.B), _p(xf.T2), _p(ids), _p(c_in),
-            _p(row_map), _p(c_out), _p(h32_out), _p(xh_next), stride, cpad_out, off, ns, h, w,
-            packed.cpad, _planes_arg(packed, xh_next), float(forget_bias), _stream())
+            _p(row_map), _p(c_out), _p(h32_out), *hp, ns, h, w, packed.cpad, _planes_arg(packed, xh_next),
+            float(forget_bias), _stream())
 
 
 def cell_fwd_onehot_fanout(xh, packed, xf, ids, c_in, c_out, h32_out, h, w, ns, fanout, forget_bias=1.0,
@@ -339,13 +331,9 @@ def beam_backtrace(step_ids, step_parents, step_logits, out_ids, out_logits):
 # --------------------------------------------------------------------------- training (BPTT) ops
 def cell_fwd_train(xh, packed, c_in, c_out, h32_out, xh_next, gates_out, h, w, ns, forget_bias=1.0):
   """cell_fwd that also stores the activated gates [R,1024] for the backward pass."""
-  if xh_next is not None:
-    stride, cpad_out, off = xh_next.stride(0), xh_next.shape[2], xh_next.shape[2] - HIDDEN
-  else:
-    stride, cpad_out, off = 0, 0, 0
-  _lib.call("mvb_convlstm_cell_fwd_train", _p(xh), _p(packed.w), _p(packed.bias), _p(c_in),
-            _p(c_out), _p(h32_out), _p(xh_next), stride, cpad_out, off, _p(gates_out), ns, h, w,
-            packed.cpad, packed.planes, float(forget_bias), _stream())
+  hp = _hp_out(xh, packed, xh_next)
+  _lib.call("mvb_convlstm_cell_fwd_train", _p(xh), _p(packed.w), _p(packed.bias), _p(c_in), _p(c_out), _p(h32_out),
+            *hp, _p(gates_out), ns, h, w, packed.cpad, packed.planes, float(forget_bias), _stream())
 
 
 def pack_dgrad(packed, kernel):
