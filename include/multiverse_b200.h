@@ -363,6 +363,14 @@ int mvb_beam_backtrace(const int32_t* step_ids, const int32_t* step_parents,
                        const float* step_logits, int32_t* out_ids, float* out_logits, int64_t N,
                        int B, int Tp, int V, void* stream);
 
+/* Parent-state gather of the beam decoder without graph attention (use_gnn off: pred_models.py:611-623, then the
+ * gathered h goes straight into the cell): for every sample row s < NS and valid cell, the h block (channels
+ * [cpad_out - 256, cpad_out)) of row s of hp_out <- the f16f8 operand values of h32 row row_map[s] (fp32 halo).
+ * hp_out is an f16f8 operand buffer of NS*(H+1)*(W+1) rows (hp_plane_stride = that times cpad_out); its x block,
+ * channel padding and halo rows are not written. */
+int mvb_beam_gather_h_f16f8(const float* h32, const int32_t* row_map, void* hp_out, int64_t hp_plane_stride,
+                            int cpad_out, int64_t NS, int H, int W, void* stream);
+
 /* ---- f-1 (next row): feed generation on the device (multifuture_inference.py:115-156, preprocess.py:436-475):
  *      traj fp64 [NT,2] frame pixels, centers fp64 [H*W,2] (the caller's scene_grid_centers) ->
  *      labels int32 [NT] (cell of every point), regress fp32 [NT,H,W,2] (point - centre of every cell). */

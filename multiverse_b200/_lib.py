@@ -79,6 +79,7 @@ SIGNATURES = {
     "mvb_min_ade_fde": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp],
     "mvb_beam_nll": [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _vp],
     "mvb_beam_backtrace": [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],
+    "mvb_beam_gather_h_f16f8": [_vp, _vp, _vp, _i64, _i, _i64, _i, _i, _vp],
 }
 _RESTYPES = {"mvb_last_error": C.c_char_p, "mvb_launch_count": C.c_longlong, "mvb_cell_variants_seen": C.c_longlong,
              "mvb_reset_launch_count": None}

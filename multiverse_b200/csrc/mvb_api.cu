@@ -112,7 +112,7 @@ static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s)
 extern "C" {
 
 const char* mvb_last_error(void) { return get_error(); }
-int mvb_abi_version(void) { return 13; }
+int mvb_abi_version(void) { return 14; }
 int mvb_cell_last_variant(void) { return cell_last_variant(); }
 long long mvb_cell_variants_seen(int reset) { return (long long)cell_variants_seen(reset); }
 long long mvb_launch_count(void) { return g_launches; }
@@ -402,6 +402,10 @@ int mvb_beam_backtrace(const int32_t* step_ids, const int32_t* step_parents,
                        int B, int Tp, int V, void* stream) {
   return beam_backtrace(step_ids, step_parents, step_logits, out_ids, out_logits, N, B, Tp, V,
                         S(stream));
+}
+int mvb_beam_gather_h_f16f8(const float* h32, const int32_t* row_map, void* hp_out, int64_t hp_plane_stride,
+                            int cpad_out, int64_t NS, int H, int W, void* stream) {
+  return beam_gather_h(h32, row_map, hp_out, hp_plane_stride, cpad_out, NS, H, W, S(stream));
 }
 
 }  // extern "C"

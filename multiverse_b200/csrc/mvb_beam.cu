@@ -281,6 +281,46 @@ int beam_step(const float* logits, const float* score_in, float* score_out, int*
   return MVB_OK;
 }
 
+// Parent-state gather of the beam decoder without graph attention (:611-623 then straight into the cell, :631-654
+// with use_gnn off): h block of the children's f16f8 operand rows <- the fp32 h of their parents' rows.  The cell's
+// A stage loads 2-D TMA boxes of consecutive halo rows, and one box spans several per-sample images, so the gather
+// cannot happen there: this kernel writes it.  One warp per valid cell, 8 channels per lane (the layout the graph
+// attention writes, packed cvt conversions); the x block, the channel padding and the halo rows are never written.
+__global__ void __launch_bounds__(256)
+beam_gather_h_kernel(const float* __restrict__ h32, const int* __restrict__ row_map, __nv_bfloat16* __restrict__ hp_out,
+                     long long plane_stride, int cpad_out, long long cells, Grid g) {
+  const int lane = threadIdx.x & 31;
+  const long long cell = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (cell >= cells) return;
+  const long long hw = (long long)g.H * g.W;
+  const long long s = cell / hw;
+  const int p = (int)(cell - s * hw);
+  const int y = p / g.W, x = p - y * g.W;
+  const long long off = (long long)y * g.Wp + x;
+  const float4* src = reinterpret_cast<const float4*>(h32 + ((long long)row_map[s] * g.S + off) * kHidden + lane * 8);
+  const float4 a = __ldg(src), b = __ldg(src + 1);
+  const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+  store_f16f8_x8(hp_out, plane_stride, s * g.S + off, cpad_out - kHidden + lane * 8, cpad_out, v);
+}
+
+int beam_gather_h(const float* h32, const int* row_map, void* hp_out, long long hp_plane_stride, int cpad_out,
+                  long long NS, int H, int W, cudaStream_t stream) {
+  MVB_REQUIRE(h32 && row_map && hp_out, "beam_gather_h: null pointer");
+  MVB_REQUIRE(NS > 0 && H > 0 && W > 0, "beam_gather_h: bad sizes NS=%lld H=%d W=%d", NS, H, W);
+  MVB_REQUIRE(cpad_out >= kHidden && cpad_out % 32 == 0,
+              "beam_gather_h: cpad_out=%d is not an operand pitch (a multiple of 32, >= 256)", cpad_out);
+  const Grid g = make_grid(H, W);
+  MVB_REQUIRE(hp_plane_stride == NS * g.S * (long long)cpad_out,
+              "beam_gather_h: plane stride %lld is not NS*(H+1)*(W+1)*cpad_out", hp_plane_stride);
+  const long long cells = NS * H * W;
+  MVB_REQUIRE((cells + 7) / 8 < (1ll << 31), "beam_gather_h: NS=%lld too large", NS);
+  beam_gather_h_kernel<<<(unsigned)((cells + 7) / 8), 256, 0, stream>>>(
+      h32, row_map, reinterpret_cast<__nv_bfloat16*>(hp_out), hp_plane_stride, cpad_out, cells, g);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
 int beam_backtrace(const int* step_ids, const int* step_parents, const float* step_logits,
                    int* out_ids, float* out_logits, long long N, int B, int Tp, int V,
                    cudaStream_t stream) {

@@ -83,6 +83,8 @@ int beam_step(const float* logits, const float* score_in, float* score_out, int*
 int beam_backtrace(const int* step_ids, const int* step_parents, const float* step_logits,
                    int* out_ids, float* out_logits, long long N, int B, int Tp, int V,
                    cudaStream_t stream);
+int beam_gather_h(const float* h32, const int* row_map, void* hp_out, long long hp_plane_stride, int cpad_out,
+                  long long NS, int H, int W, cudaStream_t stream);
 
 // mvb_metrics.cu
 int min_ade_fde(const float* pred, const float* gt, const int* gt_len, double* ade_err, int* ade_idx, double* fde,

@@ -12,11 +12,13 @@ arithmetic step is a kernel of the C-ABI library:
                                                      mvb_head_class_fwd (logits+argmax)]
   regression decoder (:298-305)              -> Tp x [mvb_convlstm_cell_fwd, mvb_head_reg_fwd]
   beam decoder (:474-806)                    -> Tp x [mvb_head_class_fwd, mvb_beam_step,
-                                                     mvb_gnn_attend_fwd,
+                                                     mvb_gnn_attend_fwd (mvb_beam_gather_h_f16f8
+                                                     without use_gnn),
                                                      mvb_convlstm_cell_fwd_onehot] + mvb_beam_backtrace
 
-The (c,h) gather by parent beam (:611-623) is never a copy: mvb_beam_step emits a row map that
-the next GNN / cell launch reads its state through.
+The (c,h) gather by parent beam (:611-623) is never a copy of c: mvb_beam_step emits a row map that
+the next GNN / cell launch reads its state through (without use_gnn, mvb_beam_gather_h_f16f8 reads h
+through it into the cell's operands).
 """
 from __future__ import annotations
 
@@ -91,8 +93,9 @@ class ConvRNNEngine(object):
     self.device = device or torch.device("cuda", torch.cuda.current_device())
     self.planes = planes
     # The class decoder's cell reads only what the graph attention writes (its one-hot input is folded into table
-    # look-ups), so that producer/consumer pair switches to the f16f8 operand format as a unit.
-    self.fast_class = self.ALLOW_F16F8 and bool(cfg.use_gnn)
+    # look-ups), so that producer/consumer pair switches to the f16f8 operand format as a unit.  Without the attention,
+    # the beam decoder's parent gather (ops.beam_gather_h) is that producer.
+    self.fast_class = self.ALLOW_F16F8 and bool(cfg.use_gnn or cfg.use_beam_search)
     self.class_planes = ops.PLANES_F16F8 if self.fast_class else self.planes
     # class encoder and regression decoder (inputs in (-1,1): tanh outputs) use the same format; the regression
     # ENCODER keeps bf16 planes: its raw pixel offsets (+-1.9e3) need the compensated x block.
@@ -309,15 +312,19 @@ class ConvRNNEngine(object):
     # N*K) and the first selection's children read it through row_map = sample index: same values, 1/K of
     # the work for 1 of the Tp steps.  The embedded one-hot input of every step is folded into table
     # look-ups (ops.cell_fwd_onehot).
-    if not cfg.use_gnn:
-      raise NotImplementedError("beam search without use_gnn is not wired (no published config)")
+    # Without the graph attention (use_gnn off) the state goes straight into the cell: the encoder has written its
+    # last h into xh1[0] (forward()), the time-0 cell writes its h into xh1[1] for the fan-out, and from time 2 on
+    # ops.beam_gather_h copies the parents' h rows into the children's operand rows.
+    assert cfg.use_gnn or self.class_planes == ops.PLANES_F16F8, \
+        "beam search without use_gnn runs on f16f8 operands (inference engine)"
     xh1 = self._xh("beam_t0", n, h, w, sw.dec_class.cpad, self.class_planes)
     c_t0 = self._state("beam_c_t0", n, h, w)
     h32_t0 = self._state("beam_h32_t0", n, h, w)
     logits_t0 = torch.empty((n, v), dtype=torch.float32, device=dev)
-    ops.gnn_attend_fwd(h32_enc, scene_mean, xh1[0], h, w, n, beam=1, row_map=None)
+    if cfg.use_gnn:
+      ops.gnn_attend_fwd(h32_enc, scene_mean, xh1[0], h, w, n, beam=1, row_map=None)
     self._cell("beam_t0", (h, w, n), ops.cell_fwd_onehot, xh1[0], sw.dec_class, xf, first_ids.contiguous(), c_enc,
-               c_t0, h32_t0, None, h, w, n)
+               c_t0, h32_t0, None if cfg.use_gnn else xh1[1], h, w, n)
     ops.head_class_fwd(h32_t0, sw.head_class, logits_t0, None, None, None, None, h, w, n, planes=self.planes)
     step_logits[0].copy_(logits_t0.unsqueeze(1).expand(n, b, v))
     h_src, c_src, cur_c = h32_t0, c_t0, 1
@@ -337,13 +344,17 @@ class ConvRNNEngine(object):
         # every child's parent is its sample's single t0 row: the K children share the graph-attended h and c and
         # differ only in the selected cell, i.e. in the folded table rows -> attention and GEMM once per sample,
         # the cell epilogue fans the K children out (ops.cell_fwd_onehot_fanout; 1/K of the step's MMAs)
-        ops.gnn_attend_fwd(h32_t0, scene_mean, xh1[1], h, w, n, beam=1, row_map=None)
+        if cfg.use_gnn:
+          ops.gnn_attend_fwd(h32_t0, scene_mean, xh1[1], h, w, n, beam=1, row_map=None)
         ws = self._buf(("beam_fanout_ws", n, h, w), lambda: torch.empty(
             (ops.halo_rows(n, h, w), 4 * ops.HIDDEN), dtype=torch.float32, device=dev))
         self._cell("beam_fanout", (h, w, n), ops.cell_fwd_onehot_fanout, xh1[1], sw.dec_class, xf,
                    step_ids[0].view(-1), c_t0, c[1 - cur_c], h32, h, w, n, b, workspace=ws)
       else:
-        ops.gnn_attend_fwd(h_src, scene_mean, nxt, h, w, ns, beam=b, row_map=row_map)
+        if cfg.use_gnn:
+          ops.gnn_attend_fwd(h_src, scene_mean, nxt, h, w, ns, beam=b, row_map=row_map)
+        else:
+          ops.beam_gather_h(h_src, row_map, nxt, h, w, ns)
         self._cell("beam", (h, w, ns), ops.cell_fwd_onehot, nxt, sw.dec_class, xf, step_ids[time - 1].view(-1), c_src,
                    c[1 - cur_c], h32, None, h, w, ns, row_map=row_map)
       cur_c = 1 - cur_c
@@ -394,7 +405,9 @@ class ConvRNNEngine(object):
       if ("class", i) in run:
         labels = feeds["grid_obs_labels"][i].to(torch.int32)
         labels_t = labels.t().contiguous()
-        xh_dec = self._xh("dec_class", n, h, w, sw.dec_class.cpad, self.class_planes)
+        # without the graph attention the encoder writes its last h straight into the decoder's first operands
+        xh_dec = self._xh("beam_t0" if cfg.use_beam_search and not cfg.use_gnn else "dec_class", n, h, w,
+                          sw.dec_class.cpad, self.class_planes)
         c_e, h_e = self.encode_class(i, convs[i], obs_scene_t, labels_t,
                                      None if cfg.use_gnn else xh_dec[0])
         if cfg.use_beam_search:

@@ -321,6 +321,15 @@ def beam_step(logits, score_in, score_out, ids_out, parents_out, row_map_out, n,
             int(diverse), float(lg), _stream())
 
 
+def beam_gather_h(h32, row_map, xh_next, h, w, ns):
+  """h block of the f16f8 operand rows of xh_next <- the fp32 h32 rows of each row's parent row_map[s] (the beam
+  decoder's state gather without graph attention)."""
+  assert planes_of(xh_next) == PLANES_F16F8, "beam_gather_h writes the f16f8 operand format only"
+  assert xh_next.shape[1] == halo_rows(ns, h, w) and row_map.dtype == torch.int32 and row_map.numel() == ns
+  _lib.call("mvb_beam_gather_h_f16f8", _p(h32), _p(row_map), _p(xh_next), xh_next.stride(0), xh_next.shape[2], ns,
+            h, w, _stream())
+
+
 def beam_backtrace(step_ids, step_parents, step_logits, out_ids, out_logits):
   tp, n, b = step_ids.shape
   v = step_logits.shape[-1]
