@@ -5,7 +5,8 @@ regenerate the inputs from the seeds in cases.REFEXEC_* and hold the oracle to t
 (tests/test_reference_exec_cpu.py, tests/test_simaug_reference_cpu.py).  Large arrays are stored as a strided sample
 (cases.sample); everything is fp64 except where a test's bar allows fp32.
 
-  python tests/golden/make_golden_refexec.py       (needs the reference repository; MVB_REFERENCE_ROOT)
+  python tests/golden/make_golden_refexec.py          (needs the reference repository; MVB_REFERENCE_ROOT)
+  python tests/golden/make_golden_refexec.py native   (refexec_native.npz alone)
 """
 import os
 import sys
@@ -54,6 +55,30 @@ def train_golden():
     g["grad_absmax/" + k] = np.float64(np.abs(got["grads"][k]).max())
     g["updated/" + k] = cases.sample(got["updated"][k])
   return g
+
+
+def native_golden():
+  """refexec_native.npz: the published configuration (cases.REFEXEC_NATIVE: scene 36x64, grids 18x32 and 9x16):
+  the greedy two-scale forward (forward/...) and one training step with Trainer's Adadelta at init_lr 0.3
+  (train/...; per-variable samples of at most cases.NATIVE_TRAIN_SAMPLE elements)."""
+  cfg, w, f = cases.refexec_native_inputs()
+  out = X.forward(cfg, w, f)
+  g = {"forward/variables": np.array(sorted(out["variables"]))}
+  for i in range(len(cfg.scene_grids)):
+    for key in ("grid_pred_decoded", "grid_pred_reg_decoded", "scene_convs"):
+      g["forward/%s_%d" % (key, i)] = cases.sample(out[key][i])
+      g["forward/%s_%d_absmax" % (key, i)] = np.float64(np.abs(out[key][i]).max())
+  got = X.train_step(cfg, w, f, **cases.REFEXEC_NATIVE[2])
+  g.update({"train/loss": np.float64(got["loss"]), "train/wd_loss": np.float64(got["wd_loss"]),
+            "train/pred_grid_loss": np.asarray(got["pred_grid_loss"], np.float64),
+            "train/global_step": np.int64(got["global_step"]), "train/variables": np.array(sorted(got["grads"]))})
+  for k in got["grads"]:
+    g["train/grad/" + k] = cases.sample(got["grads"][k], cases.NATIVE_TRAIN_SAMPLE)
+    g["train/grad_absmax/" + k] = np.float64(np.abs(got["grads"][k]).max())
+    g["train/updated/" + k] = cases.sample(got["updated"][k], cases.NATIVE_TRAIN_SAMPLE)
+  path = os.path.join(GOLD, "refexec_native.npz")
+  np.savez_compressed(path, source=np.array("reference_exec"), **g)
+  print("refexec_native.npz", os.path.getsize(path), "bytes")
 
 
 def attack_golden():
@@ -143,7 +168,12 @@ def main():
                       **attack_golden())
   for f in ("refexec_forward.npz", "refexec_train.npz", "refexec_attack.npz"):
     print(f, os.path.getsize(os.path.join(GOLD, f)), "bytes")
+  native_golden()
 
 
 if __name__ == "__main__":
-  main()
+  if sys.argv[1:] == ["native"]:
+    assert X.available(), "the reference repository is needed to make this golden"
+    native_golden()
+  else:
+    main()

@@ -1,7 +1,8 @@
 # coding=utf-8
 """Every kernel of the inference rollout around the ConvLSTM cell, element by element, at the batch the benchmark
 decodes: the K = 20 beam decoder of 512 trajectories on the 36x18 grid (10 240 beam rows per step, f16f8 operands)
-and the greedy two-scale decoder of 256 trajectories on 36x18 and 18x9; then the feed and post-decode kernels and the
+and the greedy two-scale decoder of 256 trajectories on 36x18 and 18x9 (and on the 9x16 grid of the published 36x64
+scene, whose encoders run the f16f8 pair kernel at that batch); then the feed and post-decode kernels and the
 evaluation metrics at that batch.
 
 The unit tests of test_parity_gpu.py run these kernels on a handful of rows, and the at-size rollout tests compare
@@ -30,7 +31,7 @@ import pytest
 import torch
 
 import cases
-from test_kernels_atsize_gpu import TIGHT, _taps, halo_bits, inner, ref_cell, ref_onehot_emb, rel
+from test_kernels_atsize_gpu import TIGHT, _taps, halo_bits, inner, m_tiles, num_sms, ref_cell, ref_onehot_emb, rel
 from test_train_atsize_gpu import CLAMPED, gen, on, ref_emb, ref_gnn, ref_head, ref_onehot, report
 from oracle import multiverse_ref as R
 
@@ -49,6 +50,7 @@ C4 = dict(use_grids=[True, False], use_beam_search=True, beam_size=20, diverse_b
           fix_num_timestep=1)
 C3 = dict(use_grids=[True, True])
 NATIVE = dict(C4, scene_h=36, scene_w=64)         # K = 20 on the native 18x32 grid
+NATIVE_C3 = dict(C3, scene_h=36, scene_w=64)      # greedy two-scale on the native 18x32 and 9x16 grids
 N_C4, N_C3 = 512, 256
 
 
@@ -226,7 +228,7 @@ def encoded(dev, over, n, seed):
   """ConvRNNEngine of a benchmark config (synthetic.make_config(**over), synthetic.make_weights) and n trajectories of
   synthetic.make_feeds through the scene CNN and both encoders.  Per used scale: the class encoder's c / h (halo
   layout), the scene mean the graph attention reads, the last observed cell, the regression encoder's h and the last
-  observed offsets (what the regression decoder embeds first)."""
+  observed offsets (what the regression decoder embeds first), and the cell variants the scale's encoders ran."""
   from multiverse_b200 import ops, synthetic
   from multiverse_b200.engine import ConvRNNEngine
   cfg = synthetic.make_config(batch_size=n, **over)
@@ -241,13 +243,25 @@ def encoded(dev, over, n, seed):
     if not cfg.use_grids[i]:
       continue
     lab_t = on(dev, f["grid_obs_labels"][i]).t().contiguous()
+    ops.cell_variants_seen(reset=True)
     c, h32 = eng.encode_class(i, convs[i], obs_t, lab_t, None)
     reg_t = on(dev, f["grid_obs_regress"][i]).transpose(0, 1).contiguous()
     xr = ops.alloc_xh(n, h, w, eng.scales[i].dec_reg.cpad, eng.fast_planes, dev)
     _, hr = eng.encode_reg(i, reg_t, xr)
+    torch.cuda.synchronize()
     out[i] = dict(c=c.clone(), h=h32.clone(), mean=means[i], last_label=lab_t[-1].contiguous(), h_reg=hr.clone(),
-                  reg_last=reg_t[-1].contiguous())
+                  reg_last=reg_t[-1].contiguous(), variants=ops.cell_variants_seen())
   return out
+
+
+def assert_encoder_variant(enc, i, n):
+  """The encoders of scale i ran the f16f8 cell, as the CTA-pair kernel from 2 x SMs M tiles up (single-CTA below)."""
+  from multiverse_b200 import ops
+  h, w = enc["cfg"].scene_grids[i]
+  want = (ops.PLANES_F16F8, m_tiles(n, h, w) >= 2 * num_sms())
+  assert enc[i]["variants"] == {want}, "the encoders of %dx%d n%d ran %s, expected %s" % (
+      h, w, n, sorted(enc[i]["variants"]), want)
+  return "f16f8 %s, %d M tiles" % ("pair" if want[1] else "single-CTA", m_tiles(n, h, w))
 
 
 def beam_state(dev, over, n, seed):
@@ -315,6 +329,7 @@ GNN_CASES = {
     "c3_36x18": (C3, N_C3, 0, False),
     "c3_18x9": (C3, N_C3, 1, False),
     "native_18x32_k20": (NATIVE, 8, 0, True),
+    "native_c3_9x16": (NATIVE_C3, N_C3, 1, False),
 }
 
 
@@ -340,7 +355,7 @@ def test_gnn_into_f16f8_planes_at_size(dev, case):
   else:
     enc = encoded(dev, over, n, 510 + i)
     h, w = enc["cfg"].scene_grids[i]
-    b, rm, order = 1, None, ""
+    b, rm, order = 1, None, "; encoders ran " + assert_encoder_variant(enc, i, n)
     src, mean = enc[i]["h"], enc[i]["mean"].clone()
     del enc
   ns = n * b
@@ -373,13 +388,14 @@ def test_class_head_at_beam_rows(dev):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("i", [0, 1], ids=["36x18", "18x9"])
-def test_class_head_ids_and_f16f8_feedback(dev, i):
+@pytest.mark.parametrize("over,i", [(C3, 0), (C3, 1), (NATIVE_C3, 1)], ids=["36x18", "18x9", "9x16"])
+def test_class_head_ids_and_f16f8_feedback(dev, over, i):
   """head_class_fwd on 256 greedy rows with its arg-max ids and the embedded one-hot of the ids written as f16f8 x
   planes; a sentinel in the h block must survive, the halo must stay zero."""
   from multiverse_b200 import ops
-  enc = encoded(dev, C3, N_C3, 530)
+  enc = encoded(dev, over, N_C3, 530)
   h, w = enc["cfg"].scene_grids[i]
+  variant = assert_encoder_variant(enc, i, N_C3)
   sw, hs = enc["eng"].scales[i], enc[i]["h"]
   We, be = sw.emb_class
   n = N_C3
@@ -397,13 +413,14 @@ def test_class_head_ids_and_f16f8_feedback(dev, i):
   emb = ref_emb(ref_onehot(ids, h, w), We.double(), be.double())
   errs = {"logits": rel(logits, ref), "one-hot emb planes": rel(decoded(xh, n, h, w, slice(0, n))[..., :E], emb)}
   assert block_intact(xh, n, h, w, "h") and halo_bits(xh, n, h, w) == 0
-  report("class head %dx%d, %d rows, ids kept %.3f (top-2 gap > 10 x fp32 error)" % (h, w, n, float(clear.float().mean())),
-         errs)
+  report("class head %dx%d, %d rows (encoders ran %s), ids kept %.3f (top-2 gap > 10 x fp32 error)"
+         % (h, w, n, variant, float(clear.float().mean())), errs)
   assert float(clear.float().mean()) >= 0.9
   assert errs["logits"] < FTOL and errs["one-hot emb planes"] < F8TOL
 
 
-REG_CASES = {"c4_36x18": (C4, N_C4, 0), "c3_36x18": (C3, N_C3, 0), "c3_18x9": (C3, N_C3, 1)}
+REG_CASES = {"c4_36x18": (C4, N_C4, 0), "c3_36x18": (C3, N_C3, 0), "c3_18x9": (C3, N_C3, 1),
+             "native_c3_9x16": (NATIVE_C3, N_C3, 1)}
 
 
 @pytest.mark.gpu
@@ -416,6 +433,7 @@ def test_reg_head_and_dense_embedding_into_f16f8(dev, case):
   over, n, i = REG_CASES[case]
   enc = encoded(dev, over, n, 540 + i)
   h, w = enc["cfg"].scene_grids[i]
+  variant = assert_encoder_variant(enc, i, n)
   sw, hs, x0 = enc["eng"].scales[i], enc[i]["h_reg"], enc[i]["reg_last"]
   We, be = sw.emb_reg
   cpad = ops.cell_cpad(E)
@@ -437,7 +455,7 @@ def test_reg_head_and_dense_embedding_into_f16f8(dev, case):
   errs["first input, beyond fp32 summation"] = float(((got - ref).abs() - fp32_emb_bound(x0, We, be, ref)).clamp(min=0).max()
                                                      / ref.abs().max())
   assert block_intact(xh0, n, h, w, "h") and halo_bits(xh0, n, h, w) == 0
-  report("regression feedback %s: %d rows of %dx%d" % (case, n, h, w), errs)
+  report("regression feedback %s: %d rows of %dx%d (encoders ran %s)" % (case, n, h, w, variant), errs)
   assert errs["offsets"] < FTOL
   assert errs["dense emb planes"] < F8TOL and errs["first input, beyond fp32 summation"] < F8TOL
 

@@ -7,7 +7,9 @@ kernel only.  Which kernel runs, and how many tiles each CTA loops over, depends
   - the cell runs its CTA-pair kernel (two CTAs of a cluster share every weight tile by TMA multicast) from
     2 x (number of SMs) M tiles of 128 rows up; with an odd count, rank 1 of the last pair owns a tile wholly past R;
   - grids of 31 columns and more leave room for three weight slots instead of four; W = 62 fills the A stage (256 rows);
-  - cell_dgrad loops over up to 11 tiles per CTA, cell_wgrad_direct splits K (the rows) over 5 or 2 fp32 slabs.
+  - cell_dgrad loops over up to 11 tiles per CTA, cell_wgrad_direct splits K (the rows) over 5 or 2 fp32 slabs; both
+    shift the taps by the padded row width W + 1, which the training micro-batch runs at 19 (36x18), 33 (18x32) and
+    17 (9x16).
 Here every output is compared on the full tensors with an fp64 reference computed by torch on the same device
 (ref_cell / ref_cell_grads: no multiverse_b200 kernel involved), which the CPU test of this file pins to the oracle.
 
@@ -364,13 +366,25 @@ def test_cell_refuses_a_grid_wider_than_the_a_stage(dev):
   assert ops.launch_count() == 0
 
 
+def check_fwd_train_pair(dev, h, w, seed):
+  """cell_fwd_train (P = 2, gates stored for the backward) under the pair kernel with an odd number of M tiles."""
+  ns = pair_ns(h, w, odd=True)
+  d = cell_inputs(dev, ns, h, w, 32, seed=seed)
+  out = run_fwd(d, 2, train=True)
+  check_fwd("pair fwd_train %dx%d n%d" % (h, w, ns), ns, h, w, out,
+            ref_cell(d["x"], d["h"], d["c"], d["kernel"], d["bias"]), 2, pair=True)
+
+
 @pytest.mark.gpu
 def test_cell_fwd_train_pair_stores_the_gates(dev):
-  ns = pair_ns(36, 18, odd=True)
-  d = cell_inputs(dev, ns, 36, 18, 32, seed=105)
-  out = run_fwd(d, 2, train=True)
-  check_fwd("pair fwd_train n%d" % ns, ns, 36, 18, out, ref_cell(d["x"], d["h"], d["c"], d["kernel"], d["bias"]),
-            2, pair=True)
+  """On 36x18: 4 weight slots."""
+  check_fwd_train_pair(dev, 36, 18, seed=105)
+
+
+@pytest.mark.gpu
+def test_cell_fwd_train_pair_stores_the_gates_on_18x32(dev):
+  """On the published scene's 18x32 grid, where the bf16 x 2 ring has room for 3 weight slots only."""
+  check_fwd_train_pair(dev, 18, 32, seed=106)
 
 
 def _onehot_case(dev, ns, h, w, seed):
@@ -614,16 +628,26 @@ def check_backward(tag, ns, h, w, o, ref):
   assert torch.equal(o["dwp_again"], o["dwp"]), "the weight gradient differs between two runs"
 
 
+# the training micro-batch's grids: the benchmark's 36x18, the published 18x32 and 9x16 (TRAINING.md's scene 36x64)
+BWD_GRIDS = [(36, 18), (18, 32), (9, 16)]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", sorted(BWD_CELLS))
-def test_cell_backward_at_training_size(dev, name):
-  """Micro-batch 128 of 36x18 (89 984 halo rows, 703 M tiles): the forward runs the pair kernel with stored gates,
-  dgrad loops over 5-11 tiles per CTA, wgrad splits the rows over 5 (cpad 288) or 2 (cpad 320) slabs."""
-  ns, h, w = 128, 36, 18
-  o, ref = run_backward(dev, name, ns, h, w, seed=120 + BWD_CELLS[name][0])
-  assert m_tiles(ns, h, w) >= 2 * num_sms()
-  assert o["variant"] == 2 * 2 + 1, "the forward ran %s, not the P=2 pair kernel" % variant_name(o["variant"])
-  check_backward("backward %s n%d" % (name, ns), ns, h, w, o, ref)
+@pytest.mark.parametrize("name,grid", [(n, g) for g in BWD_GRIDS for n in sorted(BWD_CELLS)],
+                         ids=[n if g == (36, 18) else "%s-%dx%d" % ((n,) + g) for g in BWD_GRIDS for n in sorted(BWD_CELLS)])
+def test_cell_backward_at_training_size(dev, name, grid):
+  """Micro-batch 128 of 36x18 (89 984 halo rows, 703 M tiles), of 18x32 (80 256 rows, 627 M tiles: the 3-slot ring,
+  dgrad / wgrad shift taps by 33 rows) and of 9x16 (21 760 rows, 170 M tiles).  The forward stores the gates under
+  the pair kernel from 2 x SMs M tiles up (36x18, 18x32 on an H100), under the single-CTA kernel in strided order
+  below (9x16); dgrad loops over several tiles per CTA, wgrad splits the rows over 5 (cpad 288) or 2 (cpad 320)
+  slabs.  The 36x18 cases are named by the cell alone."""
+  ns = 128
+  h, w = grid
+  o, ref = run_backward(dev, name, ns, h, w, seed=120 + BWD_CELLS[name][0] + (0 if grid == (36, 18) else h + w))
+  pair = m_tiles(ns, h, w) >= 2 * num_sms()
+  assert o["variant"] == 2 * 2 + int(pair), "the forward ran %s, expected %s" % (
+      variant_name(o["variant"]), variant_name(2 * 2 + int(pair)))
+  check_backward("backward %s %dx%d n%d" % (name, h, w, ns), ns, h, w, o, ref)
 
 
 @pytest.mark.gpu

@@ -111,3 +111,47 @@ def test_reference_training_step_equals_oracle():
     want = w[k].astype(np.float64) - lr * upd
     assert np.abs(got["updated/" + k] - cases.sample(want)).max() < 1e-12, k
   assert int(got["global_step"]) == 1
+
+
+def test_reference_native_two_scale_forward_equals_oracle():
+  """The published scene 36x64 (grids 18x32 and 9x16, the only ones wider than tall), greedy decode of both scales
+  with graph attention: class logits, offsets and scene convolutions (tests/golden/refexec_native.npz)."""
+  cfg, w, f = cases.refexec_native_inputs()
+  assert cfg.scene_grids == [(18, 32), (9, 16)] and cfg.use_grids == [True, True]
+  ref = R.forward(cfg, w, f, np.float64)
+  g = gold("refexec_native.npz")
+  assert set(g["forward/variables"]) - {"global_step"} == set(w.keys())
+  for i in range(2):
+    for k in ("grid_pred_decoded", "grid_pred_reg_decoded", "scene_convs"):
+      kk = "forward/%s_%d" % (k, i)
+      assert abs(np.abs(ref[k][i]).max() - g[kk + "_absmax"]) <= TOL * g[kk + "_absmax"], kk
+      assert np.abs(cases.sample(ref[k][i]) - g[kk]).max() <= TOL * g[kk + "_absmax"], kk
+
+
+def test_reference_native_training_step_equals_oracle():
+  """TRAINING.md's training step on the 36x64 scene: both scales, --train_w_onehot, loss weights 1.0 / 0.2, weight
+  decay 0.001 and one Adadelta train_op at --init_lr 0.3: the losses, the clipped gradient of every variable and the
+  updated variables against the oracle's torch-autograd restatement and the closed-form update."""
+  from oracle import multiverse_ref_torch as RT
+  cfg, w, f = cases.refexec_native_inputs()
+  opts = cases.REFEXEC_NATIVE[2]
+  assert (cfg.grid_loss_weight, cfg.grid_reg_loss_weight, cfg.wd) == (
+      opts["grid_loss_weight"], opts["grid_reg_loss_weight"], opts["wd"])
+  got = gold("refexec_native.npz")
+  tot, losses, wd, grads = RT.loss_and_grads(cfg, w, f)
+  assert abs(float(got["train/loss"]) - tot) < 1e-11 * abs(tot)
+  assert abs(float(got["train/wd_loss"]) - wd) < 1e-12 * wd
+  assert len(losses) == 4 and np.abs(got["train/pred_grid_loss"] - np.array(losses)).max() < 1e-11
+  assert set(got["train/variables"]) == set(w.keys()) == set(grads)
+  lr = opts["init_lr"] * 1.0 * 0.95 ** 0        # init_lr * emb_lr * decay^(floor(step/decay_steps)), step 0
+  smp = lambda a: cases.sample(a, cases.NATIVE_TRAIN_SAMPLE)
+  for k, g in grads.items():
+    gc = np.clip(g, -10.0, 10.0)
+    scale = max(np.abs(gc).max(), 1e-30)
+    assert abs(float(got["train/grad_absmax/" + k]) - np.abs(gc).max()) <= 1e-10 * scale, k
+    assert np.abs(got["train/grad/" + k] - smp(gc)).max() <= 1e-10 * scale, k
+    acc = 0.05 * gc * gc                                  # rho=.95, zero slots, eps=1e-8
+    upd = np.sqrt(1e-8) / np.sqrt(acc + 1e-8) * gc
+    want = w[k].astype(np.float64) - lr * upd
+    assert np.abs(got["train/updated/" + k] - smp(want)).max() < 1e-12, k
+  assert int(got["train/global_step"]) == 1

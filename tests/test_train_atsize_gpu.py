@@ -1,6 +1,8 @@
 # coding=utf-8
 """Every kernel of the training step around the ConvLSTM cell, element by element, at the micro-batch the training
-workload runs (128 trajectories on the 36x18 and 18x9 grids), and the whole-model gradient at that micro-batch.
+workload runs (128 trajectories on the 36x18 and 18x9 grids of the benchmark's 72x36 scene, and on the 18x32 and 9x16
+grids of the published 36x64 scene, the only grids wider than tall), and the whole-model gradient at that micro-batch
+on both configurations.
 
 The unit tests of test_train_gpu.py run these kernels on 3 samples of toy grids.  Three kinds of code run only at
 size:
@@ -40,7 +42,11 @@ HID = 256
 E = 32           # grid embedding size
 NS = 128         # the training micro-batch
 T_OBS, T_PRED = 8, 12
-GRIDS = [(36, 18), (18, 9)]
+GRIDS = [(36, 18), (18, 9)]              # the benchmark's scene 72x36, strides 2,4
+NATIVE_GRIDS = [(18, 32), (9, 16)]        # the published scene 36x64 (TRAINING.md), strides 2,4
+KERNEL_GRIDS = GRIDS + NATIVE_GRIDS
+KERNEL_GRID_IDS = ["%dx%d" % g for g in KERNEL_GRIDS]
+SCENES = {"72x36": dict(), "36x64": dict(scene_h=36, scene_w=64)}     # synthetic.make_config overrides
 SENTINEL = 1234.5
 
 
@@ -243,7 +249,7 @@ def report(tag, errs):
 
 # --------------------------------------------------------------------------- loss
 @pytest.mark.gpu
-@pytest.mark.parametrize("grid", GRIDS, ids=["36x18", "18x9"])
+@pytest.mark.parametrize("grid", KERNEL_GRIDS, ids=KERNEL_GRID_IDS)
 def test_loss_at_size(dev, grid):
   """CE over [12, 128, V] logits and Huber over [12, 128, HW, 2] offsets (about 4 grid-stride passes of the Huber
   kernel at 36x18), errors on both sides of |e| = 1; then the mixed-label path as TrainEngine._backward_scale chains
@@ -299,7 +305,7 @@ def head_inputs(dev, h, w, seed, steps=1):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("grid", GRIDS, ids=["36x18", "18x9"])
+@pytest.mark.parametrize("grid", KERNEL_GRIDS, ids=KERNEL_GRID_IDS)
 def test_heads_forward_at_size(dev, grid):
   """head_class_fwd (logits, arg-max ids, the embedded one-hot of the ids as the next step's x planes) and
   head_reg_fwd (offsets, their dense embedding as x planes), planes = 2, 128 samples."""
@@ -341,7 +347,7 @@ def test_heads_forward_at_size(dev, grid):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("pout", [1, 2])
-@pytest.mark.parametrize("grid", GRIDS, ids=["36x18", "18x9"])
+@pytest.mark.parametrize("grid", KERNEL_GRIDS, ids=KERNEL_GRID_IDS)
 def test_head_backward_chained_at_size(dev, grid, pout):
   """head_bwd over the 12 decoder steps into one dWo (128 blocks x 12 launches of atomics), dh as the engine passes
   it: overwritten at the last step, added to what the graph attention left there at the others.  The halo rows of
@@ -374,7 +380,7 @@ def test_head_backward_chained_at_size(dev, grid, pout):
 # --------------------------------------------------------------------------- embeddings
 @pytest.mark.gpu
 @pytest.mark.parametrize("mode", ["onehot", "dense", "mixup_pad"])
-@pytest.mark.parametrize("grid", GRIDS, ids=["36x18", "18x9"])
+@pytest.mark.parametrize("grid", KERNEL_GRIDS, ids=KERNEL_GRID_IDS)
 def test_emb_backward_at_size(dev, grid, mode):
   """emb_bwd, 12 launches accumulating into dWe / dbe.  onehot: P_out = 1, ids in the corners and on the edges
   (taps cut off by the border);  dense: P_out = 2 on an offset map, d_in accumulating;  mixup_pad: the mixed
@@ -457,7 +463,7 @@ def gnn_inputs(dev, h, w, seed, with_scene):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("with_scene", [True, False], ids=["scene", "h_only"])
-@pytest.mark.parametrize("grid", GRIDS, ids=["36x18", "18x9"])
+@pytest.mark.parametrize("grid", KERNEL_GRIDS, ids=KERNEL_GRID_IDS)
 def test_gnn_forward_at_size(dev, grid, with_scene):
   """gnn_attend_fwd into the h block of the class decoder's operand planes (planes = 2)."""
   from multiverse_b200 import ops
@@ -475,7 +481,7 @@ def test_gnn_forward_at_size(dev, grid, with_scene):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("with_scene", [True, False], ids=["scene", "h_only"])
-@pytest.mark.parametrize("grid", GRIDS, ids=["36x18", "18x9"])
+@pytest.mark.parametrize("grid", KERNEL_GRIDS, ids=KERNEL_GRID_IDS)
 def test_gnn_backward_at_size(dev, grid, with_scene):
   """gnn_bwd over the 12 decoder steps: dh of every step, d(scene mean) accumulated over the 12 launches; the halo
   rows of dh hold a sentinel that must survive.  The gradient at a clamped cell is about 1e6 x larger than
@@ -514,12 +520,11 @@ def test_gnn_backward_at_size(dev, grid, with_scene):
 FRAMES = 48
 
 
-@pytest.fixture(scope="module")
-def scene(dev):
-  """The shared-frame feeds of 128 trajectories over 48 frames, the scene CNN weights (synthetic.make_weights) and
-  the kernels' forward outputs."""
+def make_scene(dev, name):
+  """The shared-frame feeds of 128 trajectories over 48 frames of the scene SCENES[name], the scene CNN weights
+  (synthetic.make_weights) and the kernels' forward outputs."""
   from multiverse_b200 import ops, synthetic
-  cfg = synthetic.make_config()
+  cfg = synthetic.make_config(**SCENES[name])
   f = shared_frame_feeds(cfg, NS, FRAMES, 300)
   wts = synthetic.make_weights(cfg, 300)
   W = [on(dev, wts["person_pred/scene_conv%d/W" % k]) for k in (1, 2)]
@@ -527,29 +532,54 @@ def scene(dev):
   x = on(dev, f["scene_feat"])
   conv1 = ops.scene_conv_fwd(x, W[0], b[0])
   conv2 = ops.scene_conv_fwd(conv1, W[1], b[1])
-  return dict(f=f, x=x, W=W, b=b, convs=[conv1, conv2], obs=on(dev, f["obs_scene"]),
+  return dict(cfg=cfg, f=f, x=x, W=W, b=b, convs=[conv1, conv2], obs=on(dev, f["obs_scene"]),
               labels=[on(dev, a, torch.int32) for a in f["grid_obs_labels"]])
 
 
+@pytest.fixture(scope="module")
+def scene(dev):
+  """The benchmark's 72x36 scene: grids 36x18 and 18x9."""
+  return make_scene(dev, "72x36")
+
+
+@pytest.fixture(scope="module")
+def scene_native(dev):
+  """The published 36x64 scene (TRAINING.md): grids 18x32 and 9x16."""
+  return make_scene(dev, "36x64")
+
+
 def test_shared_frame_feeds_share_frames_and_cells():
-  """The feeds the scene tests run on do share what they claim to (CPU)."""
+  """The feeds the scene tests run on do share what they claim to (CPU), on both scenes."""
   from multiverse_b200 import synthetic
-  cfg = synthetic.make_config()
-  f = shared_frame_feeds(cfg, NS, FRAMES, 300)
-  obs = f["obs_scene"]
-  assert obs.min() >= 0 and obs.max() < FRAMES and np.all(np.diff(obs, axis=1) == 1)
-  uses = np.bincount(obs.reshape(-1), minlength=FRAMES)
-  assert uses.max() >= 20 and (uses > 0).sum() == FRAMES          # every frame is used, some by many trajectories
-  for lab in f["grid_obs_labels"]:
-    key = obs * 10000 + lab                                      # (frame, cell) of every observed step
-    same = [len(set(key[:, t])) < NS for t in range(cfg.obs_len)]
-    assert all(same[:4])
+  for over in SCENES.values():
+    cfg = synthetic.make_config(**over)
+    f = shared_frame_feeds(cfg, NS, FRAMES, 300)
+    assert f["scene_feat"].shape[1:3] == (cfg.scene_h, cfg.scene_w)
+    obs = f["obs_scene"]
+    assert obs.min() >= 0 and obs.max() < FRAMES and np.all(np.diff(obs, axis=1) == 1)
+    uses = np.bincount(obs.reshape(-1), minlength=FRAMES)
+    assert uses.max() >= 20 and (uses > 0).sum() == FRAMES          # every frame is used, some by many trajectories
+    for lab, (h, w) in zip(f["grid_obs_labels"], cfg.scene_grids):
+      assert lab.max() < h * w
+      key = obs * 10000 + lab                                      # (frame, cell) of every observed step
+      same = [len(set(key[:, t])) < NS for t in range(cfg.obs_len)]
+      assert all(same[:4])
 
 
 @pytest.mark.gpu
 def test_scene_forward_on_shared_frames(dev, scene):
-  """scene_conv_fwd (both layers), scene_time_mean over overlapping windows (about 10 grid-stride passes at 36x18),
-  enc_class_input and enc_class_input_mix into the class encoder's x planes, on both grids."""
+  check_scene_forward(dev, scene)
+
+
+@pytest.mark.gpu
+def test_scene_forward_on_shared_frames_36x64(dev, scene_native):
+  check_scene_forward(dev, scene_native)
+
+
+def check_scene_forward(dev, scene):
+  """scene_conv_fwd (both layers: 72x36 -> 36x18 -> 18x9, or 36x64 -> 18x32 -> 9x16), scene_time_mean over
+  overlapping windows (about 10 grid-stride passes at 36x18), enc_class_input and enc_class_input_mix into the class
+  encoder's x planes, on both grids."""
   from multiverse_b200 import ops
   x64 = scene["x"].double()
   c1 = ref_scene_conv(x64, scene["W"][0].double(), scene["b"][0].double())
@@ -558,7 +588,8 @@ def test_scene_forward_on_shared_frames(dev, scene):
   obs = scene["obs"]
   cpad = ops.cell_cpad(64)
   worst = {"mean": 0.0, "input planes": 0.0, "mix planes": 0.0}
-  for i, (h, w) in enumerate(GRIDS):
+  for i, (h, w) in enumerate(scene["cfg"].scene_grids):
+    assert tuple(scene["convs"][i].shape[1:3]) == (h, w)
     conv = scene["convs"][i]
     mean = ops.scene_time_mean(conv, obs)
     worst["mean"] = max(worst["mean"], rel(mean, conv.double()[obs.long()].mean(1)))
@@ -586,7 +617,8 @@ def test_scene_forward_on_shared_frames(dev, scene):
       want = conv.double()[fr.long()].view(NS, h * w, 64) * mix[..., None]
       worst["mix planes"] = max(worst["mix planes"], rel(inner(vals, NS, h, w)[..., :64], want.view(NS, h, w, 64)))
   errs.update(worst)
-  report("scene fwd, %d trajectories over %d frames" % (NS, FRAMES), errs)
+  report("scene fwd %dx%d, %d trajectories over %d frames" % (scene["cfg"].scene_h, scene["cfg"].scene_w, NS, FRAMES),
+         errs)
   for k in ("conv1", "conv2", "mean"):
     assert errs[k] < ATOL, (k, errs[k])
   for k in ("input planes", "mix planes"):
@@ -595,6 +627,15 @@ def test_scene_forward_on_shared_frames(dev, scene):
 
 @pytest.mark.gpu
 def test_scene_backward_on_shared_frames(dev, scene):
+  check_scene_backward(dev, scene)
+
+
+@pytest.mark.gpu
+def test_scene_backward_on_shared_frames_36x64(dev, scene_native):
+  check_scene_backward(dev, scene_native)
+
+
+def check_scene_backward(dev, scene):
   """The scene-feature gradient as the training step assembles it, on shared frames: enc_class_input_bwd over the 8
   observed steps and scene_time_mean_bwd scatter into d(conv) of each scale (enc_class_input_mix_bwd alongside);
   then scene_conv_bwd of layer 2 (the KPG 144 instantiation, din added into d(conv1)) and of layer 1 (KPG 25, din
@@ -605,7 +646,7 @@ def test_scene_backward_on_shared_frames(dev, scene):
   cpad = ops.cell_cpad(64)
   errs = {}
   dconv = []
-  for i, (h, w) in enumerate(GRIDS):
+  for i, (h, w) in enumerate(scene["cfg"].scene_grids):
     conv = scene["convs"][i]
     lab = scene["labels"][i]
     lab2 = lab.flip(0).contiguous()
@@ -644,7 +685,8 @@ def test_scene_backward_on_shared_frames(dev, scene):
   ops.scene_conv_bwd(scene["x"], scene["W"][0], conv1, dconv[0], dW1, db1, dx)
   _, (gx, gW, gb) = vjp(ref_scene_conv, [scene["x"], scene["W"][0], scene["b"][0]], dconv[0])
   errs.update({"dW1": rel(dW1, gW), "db1": rel(db1, gb), "din1": rel(dx, gx)})
-  report("scene bwd, %d trajectories over %d frames" % (NS, FRAMES), errs)
+  report("scene bwd %dx%d, %d trajectories over %d frames" % (scene["cfg"].scene_h, scene["cfg"].scene_w, NS, FRAMES),
+         errs)
   for k, err in errs.items():
     assert err < ATOL, (k, err)
 
@@ -733,14 +775,24 @@ def test_optimizer_on_every_variable(dev, name):
 
 # --------------------------------------------------------------------------- whole model at the micro-batch
 WM_SEED = 337       # seeds 330-336 put some decoded arg-max of the fp64 reference within 1e-4 x max|logit| of a tie
+WM_SEED_NATIVE = 403  # seeds 400-402 put some decoded arg-max of the fp64 reference within 1e-4 x max|logit| of a tie
 MARGIN = 1e-4        # smallest top-2 logit gap the class decoder's arg-max may have, relative to max|logit| (the
-                     # engine's logit error at this size measures 1.3e-5 at 36x18, 2.1e-5 at 18x9)
+                     # engine's logit error at this size measures 1.3e-5 at 36x18, 2.1e-5 at 18x9, 9.4e-6 at 18x32,
+                     # 1.9e-5 at 9x16)
+WM_CASES = {
+    # name: (config overrides, seed)
+    "bench_72x36": (dict(), WM_SEED),
+    # the published training command (TRAINING.md): scene 36x64, both scales, --grid_reg_loss_weight 0.2
+    "native_36x64": (dict(scene_h=36, scene_w=64, grid_reg_loss_weight=0.2), WM_SEED_NATIVE),
+}
 
 
-def wm_configs(n, chunk):
+def wm_configs(n, chunk, **over):
+  """(synthetic config of n trajectories, oracle config of chunk trajectories): loss weights 1.0 / 0.1 and weight
+  decay 0.001 unless `over` says otherwise."""
   from multiverse_b200 import synthetic
-  loss = dict(grid_loss_weight=1.0, grid_reg_loss_weight=0.1, wd=0.001)
-  return synthetic.make_config(batch_size=n, clip_gradient_norm=10.0, **loss), R.default_config(batch_size=chunk, **loss)
+  over = dict(dict(grid_loss_weight=1.0, grid_reg_loss_weight=0.1, wd=0.001), **over)
+  return synthetic.make_config(batch_size=n, clip_gradient_norm=10.0, **over), R.default_config(batch_size=chunk, **over)
 
 
 def chunk_feeds(f, sl):
@@ -771,8 +823,19 @@ def test_reference_on_cuda_equals_reference_on_cpu(dev):
 
 @pytest.mark.gpu
 def test_whole_model_gradient_at_micro_batch(dev):
+  check_whole_model_gradient(dev, "bench_72x36")
+
+
+@pytest.mark.gpu
+def test_whole_model_gradient_on_the_published_config(dev):
+  check_whole_model_gradient(dev, "native_36x64")
+
+
+def check_whole_model_gradient(dev, case):
   """TrainEngine.loss_and_grads_chunked on 256 trajectories of shared frames (frames shared across the micro-batch
-  boundary) with micro_batch = 128 - the pair cell kernel runs - against RT.loss_and_grads on the GPU over chunks of
+  boundary) with micro_batch = 128, on the benchmark's config and on the published one (scene 36x64: grids 18x32,
+  whose micro-batch runs the pair cell kernel, and 9x16, which runs the single-CTA one; regression loss weight 0.2),
+  against RT.loss_and_grads on the GPU over chunks of
   16 trajectories, gradients summed with weight 16/256 (every loss is a batch mean) minus the weight-decay term the
   engine leaves to the optimizer.  The class decoder feeds one_hot(arg-max) forward, so the comparison is
   well-posed only if no arg-max of the reference lies within the engine's logit error of a tie: asserted as a
@@ -782,10 +845,12 @@ def test_whole_model_gradient_at_micro_batch(dev):
   from multiverse_b200 import ops
   from multiverse_b200.train_engine import TrainEngine
   from multiverse_b200 import synthetic
+  from test_kernels_atsize_gpu import m_tiles, num_sms, variant_name
   n, mb, chunk = 256, NS, 16
-  cfg, rcfg = wm_configs(n, chunk)
-  w = synthetic.make_weights(cfg, WM_SEED)
-  f = shared_frame_feeds(cfg, n, FRAMES, WM_SEED)
+  over, seed = WM_CASES[case]
+  cfg, rcfg = wm_configs(n, chunk, **over)
+  w = synthetic.make_weights(cfg, seed)
+  f = shared_frame_feeds(cfg, n, FRAMES, seed)
   last = f["obs_scene"][n - mb:]
   assert np.intersect1d(f["obs_scene"][:n - mb], last).size > 0, "no frame shared across the micro-batch boundary"
   # ---- reference
@@ -810,7 +875,12 @@ def test_whole_model_gradient_at_micro_batch(dev):
   ops.cell_variants_seen(reset=True)
   got, _ = eng.loss_and_grads_chunked(feeds, mb)
   torch.cuda.synchronize()
-  assert (2, True) in ops.cell_variants_seen(), "the P=2 pair cell kernel did not run: %s" % sorted(ops.cell_variants_seen())
+  # every grid's cells run in P = 2, as the CTA-pair kernel from 2 x SMs M tiles of the micro-batch up
+  want = {(ops.PLANES_BF16X2, m_tiles(mb, h, ww) >= 2 * num_sms()) for h, ww in cfg.scene_grids}
+  seen = ops.cell_variants_seen()
+  assert want <= seen, "cell variants %s ran, expected %s" % (sorted(seen), sorted(want))
+  print("%s: %s" % (case, ", ".join("%dx%d %s (%d M tiles)" % (h, ww, variant_name(
+      2 * ops.PLANES_BF16X2 + int(m_tiles(mb, h, ww) >= 2 * num_sms())), m_tiles(mb, h, ww)) for h, ww in cfg.scene_grids)))
   # ---- well-posedness of the arg-max feedback, and the ids / logits of the last micro-batch
   fwd_err = {}
   for i, (h, ww) in enumerate(cfg.scene_grids):
@@ -828,7 +898,7 @@ def test_whole_model_gradient_at_micro_batch(dev):
   got = got.cpu().numpy()
   assert np.abs(got - losses).max() < LTOL * np.abs(losses).max(), (got, losses)
   worst = {k: rel(eng.grads[k], grads[k]) for k in sorted(grads)}
-  print("whole model, 256 trajectories in micro-batches of 128: losses %s, worst gradient errors %s"
-        % (np.abs(got - losses).max() / np.abs(losses).max(), sorted(worst.items(), key=lambda kv: -kv[1])[:4]))
+  print("whole model %s, 256 trajectories in micro-batches of 128: losses %s, worst gradient errors %s"
+        % (case, np.abs(got - losses).max() / np.abs(losses).max(), sorted(worst.items(), key=lambda kv: -kv[1])[:4]))
   bad = {k: v for k, v in worst.items() if v > GTOL}
   assert not bad, bad

@@ -14,7 +14,8 @@ torch on the device (the reference functions of test_train_atsize_gpu.py):
 The whole model: TrainEngine.loss_and_grads_chunked on 256 trajectories in micro-batches of 128 against the fp64
 truth of tests/train_options_ref.py for every option, at the bars of test_train_atsize_gpu.py; chunked equals
 unchunked for soft labels + mask (128 trajectories in micro-batches of 64).  The drop-in: train.py-shaped arguments
-with each flag run Trainer.step; on the inputs of every reference-execution golden (tests/golden/refexec_train_*.npz)
+with each flag run Trainer.step; on the inputs of every reference-execution golden (tests/golden/refexec_train_*.npz,
+and refexec_native.npz with TRAINING.md's arguments: scene 36x64, both scales, loss weights 1.0 / 0.2, init_lr 0.3)
 one Trainer.step equals the unmodified reference Model + Trainer in losses, clipped gradients and updated variables;
 the combinations that stay unimplemented raise."""
 import os
@@ -25,6 +26,7 @@ import numpy as np
 import pytest
 import torch
 
+import cases
 import train_options_ref as TO
 from test_kernels_atsize_gpu import halo_rows, inner, rel, to_halo
 from test_train_atsize_gpu import (E, FRAMES, FTOL, GRIDS, GTOL, LTOL, MARGIN, NS, PTOL, SENTINEL, T_PRED, WM_SEED,
@@ -331,9 +333,10 @@ def test_chunked_equals_unchunked_soft_mask(dev):
 
 
 # --------------------------------------------------------------------------- drop-in
-def _dropin_model(monkeypatch, w=None, f=None, n=4, **flags):
-  """The drop-in Model of code/train.py's arguments (+ flags) on weights w and feeds f (synthetic ones by default),
-  and a batch of f as the reference's pred_utils hands it to Trainer.step."""
+def _dropin_model(monkeypatch, w=None, f=None, n=4, over=None, **flags):
+  """The drop-in Model of code/train.py's arguments (+ flags; `over`: model-shape and loss-weight arguments) on
+  weights w and feeds f (synthetic ones by default), and a batch of f as the reference's pred_utils hands it to
+  Trainer.step."""
   from multiverse_b200 import synthetic
   monkeypatch.syspath_prepend(os.path.join(ROOT, "multiverse_b200", "dropin"))
   for m in ("tensorflow", "pred_models", "multiverse_b200.pred_models"):
@@ -341,9 +344,9 @@ def _dropin_model(monkeypatch, w=None, f=None, n=4, **flags):
   import tensorflow as tf
   import pred_models
   tf.reset_default_graph()
-  over = dict(batch_size=n, use_grids=[False, True])
-  cfg = synthetic.make_config(is_train=True, grid_loss_weight=1.0, grid_reg_loss_weight=0.1, wd=0.001,
-                              clip_gradient_norm=10.0, **over)
+  conf = dict(batch_size=n, use_grids=[False, True], grid_loss_weight=1.0, grid_reg_loss_weight=0.1, wd=0.001)
+  conf.update(over or {})
+  cfg = synthetic.make_config(is_train=True, clip_gradient_norm=10.0, **conf)
   args = types.SimpleNamespace(**vars(cfg))            # code/train.py's defaults for the multi-future flags
   args.modelname = "m"; args.use_gt_grid = False; args.use_teacher_forcing = False; args.train_w_onehot = False
   args.use_soft_grid_class = False; args.soft_grid = 1; args.mask_grid_regression = False
@@ -426,16 +429,24 @@ def test_dropin_trainer_step_equals_reference_execution(dev, monkeypatch, case):
   tf, pred_models, model, args, _, _, _, batch = _dropin_model(
       monkeypatch, w=w, f=f, n=cfg.batch_size, use_soft_grid_class=bool(mode), soft_grid=mode or 1,
       mask_grid_regression=mask, train_w_onehot=onehot)
+  check_step_against_reference_execution(case, tf, pred_models, model, args, batch, w, got, "")
+
+
+def check_step_against_reference_execution(tag, tf, pred_models, model, args, batch, w, got, prefix):
+  """One Trainer.step of the drop-in model against a reference-execution golden (keys under `prefix`): the losses,
+  the clipped gradients and the variables after the Adadelta step, at the learning rate of the arguments."""
   with tf.Session() as sess:
     loss, _, wd_loss, pgl = pred_models.Trainer(model, args).step(sess, batch)
     assert int(sess.run(model.global_step)) == 1
+  got = {k[len(prefix):]: got[k] for k in got.files if k.startswith(prefix)}
   assert abs(loss - float(got["loss"])) <= LTOL * abs(float(got["loss"]))
   assert abs(wd_loss - float(got["wd_loss"])) <= 1e-5 * float(got["wd_loss"])
+  assert len(pgl) == len(got["pred_grid_loss"])
   assert np.abs(np.array(pgl) - got["pred_grid_loss"]).max() <= LTOL * got["pred_grid_loss"].max()
   eng = model._engine
-  lr, worst = 0.2, {}
+  lr, worst = args.init_lr * args.emb_lr, {}        # the Adadelta rate at step 0
   for k in got["variables"]:
-    g = eng.grads[k].double().cpu().numpy() + (0.001 * w[k] if k.endswith("/W") else 0.0)   # + weight decay
+    g = eng.grads[k].double().cpu().numpy() + (args.wd * w[k] if k.endswith("/W") else 0.0)   # + weight decay
     gc = np.clip(g, -10.0, 10.0)
     bar_g = GTOL * float(got["grad_absmax/" + k])
     err_g = np.abs(G.sample(gc) - got["grad/" + k]).max()
@@ -444,5 +455,27 @@ def test_dropin_trainer_step_equals_reference_execution(dev, monkeypatch, case):
     worst[k] = (err_g / float(got["grad_absmax/" + k]), err_w)
     assert err_g <= bar_g, (k, err_g, bar_g)
     assert err_w <= bar_w, (k, err_w, bar_w)
-  print("%s: loss %.6g vs %.6g, worst gradient errors %s" % (case, loss, float(got["loss"]),
-                                                             sorted(worst.items(), key=lambda kv: -kv[1][0])[:3]))
+  print("%s: loss %.6g vs %.6g (rel %.2e), worst gradient errors %s" % (
+      tag, loss, float(got["loss"]), abs(loss - float(got["loss"])) / abs(float(got["loss"])),
+      sorted(worst.items(), key=lambda kv: -kv[1][0])[:3]))
+
+
+@pytest.mark.gpu
+def test_dropin_trainer_step_on_the_published_command_equals_reference_execution(dev, monkeypatch):
+  """One Trainer.step with TRAINING.md's arguments - scene 36x64, strides 2,4 (grids 18x32 and 9x16), use_grids 1,1,
+  --train_w_onehot, loss weights 1.0 / 0.2, --init_lr 0.3 - on the inputs of tests/golden/refexec_native.npz,
+  against what the unmodified reference Model + Trainer computed on them, with the checks of
+  test_dropin_trainer_step_equals_reference_execution."""
+  cfg, w, f = cases.refexec_native_inputs()
+  opts = cases.REFEXEC_NATIVE[2]
+  assert G.SAMPLE == cases.NATIVE_TRAIN_SAMPLE
+  got = np.load(os.path.join(ROOT, "tests", "golden", "refexec_native.npz"))
+  over = dict(scene_h=cfg.scene_h, scene_w=cfg.scene_w, scene_grid_strides=[2, 4], use_grids=[True, True],
+              grid_loss_weight=opts["grid_loss_weight"], grid_reg_loss_weight=opts["grid_reg_loss_weight"],
+              wd=opts["wd"])
+  tf, pred_models, model, args, dcfg, _, _, batch = _dropin_model(
+      monkeypatch, w=w, f=f, n=cfg.batch_size, over=over, train_w_onehot=opts["train_w_onehot"],
+      init_lr=opts["init_lr"])
+  assert dcfg.scene_grids == [(18, 32), (9, 16)] and args.init_lr == 0.3 and args.grid_reg_loss_weight == 0.2
+  check_step_against_reference_execution("published command 36x64", tf, pred_models, model, args, batch, w, got,
+                                         "train/")
