@@ -78,9 +78,8 @@ int encode_tmap_3d_u8(CUtensorMap* out, const void* base, uint64_t d0, uint64_t 
                             b0, b1, b2, swizzle_bytes);
 }
 
-int encode_tmap_4d_bf16(CUtensorMap* out, const void* base, const uint64_t (&dims)[4],
-                        const uint64_t (&strides_bytes)[3], const uint32_t (&box)[4],
-                        int swizzle_bytes) {
+static int encode_tmap_4d_any(CUtensorMapDataType dt, CUtensorMap* out, const void* base, const uint64_t (&dims)[4],
+                              const uint64_t (&strides_bytes)[3], const uint32_t (&box)[4], int swizzle_bytes) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return MVB_ERR_DRIVER;
   cuuint64_t d[4] = {dims[0], dims[1], dims[2], dims[3]};
@@ -91,7 +90,7 @@ int encode_tmap_4d_bf16(CUtensorMap* out, const void* base, const uint64_t (&dim
                           : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
                           : swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
                                                 : CU_TENSOR_MAP_SWIZZLE_NONE;
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), d, st, bx, estr,
+  CUresult r = fn(out, dt, 4, const_cast<void*>(base), d, st, bx, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -101,6 +100,16 @@ int encode_tmap_4d_bf16(CUtensorMap* out, const void* base, const uint64_t (&dim
     return MVB_ERR_DRIVER;
   }
   return MVB_OK;
+}
+
+int encode_tmap_4d_bf16(CUtensorMap* out, const void* base, const uint64_t (&dims)[4],
+                        const uint64_t (&strides_bytes)[3], const uint32_t (&box)[4],
+                        int swizzle_bytes) {
+  return encode_tmap_4d_any(CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, out, base, dims, strides_bytes, box, swizzle_bytes);
+}
+int encode_tmap_4d_u8(CUtensorMap* out, const void* base, const uint64_t (&dims)[4],
+                      const uint64_t (&strides_bytes)[3], const uint32_t (&box)[4], int swizzle_bytes) {
+  return encode_tmap_4d_any(CU_TENSOR_MAP_DATA_TYPE_UINT8, out, base, dims, strides_bytes, box, swizzle_bytes);
 }
 
 }  // namespace mvb

@@ -21,6 +21,8 @@
 //   warpgroup 0      TMA producer (one thread), registers handed to the others (setmaxnreg)
 //   warpgroups 1, 2  MMA + epilogue: each owns 64 rows of the 128-row tile, all 256 columns (128 fp32
 //                    accumulators per thread)
+// f16f8 launches of many M tiles per SM run cell_fwd_epi_kernel instead: tiles of 128 x 128 (4 gates x 32
+// channels) and a fourth warpgroup that runs the epilogue of one tile from shared memory while the MMA warpgroups compute the next.
 #include "mvb_common.cuh"
 #include "mvb_kernels.h"
 #include <stdlib.h>
@@ -90,6 +92,9 @@ static_assert(CellCfg<0>::ring(168).b_slots == 4 && CellCfg<0>::ring(200).b_slot
 enum CellProbePhase {
   kProbeFullWait, kProbeAFullWait, kProbeMmaWait, kProbeEpilogue, kProbeConsumer,    // MMA warpgroups
   kProbeEmptyWait, kProbeAEmptyWait, kProbeProducer,                                 // TMA producer thread
+  // cell_fwd_epi_kernel: the MMA warpgroups' wait for a free staging buffer (their kProbeEpilogue is the staging
+  // write), the epilogue warpgroup's wait for a staged tile and the rest of its time
+  kProbeFreeWait, kProbeStagedWait, kProbeEpiBusy,
   kProbeTiles, kProbePhases
 };
 #ifdef MVB_CELL_PROBE
@@ -560,6 +565,333 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 }
 
 // ----------------------------------------------------------------------------------
+// f16f8 cell with an epilogue warpgroup (the f16f8 kernel of large launches, kEpiWgMinTilesPerSm; MVB_CELL_EPI_WG=0
+// runs cell_fwd_kernel instead, MVB_CELL_EPI_WG=1 this one at every size).
+// Tiles of 128 rows x 128 columns, 512 threads, 1 CTA/SM, persistent over tiles:
+//   warpgroup 0      TMA producer (one thread)
+//   warpgroups 1, 2  MMA only: each owns 64 rows of the tile (m64n128: 64 fp32 accumulators per thread).  When a
+//                    tile's MMAs have completed they copy the accumulators into a 64 KB fp32 staging buffer in shared
+//                    memory and start the next tile at once
+//   warpgroup 3      the epilogue of the staged tile (epi_row, epi_cprev, epi_inputs, epi_pair: the same functions of
+//                    the same accumulators as cell_fwd_kernel) while the MMA warpgroups run the next tile's mainloop
+// The mainloop is cell_fwd_kernel's f16f8 one (both passes, e4m3 first; halo'd A stages read by all nine taps; pair
+// multicast of the weight slots).  A weight slot still serves 128 rows, so the weight bytes per FLOP are unchanged;
+// an A stage now serves eight N tiles instead of four.
+// Columns: N tile nt of 128 holds all four gates of 32 channels: packed columns T * 256 + gate * 64 + 32 h + [0, 32)
+// with T = nt / 2, h = nt % 2.  Its weight rows are four 32-row groups of the packed weights, loaded as one 4-D TMA
+// box (rows = [32 rows][2 halves][16 (tile, gate)]), so the packed column order of the weights and of every table
+// is the one cell_fwd_kernel reads.
+// ----------------------------------------------------------------------------------
+constexpr int EW_BLOCK_N = 128;
+constexpr int EW_TILE_CH = EW_BLOCK_N / 4;                  // 32 channels per N tile
+constexpr int EW_N_TILES = kGates / EW_BLOCK_N;             // 8
+constexpr int EW_THREADS = 512;
+constexpr int EW_SLOT_BYTES = EW_BLOCK_N * ROW_BYTES;       // 16 KB: 128 weight rows x 128 B
+constexpr int EW_STAGING_BYTES = BLOCK_M * EW_BLOCK_N * 4;  // 64 KB: the fp32 accumulators of one tile
+// setmaxnreg budgets: producer, each MMA warpgroup, the epilogue warpgroup
+constexpr int kEwRegsProducer = 40, kEwRegsMma = 152, kEwRegsEpi = 168;
+static_assert(128 * (kEwRegsProducer + 2 * kEwRegsMma + kEwRegsEpi) <= 65536, "the four warpgroups fit the register file");
+
+// Layout: [staging][B slots][A stages][barriers: full, empty (kMaxBSlots each), afull, aempty (kMaxAStages each),
+// staged, staging free].  Three A stages where 6 weight slots of 16 KB still fit beside them and the staging buffer
+// (36x18, 18x9), else two stages and as many slots as fit (6 at 18x32 and 4x62): measured on the beam launch, the third
+// stage is worth a slot, a sixth slot is worth more than the third stage.
+struct CellEpiCfg {
+  static constexpr int slots(int a, int stages) {
+    const int b = (kSmemLimit - kSmemExtra - EW_STAGING_BYTES - stages * a) / EW_SLOT_BYTES;
+    return b > kMaxBSlots ? kMaxBSlots : b;
+  }
+  static constexpr CellRing ring(int ra8) {
+    const int a = ra8 * ROW_BYTES;
+    return slots(a, 3) >= 6 ? CellRing{slots(a, 3), 3, a} : CellRing{slots(a, 2), 2, a};
+  }
+  static constexpr int smem_bytes(const CellRing& r) {
+    return EW_STAGING_BYTES + r.b_slots * EW_SLOT_BYTES + r.a_stages * r.a_stage_bytes + kSmemExtra;
+  }
+};
+static_assert((2 * kMaxBSlots + 2 * kMaxAStages + 2) * 8 <= 512, "the barrier area holds the staging barriers too");
+static_assert(CellEpiCfg::ring(168).b_slots == 6 && CellEpiCfg::ring(168).a_stages == 3 &&
+              CellEpiCfg::smem_bytes(CellEpiCfg::ring(168)) <= kSmemLimit, "36x18: 6 slots, 3 stages");
+static_assert(CellEpiCfg::ring(152).b_slots == 6 && CellEpiCfg::ring(152).a_stages == 3 &&
+              CellEpiCfg::smem_bytes(CellEpiCfg::ring(152)) <= kSmemLimit, "18x9: 6 slots, 3 stages");
+static_assert(CellEpiCfg::ring(200).b_slots == 6 && CellEpiCfg::ring(200).a_stages == 2 && CellEpiCfg::smem_bytes(CellEpiCfg::ring(200)) <= kSmemLimit,
+              "18x32: 6 slots, 2 stages");
+static_assert(CellEpiCfg::ring(256).b_slots == 6 && CellEpiCfg::ring(256).a_stages == 2 && CellEpiCfg::smem_bytes(CellEpiCfg::ring(256)) <= kSmemLimit,
+              "4x62: 6 slots, 2 stages");
+
+// fp32 offset of (row r, column col) of the staging buffer: rows of 128 floats whose 16-byte chunks are XOR-swizzled
+// by the row, so that the float2 accesses of the accumulator fragment layout (8 rows x 4 threads per 8-column group)
+// - the MMA warpgroups' writes and the epilogue warpgroup's reads alike - touch 32 different banks per 16 threads.
+__device__ __forceinline__ int staging_off(int r, int col) {
+  return r * EW_BLOCK_N + ((((col >> 2) ^ ((r & 3) << 1))) << 2) + (col & 3);
+}
+
+template <bool MC>
+__global__ void __launch_bounds__(EW_THREADS, 1)
+cell_fwd_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    const __grid_constant__ CUtensorMap tmA8, const __grid_constant__ CUtensorMap tmB8,
+                    const CellParams prm) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
+  const int ra8 = (BLOCK_M + 2 * (prm.W + 2) + 7) & ~7;     // rows of an A stage
+  const int a_stage_bytes = prm.ring.a_stage_bytes;           // one plane: ra8 rows of 128 B
+  const int b_slots = prm.ring.b_slots, a_stages = prm.ring.a_stages;
+  float* staging = reinterpret_cast<float*>(smem);
+  uint8_t* smem_b = smem + EW_STAGING_BYTES;
+  uint8_t* smem_a = smem_b + b_slots * EW_SLOT_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_a + a_stages * a_stage_bytes);
+  uint64_t* empty_bar = full_bar + kMaxBSlots;
+  uint64_t* afull_bar = empty_bar + kMaxBSlots;
+  uint64_t* aempty_bar = afull_bar + kMaxAStages;
+  uint64_t* staged_bar = aempty_bar + kMaxAStages;   // every MMA thread has written its accumulators to the staging
+  uint64_t* free_bar = staged_bar + 1;               // every epilogue thread has read the staged tile
+  CELL_PROBE(long long probe[kProbePhases] = {};)
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;                    // 0: TMA producer; 1, 2: MMA of rows [64 (wg - 1), +64); 3: epilogue
+  const Grid g = make_grid(prm.H, prm.W);
+  const int cxp = prm.cpad - kHidden;
+  const int q_begin = prm.skip_x ? 1 : 0;
+  constexpr int NQ = 1 + kHidden / CHUNK;      // 5
+  const long long num_m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
+  const uint32_t rank = MC ? cluster_ctarank() : 0u;
+  const long long num_tiles = (MC ? (num_m_tiles + 1) / 2 : num_m_tiles) * EW_N_TILES;
+  const long long w_begin = MC ? (long long)(blockIdx.x >> 1) : (long long)blockIdx.x;
+  const long long w_step = MC ? (long long)(gridDim.x >> 1) : (long long)gridDim.x;
+  auto work_index = [&](long long it) -> long long {      // as in cell_fwd_kernel, with eight N tiles per M tile
+    return prm.order ? (w_begin + (it / EW_N_TILES) * w_step) * EW_N_TILES + it % EW_N_TILES : w_begin + it * w_step;
+  };
+  auto tile_m0 = [&](long long w) -> long long { return ((w / EW_N_TILES) * (MC ? 2 : 1) + rank) * BLOCK_M; };
+
+  if (warp == 0 && lane == 0) {
+    prefetch_tmap(&tmA); prefetch_tmap(&tmB); prefetch_tmap(&tmA8); prefetch_tmap(&tmB8);
+#pragma unroll 1
+    for (int s = 0; s < b_slots; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], MC ? 4 : 2); }
+#pragma unroll 1
+    for (int s = 0; s < a_stages; ++s) { mbar_init(&afull_bar[s], 1); mbar_init(&aempty_bar[s], 2); }
+    mbar_init(staged_bar, 256);
+    mbar_init(free_bar, 128);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (MC) cluster_sync_all();     // the peer's barriers exist before anything is sent to them
+
+  if (wg == 0) {
+    regs_dealloc<kEwRegsProducer>();
+    if (warp == 0 && lane == 0) {
+      // ===================== TMA producer =====================
+      int slot = 0, astage = 0; uint32_t phase = 0, aphase = 0;
+      CELL_PROBE(const long long probe_t0 = clock64();)
+      for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
+        const long long m0 = tile_m0(t);
+        const int nt = (int)(t % EW_N_TILES);
+        const int half = nt & 1, tg0 = (nt >> 1) * 4;      // 32-row half and (tile, gate) index of gate 0
+        for (int pass = 0; pass < 2; ++pass)
+        for (int q = q_begin; q < NQ; ++q) {
+          const int c16 = q == 0 ? 0 : cxp + (q - 1) * CHUNK;
+          const int c8 = q == 0 ? 0 : 2 * cxp + (q - 1) * 2 * CHUNK;
+          const bool f8 = pass == 0;
+          CELL_PROBED(kProbeAEmptyWait, mbar_wait(&aempty_bar[astage], aphase ^ 1));
+          uint8_t* sa = smem_a + astage * a_stage_bytes;
+          mbar_expect_tx(&afull_bar[astage], a_stage_bytes);
+          if (f8) tma_load_3d(sa, &tmA8, &afull_bar[astage], c8, (int)(m0 - g.Wp - 1), 0);
+          else tma_load_3d(sa, &tmA, &afull_bar[astage], c16, (int)(m0 - g.Wp - 1), 0);
+          if (++astage == a_stages) { astage = 0; aphase ^= 1; }
+          for (int tap = 0; tap < 9; ++tap) {
+            CELL_PROBED(kProbeEmptyWait, mbar_wait(&empty_bar[slot], phase ^ 1));
+            uint8_t* sb = smem_b + slot * EW_SLOT_BYTES;
+            mbar_expect_tx(&full_bar[slot], EW_SLOT_BYTES);
+            const CUtensorMap* tm = f8 ? &tmB8 : &tmB;
+            const int kcol = f8 ? tap * 2 * prm.cpad + c8 : tap * prm.cpad + c16;
+            // MC: this CTA's two gates (64 rows) of the slot, delivered to both CTAs of the pair
+            if (MC) tma_load_4d_mc(sb + rank * (EW_SLOT_BYTES / 2), tm, &full_bar[slot], kcol, 0, half,
+                                   tg0 + 2 * (int)rank, (uint16_t)3);
+            else tma_load_4d(sb, tm, &full_bar[slot], kcol, 0, half, tg0);
+            if (++slot == b_slots) { slot = 0; phase ^= 1; }
+          }
+        }
+      }
+#ifdef MVB_CELL_PROBE
+      atomicAdd(&g_cell_probe[kProbeEmptyWait], (unsigned long long)probe[kProbeEmptyWait]);
+      atomicAdd(&g_cell_probe[kProbeAEmptyWait], (unsigned long long)probe[kProbeAEmptyWait]);
+      atomicAdd(&g_cell_probe[kProbeProducer], (unsigned long long)(clock64() - probe_t0));
+#endif
+    }
+  } else if (wg < 3) {
+    regs_alloc<kEwRegsMma>();
+    // ===================== MMA (one warpgroup per 64 rows of the tile) =====================
+    const int c = wg - 1;
+    const bool leader = (threadIdx.x & 127) == 0;          // arrives on the ring barriers for the warpgroup
+    constexpr uint32_t kHi = smem_desc_hi(SW128_SBO, SW128_LAYOUT);
+    const uint32_t a_wg_lo = (uint32_t)(64 * c) * (ROW_BYTES >> 4);      // this warpgroup's 64 rows of the A tile
+    int slot = 0, astage = 0; uint32_t phase = 0, aphase = 0, free_phase = 0;
+    float acc[64];
+    // Two MMA batches (weight slots) in flight per warpgroup: a slot of 128 columns is 512 tensor clocks, half of
+    // cell_fwd_kernel's, and with one batch in flight the barrier / fence / wait of every slot left the tensor pipe
+    // idle.  A batch's slot (and, after its ninth tap, A stage) is released once the batch after next is issued and
+    // wgmma.wait_group 2 has returned.
+    constexpr int D = 2;
+    int rq_slot[D], rq_astage[D];
+#pragma unroll
+    for (int i = 0; i < D; ++i) { rq_slot[i] = -1; rq_astage[i] = -1; }
+    auto release_one = [&](int rs, int ra) {
+      if (leader && rs >= 0) {
+        if (MC) { mbar_arrive_remote(&empty_bar[rs], 0); mbar_arrive_remote(&empty_bar[rs], 1); }
+        else mbar_arrive(&empty_bar[rs]);
+        if (ra >= 0) mbar_arrive(&aempty_bar[ra]);
+      }
+    };
+    CELL_PROBE(const long long probe_t0 = clock64();)
+    for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
+      CELL_PROBE(++probe[kProbeTiles];)
+      uint32_t fresh = 1;                      // the tile's first MMA overwrites the accumulator
+      for (int pass = 0; pass < 2; ++pass)
+      for (int q = q_begin; q < NQ; ++q) {
+        const bool f8 = pass == 0;
+        CELL_PROBED(kProbeAFullWait, mbar_wait(&afull_bar[astage], aphase));
+        const uint32_t sa_lo = (smem_u32(smem_a + astage * a_stage_bytes) >> 4) + a_wg_lo;
+        for (int tap = 0; tap < 9; ++tap) {
+          const uint32_t a_lo = sa_lo + (uint32_t)((tap / 3) * g.Wp + (tap % 3)) * (ROW_BYTES >> 4);
+          CELL_PROBED(kProbeFullWait, mbar_wait(&full_bar[slot], phase));
+          const uint32_t b_lo = smem_u32(smem_b + slot * EW_SLOT_BYTES) >> 4;
+          wgmma_fence_regs(acc);
+          wgmma_fence();
+          if (q > 0) {
+            if (f8) {
+              for (int k = 0; k < 4; ++k) {           // [e0 (64 B) | e1 (64 B)]
+                wgmma_e4m3_n128(acc, desc_of(a_lo + 2 * k, kHi), desc_of(b_lo + 2 * k, kHi), fresh ^ 1u);
+                fresh = 0;
+              }
+            } else {
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                wgmma_f16<128, 0, 0>(acc, desc_of(a_lo + 2 * k, kHi), desc_of(b_lo + 2 * k, kHi), fresh ^ 1u);
+                fresh = 0;
+              }
+            }
+          } else {
+            // ---- x chunk (only cells whose input is not folded): cxp = 32 or 64 channels ----
+            const int ks16 = cxp / MMA_K, ks8 = cxp / 32;
+            const uint32_t poff = (uint32_t)cxp >> 4;              // e1 sits cxp bytes after e0 in an fp8 row
+            if (f8) {
+              for (int pk = 0; pk < 2 * ks8; ++pk) {
+                const uint32_t o = (pk / ks8) * poff + (pk % ks8) * 2;
+                wgmma_e4m3_n128(acc, desc_of(a_lo + o, kHi), desc_of(b_lo + o, kHi), fresh ^ 1u);
+                fresh = 0;
+              }
+            } else {
+              for (int k = 0; k < ks16; ++k) {
+                wgmma_f16<128, 0, 0>(acc, desc_of(a_lo + 2 * k, kHi), desc_of(b_lo + 2 * k, kHi), fresh ^ 1u);
+                fresh = 0;
+              }
+            }
+          }
+          wgmma_commit();
+          wgmma_fence_regs(acc);
+          CELL_PROBED(kProbeMmaWait, wgmma_wait<D>());
+          release_one(rq_slot[0], rq_astage[0]);
+#pragma unroll
+          for (int i = 0; i + 1 < D; ++i) { rq_slot[i] = rq_slot[i + 1]; rq_astage[i] = rq_astage[i + 1]; }
+          rq_slot[D - 1] = slot;
+          rq_astage[D - 1] = tap == 8 ? astage : -1;
+          if (++slot == b_slots) { slot = 0; phase ^= 1; }
+        }
+        if (++astage == a_stages) { astage = 0; aphase ^= 1; }
+      }
+      CELL_PROBED(kProbeMmaWait, wgmma_wait<0>());
+      wgmma_fence_regs(acc);
+#pragma unroll
+      for (int i = 0; i < D; ++i) { release_one(rq_slot[i], rq_astage[i]); rq_slot[i] = -1; rq_astage[i] = -1; }
+      // ===================== accumulators -> staging =====================
+      // thread (warp w, lane l) holds rows 16 w + l / 4 (+ 8) and columns 8 i + 2 (l % 4) (+ 1) of its 64 rows
+      CELL_PROBED(kProbeFreeWait, mbar_wait(free_bar, free_phase ^ 1));
+      free_phase ^= 1;
+      CELL_PROBE(const long long probe_e0 = clock64();)
+      const int r0 = 64 * c + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+      for (int i = 0; i < EW_BLOCK_N / 8; ++i)
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr)
+          *reinterpret_cast<float2*>(staging + staging_off(r0 + 8 * hr, 8 * i + 2 * (lane & 3))) =
+              make_float2(acc[4 * i + 2 * hr], acc[4 * i + 2 * hr + 1]);
+      mbar_arrive(staged_bar);
+      CELL_PROBE(probe[kProbeEpilogue] += clock64() - probe_e0;)
+    }
+#ifdef MVB_CELL_PROBE
+    if (leader) {
+      for (int p = kProbeFullWait; p <= kProbeEpilogue; ++p) atomicAdd(&g_cell_probe[p], (unsigned long long)probe[p]);
+      atomicAdd(&g_cell_probe[kProbeFreeWait], (unsigned long long)probe[kProbeFreeWait]);
+      atomicAdd(&g_cell_probe[kProbeConsumer], (unsigned long long)(clock64() - probe_t0));
+      atomicAdd(&g_cell_probe[kProbeTiles], (unsigned long long)probe[kProbeTiles]);
+    }
+#endif
+  } else {
+    regs_alloc<kEwRegsEpi>();
+    // ===================== epilogue of the staged tile =====================
+    // thread (warp w, lane l) takes rows 32 w + 8 k + l / 4 (k < 4) and channel pairs 8 ip + 2 (l % 4) (ip < 4) of the
+    // N tile's 32 channels: the accumulator fragment layout, so that its staging reads are free of bank conflicts.
+    // Two rows at a time (ptxas allocates every warpgroup's registers under the 128 of the launch bound): their
+    // context and c are loaded first - for the first two while the tile is still being computed.
+    const int ew = warp & 3, lc = 2 * (lane & 3);
+    uint32_t staged_phase = 0;
+    CELL_PROBE(const long long probe_t0 = clock64();)
+    for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
+      const long long m0 = tile_m0(t);
+      const int nt = (int)(t % EW_N_TILES);
+      const int tn = nt >> 1, jh = (nt & 1) * EW_TILE_CH;   // 256-column tile and this N tile's first channel in it
+      const int rb = 32 * ew + (lane >> 2);
+#pragma unroll 1
+      for (int k2 = 0; k2 < 4; k2 += 2) {
+        EpiRow rows[2];
+        float2 cprev[2][4];
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          rows[hr] = epi_row(prm, g, m0 + rb + 8 * (k2 + hr));
+#pragma unroll
+          for (int ip = 0; ip < 4; ++ip) cprev[hr][ip] = epi_cprev(prm, rows[hr], tn * TILE_CH + jh + 8 * ip + lc);
+        }
+        if (k2 == 0) {
+          CELL_PROBED(kProbeStagedWait, mbar_wait(staged_bar, staged_phase));
+          staged_phase ^= 1;
+        }
+#pragma unroll
+        for (int ip = 0; ip < 4; ++ip) {
+          const int j = jh + 8 * ip + lc;            // packed column of gate 0 in the 256-column tile tn
+          EpiIn in[2];
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) in[hr] = epi_inputs<1>(prm, g, rows[hr], tn, j);
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            if (!rows[hr].valid) continue;
+            float a[4][2];
+#pragma unroll
+            for (int gt = 0; gt < 4; ++gt) {
+              const float2 v = *reinterpret_cast<const float2*>(
+                  staging + staging_off(rb + 8 * (k2 + hr), gt * EW_TILE_CH + 8 * ip + lc));
+              a[gt][0] = v.x; a[gt][1] = v.y;
+            }
+            epi_pair<1>(prm, rows[hr], tn, j, a, cprev[hr][ip], in[hr]);
+          }
+        }
+      }
+      mbar_arrive(free_bar);
+    }
+#ifdef MVB_CELL_PROBE
+    if ((threadIdx.x & 127) == 0) {
+      atomicAdd(&g_cell_probe[kProbeStagedWait], (unsigned long long)probe[kProbeStagedWait]);
+      atomicAdd(&g_cell_probe[kProbeEpiBusy],
+                (unsigned long long)(clock64() - probe_t0 - probe[kProbeStagedWait]));
+    }
+#endif
+  }
+
+  __syncthreads();
+  if (MC) cluster_sync_all();     // the peer may still send into this CTA's smem / barriers
+}
+
+// ----------------------------------------------------------------------------------
 // Fan-out step of the beam decoder (the first K-row step: every child's parent is its sample's single t0 row, so the
 // K children share the graph-attended h, the GEMM and c, and differ only in the folded table rows of their selected
 // cell).  Stage 1 = the cell kernel with preact_out (one GEMM per PARENT row, raw accumulators to HBM: 4 KB per cell);
@@ -838,7 +1170,10 @@ extern "C" int mvb_cell_probe(unsigned long long* out, int reset) {
 }
 #endif
 
-struct CellMaps { CUtensorMap A, B, Bh, A8, B8, B8h; };
+// A, B, Bh: 16-bit (bf16x2 planes, or the fp16 region of f16f8) activation rows, weight tiles of 256 rows, halves of
+// them (CTA pairs); A8, B8, B8h: the same over the e4m3 region.  f16f8 only: Bq / B8q the four 32-row gate groups of
+// an N tile of cell_fwd_epi_kernel, Bqh / B8qh two of them (CTA pairs).
+struct CellMaps { CUtensorMap A, B, Bh, A8, B8, B8h, Bq, Bqh, B8q, B8qh; };
 
 // Work order of a launch (CellParams::order, work_index()).  1: the four N tiles of an M tile (pair) run back to back
 // on the same CTA (pair), so the tile's operand rows are re-read from L2 by the SM that fetched them.
@@ -846,19 +1181,67 @@ struct CellMaps { CUtensorMap A, B, Bh, A8, B8, B8h; };
 // shard: 32 trajectories of 36x18 = 176 M tiles on 132 CTAs) is bound by its longest CTA instead: back to back the
 // busiest CTA runs 2 x 4 items, strided ceil(704 / 132) = 6.  Strided whenever that makespan is shorter and the
 // launch is small enough for its operands to stay in L2.
-static int pick_order(int forced, long long units, long long ctas) {
+static int pick_order(int forced, long long units, long long ctas, int n_tiles) {
   if (forced == 0 || forced == 1) return forced;
-  const long long back_to_back = ((units + ctas - 1) / ctas) * N_TILES, strided = (units * N_TILES + ctas - 1) / ctas;
+  const long long back_to_back = ((units + ctas - 1) / ctas) * n_tiles, strided = (units * n_tiles + ctas - 1) / ctas;
   return (strided < back_to_back && units < 4 * ctas) ? 0 : 1;
 }
 
+// cell_fwd_epi_kernel (f16f8): the same choice of pair or single-CTA kernel and of work order as launch_cell
+static int launch_cell_epi(const CellMaps& tm, const CellParams& prm_in, int num_sms, bool multicast,
+                           cudaStream_t stream) {
+  CellParams prm = prm_in;
+  static SmemOptIn opt_plain, opt_mc;
+  const int ra8 = (BLOCK_M + 2 * (prm.W + 2) + 7) & ~7;
+  prm.ring = CellEpiCfg::ring(ra8);
+  const int smem_bytes = CellEpiCfg::smem_bytes(prm.ring);
+  MVB_REQUIRE(ra8 <= CellCfg<1>::MAX_RA8 && smem_bytes <= kSmemLimit && prm.ring.b_slots >= 2,
+              "cell_fwd: grid width W=%d too large (A stage of %d rows: %d weight slots, %d B shared memory)",
+              prm.W, ra8, prm.ring.b_slots, smem_bytes);
+  CELL_PROBE(g_probe_ring = prm.ring;)
+  MVB_CHECK_CUDA(smem_opt_in(opt_plain, cell_fwd_epi_kernel<false>, smem_bytes));
+  MVB_CHECK_CUDA(smem_opt_in(opt_mc, cell_fwd_epi_kernel<true>, smem_bytes));
+  const long long m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
+  if (multicast && m_tiles >= 2 * (long long)num_sms) {
+    prm.order = pick_order(prm_in.order, (m_tiles + 1) / 2, num_sms / 2, EW_N_TILES);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(num_sms / 2 * 2)); cfg.blockDim = dim3(EW_THREADS);
+    cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    MVB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, cell_fwd_epi_kernel<true>, tm.A, tm.Bqh, tm.A8, tm.B8qh, prm));
+    count_launch(1);
+    note_variant(1, 1);
+    return MVB_OK;
+  }
+  const long long num_tiles = m_tiles * EW_N_TILES;
+  const int grid = (int)(num_tiles < num_sms ? num_tiles : num_sms);
+  prm.order = pick_order(prm_in.order, m_tiles, grid, EW_N_TILES);
+  cell_fwd_epi_kernel<false><<<grid, EW_THREADS, smem_bytes, stream>>>(tm.A, tm.Bq, tm.A8, tm.B8q, prm);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  note_variant(1, 0);
+  return MVB_OK;
+}
+
+// cell_fwd_epi_kernel runs f16f8 launches of at least this many M tiles per SM (the K=20 beam steps: over 400).  On
+// the H100 it is 5 % faster there, but slower on launches of a few M tiles per SM (the greedy decoders of c3: 3 - 11),
+// where each CTA's first and last tiles - its pipeline fill and the epilogue of its last tile, which nothing hides -
+// weigh more.
+constexpr long long kEpiWgMinTilesPerSm = 64;
+
 template <int FMT>
-static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms, bool multicast, cudaStream_t stream) {
+static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms, bool multicast, int epi_wg,
+                       cudaStream_t stream) {
   CellParams prm = prm_in;
   static SmemOptIn opt_plain, opt_mc;
   // MVB_CELL_FORMAT_RINGS=0: f16f8 launches use the bf16x2 rings (two-plane A stages, 4 or 3 weight slots), the
   // layout before the rings were sized per format, for A/B runs; the results are bit-identical either way
   static const bool format_rings = [] { const char* e = getenv("MVB_CELL_FORMAT_RINGS"); return !(e && e[0] == '0'); }();
+  if (FMT == 1 && (epi_wg == 1 || (epi_wg == 2 && (prm.R + BLOCK_M - 1) / BLOCK_M >= kEpiWgMinTilesPerSm * num_sms)))
+    return launch_cell_epi(tm, prm, num_sms, multicast, stream);
   const int ra8 = (BLOCK_M + 2 * (prm.W + 2) + 7) & ~7;
   prm.ring = format_rings ? CellCfg<FMT>::ring(ra8) : CellCfg<0>::ring(ra8);
   const int smem_bytes = prm.ring.smem_bytes();
@@ -871,7 +1254,7 @@ static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms
   MVB_CHECK_CUDA(smem_opt_in(opt_mc, cell_fwd_kernel<true, FMT>, smem_bytes));
   const long long m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
   if (multicast && m_tiles >= 2 * (long long)num_sms) {
-    prm.order = pick_order(prm_in.order, (m_tiles + 1) / 2, num_sms / 2);
+    prm.order = pick_order(prm_in.order, (m_tiles + 1) / 2, num_sms / 2, N_TILES);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(num_sms / 2 * 2)); cfg.blockDim = dim3(NUM_THREADS);
     cfg.dynamicSmemBytes = smem_bytes; cfg.stream = stream;
@@ -886,7 +1269,7 @@ static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms
   }
   const long long num_tiles = m_tiles * N_TILES;
   const int grid = (int)(num_tiles < num_sms ? num_tiles : num_sms);
-  prm.order = pick_order(prm_in.order, m_tiles, grid);
+  prm.order = pick_order(prm_in.order, m_tiles, grid, N_TILES);
   cell_fwd_kernel<false, FMT><<<grid, NUM_THREADS, smem_bytes, stream>>>(tm.A, tm.B, tm.A8, tm.B8, prm);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
@@ -918,6 +1301,14 @@ int cell_fwd(const CellStep& s, cudaStream_t stream) {
 
   // weight-tile multicast across CTA pairs is on by default (MVB_CELL_MULTICAST=0 turns it off for A/B runs)
   static const bool multicast = [] { const char* e = getenv("MVB_CELL_MULTICAST"); return !(e && e[0] == '0'); }();
+  // Large f16f8 launches run cell_fwd_epi_kernel (an epilogue warpgroup, kEpiWgMinTilesPerSm).  For A/B runs,
+  // MVB_CELL_EPI_WG=1 runs it for every f16f8 launch, MVB_CELL_EPI_WG=0 (or MVB_CELL_FORMAT_RINGS=0) for none; the
+  // results are bit-identical either way.  0: never, 1: always, 2: by size
+  static const int epi_wg = [] {
+    const char* e = getenv("MVB_CELL_EPI_WG"), *r = getenv("MVB_CELL_FORMAT_RINGS");
+    if ((e && e[0] == '0') || (r && r[0] == '0')) return 0;
+    return (e && e[0] == '1') ? 1 : 2;
+  }();
   CellMaps tm;
   const int P16 = mixed ? 1 : kBf16Planes;      // 16-bit "planes" the A / B maps describe
   const uint32_t ra8 = (uint32_t)((BLOCK_M + 2 * (W + 2) + 7) & ~7);      // rows of an A stage (see CellCfg)
@@ -947,6 +1338,19 @@ int cell_fwd(const CellStep& s, cudaStream_t stream) {
     if (rc) return rc;
     col_scale = reinterpret_cast<const float*>(b8 + 2ull * kGates * ktot);
   }
+  if (mixed && epi_wg) {
+    const uint8_t* b8 = reinterpret_cast<const uint8_t*>(s.w) + 2ull * kGates * ktot;
+    // cell_fwd_epi_kernel: weight rows as [32 rows][2 halves][16 (256-column tile, gate)], a box of 32 rows x 1 half
+    // x 4 gates (2 for each CTA of a pair) is one N tile of 128 columns
+    const uint64_t d16[4] = {ktot, 32, 2, 16}, s16[3] = {ktot * 2, 32 * ktot * 2, 64 * ktot * 2};
+    const uint64_t d8[4] = {2 * ktot, 32, 2, 16}, s8[3] = {2 * ktot, 32 * 2 * ktot, 64 * 2 * ktot};
+    const uint32_t q16[4] = {CHUNK, 32, 1, 4}, q16h[4] = {CHUNK, 32, 1, 2};
+    const uint32_t q8[4] = {ROW_BYTES, 32, 1, 4}, q8h[4] = {ROW_BYTES, 32, 1, 2};
+    if ((rc = encode_tmap_4d_bf16(&tm.Bq, s.w, d16, s16, q16, 128))) return rc;
+    if ((rc = encode_tmap_4d_bf16(&tm.Bqh, s.w, d16, s16, q16h, 128))) return rc;
+    if ((rc = encode_tmap_4d_u8(&tm.B8q, b8, d8, s8, q8, 128))) return rc;
+    if ((rc = encode_tmap_4d_u8(&tm.B8qh, b8, d8, s8, q8h, 128))) return rc;
+  }
 
   CellParams prm;
   prm.bias = s.bias; prm.col_scale = col_scale; prm.c_in = s.c_in; prm.row_map = s.row_map; prm.c_out = s.c_out;
@@ -966,7 +1370,8 @@ int cell_fwd(const CellStep& s, cudaStream_t stream) {
   int dev = 0, num_sms = 0;
   MVB_CHECK_CUDA(cudaGetDevice(&dev));
   MVB_CHECK_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-  rc = mixed ? launch_cell<1>(tm, prm, num_sms, multicast, stream) : launch_cell<0>(tm, prm, num_sms, multicast, stream);
+  rc = mixed ? launch_cell<1>(tm, prm, num_sms, multicast, epi_wg, stream)
+             : launch_cell<0>(tm, prm, num_sms, multicast, 0, stream);
   if (rc || !fan) return rc;
   // fan-out stage 2: every parent row -> its K children (c_out / h32_out hold NS * fanout sample rows)
   const unsigned blocks = (unsigned)((NS * H * W * 32 + 255) / 256);      // a warp per parent cell

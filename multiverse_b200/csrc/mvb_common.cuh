@@ -327,6 +327,14 @@ __device__ __forceinline__ void tma_load_3d_mc(void* dst, const CUtensorMap* m, 
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_4d_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0,
+                                               int c1, int c2, int c3, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(mask)
+      : "memory");
+}
 // arrive on the barrier at the same offset in CTA `cta` of the cluster
 __device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
   asm volatile(
@@ -378,5 +386,7 @@ int encode_tmap_3d_u8(CUtensorMap* out, const void* base, uint64_t d0, uint64_t 
 int encode_tmap_4d_bf16(CUtensorMap* out, const void* base, const uint64_t (&dims)[4],
                         const uint64_t (&strides_bytes)[3], const uint32_t (&box)[4],
                         int swizzle_bytes);
+int encode_tmap_4d_u8(CUtensorMap* out, const void* base, const uint64_t (&dims)[4],
+                      const uint64_t (&strides_bytes)[3], const uint32_t (&box)[4], int swizzle_bytes);
 
 }  // namespace mvb

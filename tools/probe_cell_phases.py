@@ -8,11 +8,14 @@ multiverse_b200.build.build_variant) and runs the class-decoder cell - x-fold, r
 of every beam step after the first - with the pair kernel on three grids: the c4 beam step (10 240 sample rows of
 36x18), 18x32 and 18x9.  In the probe build every warpgroup's first thread sums clock64() per phase:
   MMA warpgroups:  waiting for a weight slot (full_bar), for an A stage (afull_bar), in wgmma.wait_group, in the
-                   epilogue (state update and stores), and the rest (descriptors, MMA issue, barrier arrivals);
-  TMA producer:    waiting for a free weight slot (empty_bar), for a free A stage (aempty_bar), the rest.
+                   epilogue (state update and stores; with the epilogue warpgroup: the copy of the accumulators into
+                   the staging buffer), waiting for the staging buffer to be free, and the rest (descriptors, MMA
+                   issue, barrier arrivals);
+  TMA producer:    waiting for a free weight slot (empty_bar), for a free A stage (aempty_bar), the rest;
+  epilogue warpgroup (cell_fwd_epi_kernel only): waiting for a staged tile, and the rest (the epilogue).
 Shares are of each role's total cycles.  The clocks of a launch are the consumer cycles per warpgroup over the
-event-timed launch time.  --compare runs it once per ring layout (MVB_CELL_FORMAT_RINGS=0 and 1) in child
-processes.  The probe build adds clock reads to the mainloop, so its launch times are a little longer than the
+event-timed launch time.  --compare runs it once per kernel (MVB_CELL_EPI_WG=0: the MMA warpgroups run the
+epilogue; 1: the epilogue warpgroup does) in child processes.  The probe build adds clock reads to the mainloop, so its launch times are a little longer than the
 product's; the shares are what it is for.
 """
 from __future__ import annotations
@@ -29,9 +32,9 @@ sys.path.insert(0, ROOT)
 
 # CellProbePhase (csrc/mvb_cell.cu), then the ring of the last launch
 PHASES = ["full_wait", "afull_wait", "mma_wait", "epilogue", "consumer", "empty_wait", "aempty_wait", "producer",
-          "tiles"]
+          "free_wait", "staged_wait", "epi_busy", "tiles"]
 SHAPES = [("c4 beam step", 36, 18, 10240), ("18x32", 18, 32, 4096), ("18x9", 18, 9, 10240)]
-MMA_CLOCKS_PER_SLOT = 1024     # one weight slot: 4 m64n256 MMAs per warpgroup, k16 fp16 or k32 e4m3
+MMA_CLOCKS_PER_SLOT = 1024     # one weight slot of 256 columns: 4 m64n256 MMAs per warpgroup, k16 fp16 or k32 e4m3
 
 
 def card():
@@ -57,9 +60,13 @@ def run(lib_path, reps):
   from multiverse_b200 import ops
   dev = torch.device("cuda:0")
   rings = os.environ.get("MVB_CELL_FORMAT_RINGS", "1")
-  print("card: %s; SMs %d; rings: %s" % (card(), torch.cuda.get_device_properties(0).multi_processor_count,
-                                         "bf16x2-sized (MVB_CELL_FORMAT_RINGS=0)" if rings == "0" else "format-sized"),
+  epi_wg = os.environ.get("MVB_CELL_EPI_WG", "1") != "0" and rings != "0"
+  print("card: %s; SMs %d; rings: %s; %s" % (
+      card(), torch.cuda.get_device_properties(0).multi_processor_count,
+      "bf16x2-sized (MVB_CELL_FORMAT_RINGS=0)" if rings == "0" else "format-sized",
+      "epilogue warpgroup (128-column tiles)" if epi_wg else "epilogue on the MMA warpgroups (MVB_CELL_EPI_WG=0)"),
         flush=True)
+  cols = 128 if epi_wg else 256      # columns of an N tile
   cx = 32
   g = torch.Generator(device=dev)
   g.manual_seed(7)
@@ -95,18 +102,23 @@ def run(lib_path, reps):
     cons, prod = float(v["consumer"]), float(v["producer"])
     ghz = cons / (2 * ctas * reps) / (ms * 1e6)
     wg_tiles = v["tiles"] / (2 * ctas)          # tiles per warpgroup (= per CTA), over the reps
-    clk_tile = cons / v["tiles"]
+    clk_tile = cons / v["tiles"] * (256 // cols)      # per 128 x 256 of work
     ideal = 8 * 9 * MMA_CLOCKS_PER_SLOT          # x-fold: 4 h chunks x 2 passes x 9 taps
-    other_c = cons - sum(v[k] for k in ("full_wait", "afull_wait", "mma_wait", "epilogue"))
+    other_c = cons - sum(v[k] for k in ("full_wait", "afull_wait", "mma_wait", "epilogue", "free_wait"))
     other_p = prod - v["empty_wait"] - v["aempty_wait"]
     pct = lambda x, tot: 100.0 * x / tot
     print("%s: %d sample rows of %dx%d, %d M tiles; rings %d weight slots + %d A stages of %d B; %.2f ms/launch, "
-          "%.2f GHz effective SM clock, %.1f tiles per CTA, %.0f clocks per tile (%.0f tensor clocks: %.2f)"
+          "%.2f GHz effective SM clock, %.1f tiles per CTA, %.0f clocks per 128x256 of work (%.0f tensor clocks: %.2f)"
           % (tag, ns, h, w, -(-ops.halo_rows(ns, h, w) // 128), b_slots, a_stages, a_stage_bytes, ms, ghz,
              wg_tiles / reps, clk_tile, ideal, ideal / clk_tile))
     print("  MMA warpgroups: full_bar wait %.1f%%, afull_bar wait %.1f%%, wgmma wait %.1f%%, epilogue %.1f%%, "
-          "issue/other %.1f%%" % (pct(v["full_wait"], cons), pct(v["afull_wait"], cons), pct(v["mma_wait"], cons),
-                                  pct(v["epilogue"], cons), pct(other_c, cons)))
+          "staging-free wait %.1f%%, issue/other %.1f%%"
+          % (pct(v["full_wait"], cons), pct(v["afull_wait"], cons), pct(v["mma_wait"], cons), pct(v["epilogue"], cons),
+             pct(v["free_wait"], cons), pct(other_c, cons)))
+    if epi_wg:
+      epi = float(v["staged_wait"] + v["epi_busy"])
+      print("  epilogue warpgroup: staged wait %.1f%%, epilogue %.1f%% (%.0f clocks per tile)"
+            % (pct(v["staged_wait"], epi), pct(v["epi_busy"], epi), v["epi_busy"] / max(v["tiles"] / 2, 1)))
     print("  TMA producer:   empty_bar wait %.1f%%, aempty_bar wait %.1f%%, issue/other %.1f%%"
           % (pct(v["empty_wait"], prod), pct(v["aempty_wait"], prod), pct(other_p, prod)), flush=True)
     del xh, ids, row_map, c_in, c_out, h_out
@@ -117,7 +129,7 @@ def main():
   ap = argparse.ArgumentParser()
   ap.add_argument("--lib", default=None, help="a library built with MVB_CELL_PROBE (default: build one now)")
   ap.add_argument("--reps", type=int, default=5)
-  ap.add_argument("--compare", action="store_true", help="run once per ring layout, in child processes")
+  ap.add_argument("--compare", action="store_true", help="run once per kernel (MVB_CELL_EPI_WG=0, 1), in child processes")
   args = ap.parse_args()
   tmp = None
   if args.lib is None:
@@ -125,8 +137,8 @@ def main():
     tmp = tempfile.TemporaryDirectory(prefix="mvb_probe_")
     args.lib = build.build_variant(tmp.name, ["MVB_CELL_PROBE"])
   if args.compare:
-    for rings in ("0", "1"):
-      env = dict(os.environ, MVB_CELL_FORMAT_RINGS=rings)
+    for epi_wg in ("0", "1"):
+      env = dict(os.environ, MVB_CELL_EPI_WG=epi_wg)
       r = subprocess.run([sys.executable, "-B", os.path.abspath(__file__), "--lib", args.lib, "--reps",
                           str(args.reps)], env=env, cwd=ROOT)
       if r.returncode:
