@@ -7,6 +7,7 @@ arithmetic step is a kernel of the C-ABI library:
 
   scene CNN (:146-165)                      -> mvb_scene_conv_fwd x2, mvb_scene_time_mean
   class encoder (:210-215, dynamic_rnn)      -> T x [mvb_enc_class_input, mvb_convlstm_cell_fwd]
+    without use_scene_enc (:218-229)         -> T x mvb_convlstm_cell_fwd_onehot (no scene CNN)
   regression encoder (:232-234)              -> T x [mvb_nhwc_to_planes, mvb_convlstm_cell_fwd]
   greedy class decoder (:311-471, raw_rnn)   -> Tp x [mvb_gnn_attend_fwd, mvb_convlstm_cell_fwd_onehot,
                                                      mvb_head_class_fwd (logits+argmax)]
@@ -27,6 +28,9 @@ import torch
 from . import ops
 
 P_ = "person_pred/"
+# the class encoder's input embedding without use_scene_enc (code/pred_models.py:221-225): created under the top scope
+# with AUTO_REUSE, so one variable serves every scale
+ENC_EMB = (P_ + "grid_emb/W", P_ + "grid_emb/b")
 
 
 def _names(i):
@@ -52,7 +56,7 @@ def _names(i):
 class ScaleWeights(object):
   """Packed / device-resident weights of one grid scale."""
 
-  def __init__(self, weights, i, planes, fast_class=False, fast=False):
+  def __init__(self, weights, i, planes, fast_class=False, fast=False, scene_enc=True):
     nm = _names(i)
     f = lambda n: weights[n].detach().to(torch.float32).contiguous()
     fp = ops.PLANES_F16F8 if fast else planes
@@ -79,6 +83,19 @@ class ScaleWeights(object):
     self.head_reg = f(nm["head_reg"])
     # inference: the class decoder's embedded one-hot input folded into table look-ups
     self.dec_class_xf = ops.XFold(f(nm["dec_class"][0]), f(nm["dec_class"][1]), *self.emb_class)
+    # without scene encoding the class encoder's input, grid_emb(one_hot(label)), has the decoder's form: folded the
+    # same way at inference (enc_class_fold); training embeds it (emb_onehot_fwd)
+    self.enc_emb = self._enc_class_xf = None
+    if not scene_enc:
+      self.enc_emb = (f(ENC_EMB[0]), f(ENC_EMB[1]))
+      self._enc_cell = (f(nm["enc_class"][0]), f(nm["enc_class"][1]))
+
+  def enc_class_fold(self):
+    """XFold of the class encoder's embedded one-hot input (models without scene encoding), built on first use: the
+    training step, which repacks the weights after every update, never reads it."""
+    if self._enc_class_xf is None:
+      self._enc_class_xf = ops.XFold(*self._enc_cell, *self.enc_emb)
+    return self._enc_class_xf
 
 
 class ConvRNNEngine(object):
@@ -103,8 +120,8 @@ class ConvRNNEngine(object):
     self.fast_planes = ops.PLANES_F16F8 if self.fast else self.planes
     assert cfg.enc_hidden_size == ops.HIDDEN and cfg.dec_hidden_size == ops.HIDDEN, \
         "the kernels are specialised for hidden size 256 (every published config)"
-    assert cfg.use_scene_enc, "only the published use_scene_enc path is implemented"
     assert cfg.convlstm_kernel == 3 and cfg.scene_conv_kernel == 3
+    assert cfg.use_scene_enc or cfg.emb_size == 32, "without use_scene_enc the class encoder's input is emb_size 32"
     assert cfg.scene_conv_dim == 64
     assert getattr(cfg, "activation_func", "tanh") in ("tanh",) or \
         getattr(cfg.activation_func, "__name__", "") == "tanh", "kernels implement tanh"
@@ -119,7 +136,13 @@ class ConvRNNEngine(object):
     """False = SimAug's model variant: its gnn_edge (SimAug/code/pred_models.py:1213-1226) concatenates the scene
     features to the node features only under `if tile_to_beam:`, so the greedy class decoder (training, test.py)
     attends over h alone; the Multiverse file (code/pred_models.py:824-838) always uses them (default)."""
-    return bool(getattr(self.cfg, "gnn_scene_in_greedy", True))
+    return bool(self.scene_enc and getattr(self.cfg, "gnn_scene_in_greedy", True))
+
+  @property
+  def scene_enc(self):
+    """use_scene_enc (code/pred_models.py:146, :184-229, :824): the scene CNN feeds the class encoder and the graph
+    attention; without it the class encoder reads grid_emb(one_hot(label))."""
+    return bool(getattr(self.cfg, "use_scene_enc", True))
 
   # ------------------------------------------------------------------ weights
   def set_weights(self, weights):
@@ -128,11 +151,12 @@ class ConvRNNEngine(object):
       self._graphs.clear()      # captured graphs point at the previous weight buffers
       self._graph_seen.clear()
     w = {k: (v if torch.is_tensor(v) else torch.as_tensor(v)).to(dev) for k, v in weights.items()}
+    scene_enc = self.scene_enc
     self.scene_w = [(w[P_ + "scene_conv%d/W" % (i + 1)].float().contiguous(),
                      w[P_ + "scene_conv%d/b" % (i + 1)].float().contiguous())
-                    for i in range(len(self.cfg.scene_grid_strides))]
-    self.scales = [ScaleWeights(w, i, self.planes, self.fast_class, self.fast) if self.cfg.use_grids[i] else None
-                   for i in range(len(self.cfg.scene_grids))]
+                    for i in range(len(self.cfg.scene_grid_strides))] if scene_enc else []
+    self.scales = [ScaleWeights(w, i, self.planes, self.fast_class, self.fast, scene_enc) if self.cfg.use_grids[i]
+                   else None for i in range(len(self.cfg.scene_grids))]
 
   # ------------------------------------------------------------------ buffers
   def _buf(self, key, maker):
@@ -166,7 +190,10 @@ class ConvRNNEngine(object):
   # ------------------------------------------------------------------ pieces
   def scene_cnn(self, scene_feat, obs_scene):
     """code/pred_models.py:146-165 on the unique frames; returns per-scale [F,h,w,64] maps and
-    the per-sample time means used by the graph attention (:826-828)."""
+    the per-sample time means used by the graph attention (:826-828).  Without use_scene_enc nothing reads the scene
+    (:146, :824): None per scale."""
+    if not self.scene_enc:
+      return [None] * len(self.cfg.scene_grids), [None] * len(self.cfg.scene_grids)
     x = scene_feat
     convs, means = [], []
     for (W, b) in self.scene_w:
@@ -176,8 +203,9 @@ class ConvRNNEngine(object):
     return convs, means
 
   def encode_class(self, i, scene_conv, obs_scene_t, labels_t, xh_out):
-    """Class encoder (:210-215).  obs_scene_t / labels_t: int32 [T,N].  Writes the planes of the
-    last h into the h block of xh_out (if given) and returns (c, h32) halo buffers."""
+    """Class encoder (:210-215; without use_scene_enc :218-229, scene_conv None).  obs_scene_t / labels_t: int32
+    [T,N].  Writes the planes of the last h into the h block of xh_out (if given) and returns (c, h32) halo
+    buffers."""
     h, w = self.cfg.scene_grids[i]
     n = labels_t.shape[1]
     t_len = labels_t.shape[0]
@@ -185,6 +213,17 @@ class ConvRNNEngine(object):
     xh = self._xh("enc_class", n, h, w, sw.enc_class.cpad, self.fast_planes)
     c = [self._state("enc_c0", n, h, w), self._state("enc_c1", n, h, w)]
     h32 = self._state("enc_h32", n, h, w)
+    if sw.enc_emb is not None:
+      # the embedded one_hot(label_t) input is folded into table look-ups: nobody writes the x blocks
+      xf = sw.enc_class_fold()
+      xh[0][:, :, sw.enc_class.cxp:].zero_()   # h_0 = 0
+      for t in range(t_len):
+        cur, nxt = xh[t % 2], xh[(t + 1) % 2]
+        last = t == t_len - 1
+        self._cell("enc_class", (h, w, n), ops.cell_fwd_onehot, cur, sw.enc_class, xf, labels_t[t],
+                   None if t == 0 else c[t % 2], c[(t + 1) % 2], h32 if last else None, xh_out if last else nxt,
+                   h, w, n)
+      return c[t_len % 2], h32
     if sw.enc_class_xs is not None:
       # (one table per scale: the chains of different scales run concurrently under forward_graph)
       table = self._buf(("enc_class_xtab", n, h, w), lambda: torch.empty((n, 9, 4 * ops.HIDDEN), dtype=torch.float32,

@@ -141,6 +141,9 @@ class Model(object):
     self._own_vars.append(v)
     return v
 
+  def _var_names(self):
+    return {v.name.split(":")[0] for v in self._own_vars}
+
   def _variables_changed(self):
     self._stale = True
 
@@ -162,10 +165,9 @@ class Model(object):
     """code/pred_models.py:123-308: declares the variables under the reference's names and the
     fetch handles; the computation itself is ConvRNNEngine.forward."""
     cfg = self.config
-    assert cfg.use_scene_enc, "only the published --use_scene_enc models are implemented"
     zeros = lambda shp, rng: np.zeros(shp, dtype=np.float32)
     cin = cfg.scene_class
-    for i in range(len(cfg.scene_grid_strides)):
+    for i in range(len(cfg.scene_grid_strides) if cfg.use_scene_enc else 0):
       self._var("person_pred/scene_conv%d/W" % (i + 1), (3, 3, cin, cfg.scene_conv_dim), init=_he)
       self._var("person_pred/scene_conv%d/b" % (i + 1), (cfg.scene_conv_dim,), init=zeros)
       cin = cfg.scene_conv_dim
@@ -179,7 +181,12 @@ class Model(object):
         continue
       cell = lambda name, cx: (self._var(name + "/kernel", (k, k, cx + ch, 4 * ch), init=_glorot),
                                self._var(name + "/biases", (4 * ch,), init=zeros))
-      cell(p + "encoder_grid_class_%d/enc_grid_%d" % (i, i), cfg.scene_conv_dim)
+      if not cfg.use_scene_enc and p + "grid_emb/W" not in self._var_names():
+        # the class encoder's embedding of one_hot(label): created under the top scope with AUTO_REUSE (:221-225,
+        # :1339), so every scale shares it
+        self._var(p + "grid_emb/W", (3, 3, 1, e), init=_he)
+        self._var(p + "grid_emb/b", (e,), init=zeros)
+      cell(p + "encoder_grid_class_%d/enc_grid_%d" % (i, i), cfg.scene_conv_dim if cfg.use_scene_enc else e)
       cell(p + "encoder_grid_reg_%d/enc_grid_regress_%d" % (i, i), 2)
       for kind, cname, pdim in (("class", "dec_grid_%d" % i, 1), ("reg", "dec_grid_reg_%d" % i, 2)):
         d = p + "decoder_grid_%s_%d/decoder_rnn/" % (kind, i)
@@ -661,6 +668,10 @@ def _engine_config(config):
   # tile_to_beam): a config that carries SimAug's flags selects that variant unless it says otherwise
   simaug = any(hasattr(config, k) for k in ("multiview_train", "adv_train"))
   d["gnn_scene_in_greedy"] = bool(getattr(config, "gnn_scene_in_greedy", not simaug))
+  aug = [k for k in ("adv_train", "multiview_train", "standard_aug", "norm_input") if getattr(config, k, False)]
+  if not config.use_scene_enc and aug:
+    raise NotImplementedError("--%s without --use_scene_enc: SimAug's model always encodes the scene, and its "
+                              "augmentations act on the scene input" % " / --".join(aug))
   for flag in ("use_single_decoder", "use_teacher_forcing"):
     if getattr(config, flag, False):
       raise NotImplementedError("--%s is not implemented (no published config uses it)" % flag)

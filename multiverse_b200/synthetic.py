@@ -34,7 +34,7 @@ def make_config(**kw):
 def weight_shapes(cfg):
   k, ch, e, cs = cfg.convlstm_kernel, cfg.enc_hidden_size, cfg.emb_size, cfg.scene_conv_dim
   shp, cin = {}, cfg.scene_class
-  for i in range(len(cfg.scene_grid_strides)):
+  for i in range(len(cfg.scene_grid_strides) if cfg.use_scene_enc else 0):
     shp["person_pred/scene_conv%d/W" % (i + 1)] = (3, 3, cin, cs)
     shp["person_pred/scene_conv%d/b" % (i + 1)] = (cs,)
     cin = cs
@@ -42,7 +42,11 @@ def weight_shapes(cfg):
   for i in range(len(cfg.scene_grids)):
     if not cfg.use_grids[i]:
       continue
-    shp[p + "encoder_grid_class_%d/enc_grid_%d/kernel" % (i, i)] = (k, k, cs + ch, 4 * ch)
+    if not cfg.use_scene_enc:
+      # the class encoder's embedding of one_hot(label) (code/pred_models.py:221-225), one variable for every scale
+      shp.setdefault(p + "grid_emb/W", (3, 3, 1, e))
+      shp.setdefault(p + "grid_emb/b", (e,))
+    shp[p + "encoder_grid_class_%d/enc_grid_%d/kernel" % (i, i)] = (k, k, (cs if cfg.use_scene_enc else e) + ch, 4 * ch)
     shp[p + "encoder_grid_class_%d/enc_grid_%d/biases" % (i, i)] = (4 * ch,)
     shp[p + "encoder_grid_reg_%d/enc_grid_regress_%d/kernel" % (i, i)] = (k, k, 2 + ch, 4 * ch)
     shp[p + "encoder_grid_reg_%d/enc_grid_regress_%d/biases" % (i, i)] = (4 * ch,)

@@ -15,6 +15,8 @@ all-reduced across ranks) and the class decoder fed its own logits map instead o
 
 Per cell step the backward is  lstm_gates_bwd -> cell_dgrad (wgmma) -> cell_wgrad_direct (wgmma,
 MN-major operands read straight from the stored planes);  around it: head_bwd, emb_bwd, gnn_bwd, enc_class_input_bwd, scene_*_bwd.
+Without use_scene_enc the class encoder's input is embedded by emb_onehot_fwd and its gradient goes through emb_bwd into
+the one grid_emb variable every scale and step shares (code/pred_models.py:218-229); there is no scene CNN.
 """
 from __future__ import annotations
 
@@ -23,7 +25,7 @@ import math
 import torch
 
 from . import ops
-from .engine import ConvRNNEngine, P_, _names
+from .engine import ENC_EMB, ConvRNNEngine, P_, _names
 
 HID = ops.HIDDEN
 
@@ -107,11 +109,15 @@ class TrainEngine(ConvRNNEngine):
     xh = xs("xh_ec", T, sw.enc_class.cpad); c = st("c_ec", T); g = gt("g_ec", T)
     h32_last = self._one(("h32_ec", i, n), lambda: ops.alloc_state(n, h, w, dev))
     xh_dc = xs("xh_dc", Tp, sw.dec_class.cpad)
+    assert sw.enc_emb is None or mix is None, "SimAug's mixup perturbs the scene input, which this model does not have"
     for t in range(T):
-      xh[t][:, :, :sw.enc_class.cxp].zero_()
+      if sw.enc_emb is None:
+        xh[t][:, :, :sw.enc_class.cxp].zero_()
       if t == 0:
         xh[0][:, :, sw.enc_class.cxp:].zero_()
-      if mix is None:
+      if sw.enc_emb is not None:    # tanh(conv3x3(one_hot(label_t)) + b) into every valid cell of the x block
+        ops.emb_onehot_fwd(labels_t[t], *sw.enc_emb, xh[t], h, w)
+      elif mix is None:
         ops.enc_class_input(convs[i], obs_scene_t[t], labels_t[t], None, xh[t], h, w)
       else:          # SimAug multiview_exp 3: the observed class map is a mix of two views' one-hot maps
         ops.enc_class_input_mix(convs[i], obs_scene_t[t], labels_t[t], labels2_t[t], mix["beta"], xh[t], h, w)
@@ -252,8 +258,10 @@ class TrainEngine(ConvRNNEngine):
         dlogits *= focal.float()[None, :, None]
       ops.loss_fwd_bwd(None, None, None, 0.0, S["offs"], tgt, doffs, rw, loss_out)
     # ---- class decoder
-    dsm = self._one(("dsm", i, n), lambda: torch.zeros_like(means[i]))
-    dsm.zero_()
+    dsm = None
+    if self.scene_enc:
+      dsm = self._one(("dsm", i, n), lambda: torch.zeros_like(means[i]))
+      dsm.zero_()
     work = self._one(("gnnwork", i, n), lambda: torch.empty((19 * n * h * w,), device=dev))
     We, be = sw.emb_class
     dc = None
@@ -285,7 +293,9 @@ class TrainEngine(ConvRNNEngine):
     for t in range(T - 1, -1, -1):
       dxh, dc = self._cell_bwd(S, i, sw.enc_class, cgr["enc_class"], S["xh_ec"][t], S["g_ec"][t],
                                None if t == 0 else S["c_ec"][t - 1], S["c_ec"][t], dh, dc)
-      if mix is None:
+      if sw.enc_emb is not None:    # summed over steps and scales (the kernel adds into the shared gradient)
+        ops.emb_bwd(dxh, S["labels_t"][t], None, *sw.enc_emb, G[ENC_EMB[0]], G[ENC_EMB[1]], None, False, h, w, n)
+      elif mix is None:
         ops.enc_class_input_bwd(dxh, S["obs_scene_t"][t], S["labels_t"][t], dconv[i], h, w)
       else:
         ops.enc_class_input_mix_bwd(dxh, S["obs_scene_t"][t], S["labels_t"][t], S["labels2_t"][t], mix["beta"],
@@ -360,7 +370,8 @@ class TrainEngine(ConvRNNEngine):
     convs, means = self.scene_cnn(scene_feat, obs_scene)
     used = [i for i in range(len(cfg.scene_grids)) if cfg.use_grids[i]]
     loss_out = torch.zeros((len(cfg.scene_grids), 2), dtype=torch.float32, device=dev)
-    dconv = [torch.zeros_like(c) for c in convs]
+    dconv = [None if c is None else torch.zeros_like(c) for c in convs]
+    assert dscene_out is None or self.scene_enc, "the scene-input gradient needs a model that encodes the scene"
     fg = None
     mask = getattr(cfg, "mask_grid_regression", False)
     assert fg_count is None or mask, "fg_count is the denominator of the masked regression loss (mask_grid_regression)"
@@ -379,7 +390,7 @@ class TrainEngine(ConvRNNEngine):
                            cls_w * loss_scale, reg_w * loss_scale, fg)
     # scene CNN backward: conv_k -> conv_{k-1} chain (code/pred_models.py:155-165)
     ins = [scene_feat] + convs[:-1]
-    for k in range(len(convs) - 1, -1, -1):
+    for k in range(len(self.scene_w) - 1, -1, -1):
       W, _ = self.scene_w[k]
       ops.scene_conv_bwd(ins[k], W, convs[k], dconv[k], self.grads[P_ + "scene_conv%d/W" % (k + 1)],
                          self.grads[P_ + "scene_conv%d/b" % (k + 1)], dconv[k - 1] if k > 0 else dscene_out)
