@@ -32,6 +32,7 @@ namespace mvb {
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_N = 256;
 constexpr int XPAD = 32;      // the x block is zero-padded to a multiple of 32 channels (cpad = roundup(cx,32) + 256)
+constexpr int kMaxXBlock = 256;   // widest x block of the GEMM: four 64-channel chunks (emb_size up to 256)
 constexpr int CHUNK = 64;     // channels per K chunk: 64 16-bit elements = 128 B = one SWIZZLE_128B row
 constexpr int ROW_BYTES = 128;
 constexpr int MMA_K = 16;       // K of one 16-bit wgmma
@@ -310,6 +311,15 @@ __device__ __forceinline__ void epi_pair(const CellParams& prm, const EpiRow& r,
   }
 }
 
+// MMA steps of x chunk q (channels [64 q, +64) of the x block, cut at its end cxp): K16 steps of a 16-bit plane,
+// K32 steps of one e4m3 plane, and the distance in 16-byte units from e0 to e1 in an fp8 row (f8_off).
+__device__ __forceinline__ void x_chunk_steps(int q, int cxp, int cpad, int& ks16, int& ks8, uint32_t& poff) {
+  const int c16 = q * CHUNK, width = cxp - c16 < CHUNK ? cxp - c16 : CHUNK;
+  ks16 = width / MMA_K;
+  ks8 = width / 32;
+  poff = (uint32_t)(f8_off(c16, 1, cpad) - f8_off(c16, 0, cpad)) >> 4;
+}
+
 // MC = true: clusters of two CTAs work on two M tiles of the same N tile in lock step; each loads half of every B
 // (weight) tile and TMA-multicasts it to both, so the L2 -> shared-memory traffic per CTA and stage drops from
 // 48 KB to 32 KB (bf16x2).  A slot may be refilled once the MMA warpgroups of BOTH CTAs have consumed it (empty
@@ -340,12 +350,13 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int lane = threadIdx.x & 31;
   const int wg = warp >> 2;                    // 0: TMA producer; 1, 2: MMA + epilogue of rows [64 (wg - 1), +64)
   const Grid g = make_grid(prm.H, prm.W);
-  // K chunks of 64 channels: the x chunk [0, 64) - of which only the cxp channels of the x block are multiplied -
-  // then the four chunks of the h block [cxp + 64 j, +64).  fp8 rows (f16f8): [x: e0 (cxp) | e1 (cxp)] then per h
-  // chunk [e0 (64) | e1 (64)], 2 * cpad bytes per row (mvb_common.cuh f8_off).
+  // K chunks of 64 channels: the nqx x chunks [64 q, +64) - of which only the cxp channels of the x block are
+  // multiplied, so the last one may be half a chunk - then the four chunks of the h block [cxp + 64 j, +64).  fp8 rows
+  // (f16f8): both e4m3 planes of a chunk side by side (mvb_common.cuh f8_off), 2 * cpad bytes per row.
   const int cxp = prm.cpad - kHidden;
-  const int q_begin = prm.skip_x ? 1 : 0;
-  constexpr int NQ = 1 + kHidden / CHUNK;      // 5
+  const int nqx = (cxp + CHUNK - 1) / CHUNK;
+  const int q_begin = prm.skip_x ? nqx : 0;
+  const int NQ = nqx + kHidden / CHUNK;
   // f16f8: two passes over K, the e4m3 cross terms first and then the fp16 main products.  The e4m3 MMAs accumulate
   // with a short internal sum (about 14 significant bits of the accumulator), so they run while the accumulator holds
   // only their own small sum (~2^-11 of the result); the fp16 MMAs, exact in fp32, then add the main products.
@@ -392,8 +403,8 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         // onto a large transient partial sum.
         for (int pass = 0; pass < NPASS; ++pass)
         for (int q = q_begin; q < NQ; ++q) {
-          const int c16 = q == 0 ? 0 : cxp + (q - 1) * CHUNK;              // 16-bit channel coordinate
-          const int c8 = q == 0 ? 0 : 2 * cxp + (q - 1) * 2 * CHUNK;       // fp8 byte coordinate
+          const int c16 = q < nqx ? q * CHUNK : cxp + (q - nqx) * CHUNK;     // 16-bit channel coordinate
+          const int c8 = f8_off(c16, 0, prm.cpad);                          // fp8 byte coordinate
           const bool f8 = FMT == 1 && pass == 0;
           CELL_PROBED(kProbeAEmptyWait, mbar_wait(&aempty_bar[astage], aphase ^ 1));
           uint8_t* sa = smem_a + astage * a_stage_bytes;
@@ -473,7 +484,7 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             const uint32_t b_lo = smem_u32(smem + slot * B_SLOT_BYTES) >> 4;
             wgmma_fence_regs(acc);
             wgmma_fence();
-            if (q > 0) {
+            if (q >= nqx) {
               // ---- h chunk: 64 channels = 4 K16 steps per 16-bit plane pair, 4 K32 steps over the two e4m3 planes ----
               if (f8) {
                 for (int k = 0; k < 4; ++k) mma8(a_lo + 2 * k, b_lo + 2 * k);    // [e0 (64 B) | e1 (64 B)]
@@ -486,9 +497,9 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                   for (int k = 0; k < 4; ++k) mma16(a_lo + pa * a_plane_lo + 2 * k, b_lo + 2 * k);
               }
             } else {
-              // ---- x chunk (only cells whose input is not folded): cxp = 32 or 64 channels ----
-              const int ks16 = cxp / MMA_K, ks8 = cxp / 32;
-              const uint32_t poff = (uint32_t)cxp >> 4;              // e1 sits cxp bytes after e0 in an fp8 row
+              // ---- x chunk (only cells whose input is not folded): 64 channels, or 32 for a trailing half chunk ----
+              int ks16, ks8; uint32_t poff;
+              x_chunk_steps(q, cxp, prm.cpad, ks16, ks8, poff);
               if (f8) {
                 for (int pk = 0; pk < 2 * ks8; ++pk) {
                   const uint32_t o = (pk / ks8) * poff + (pk % ks8) * 2;
@@ -653,8 +664,9 @@ cell_fwd_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   const int wg = warp >> 2;                    // 0: TMA producer; 1, 2: MMA of rows [64 (wg - 1), +64); 3: epilogue
   const Grid g = make_grid(prm.H, prm.W);
   const int cxp = prm.cpad - kHidden;
-  const int q_begin = prm.skip_x ? 1 : 0;
-  constexpr int NQ = 1 + kHidden / CHUNK;      // 5
+  const int nqx = (cxp + CHUNK - 1) / CHUNK;   // x chunks, then the four h chunks (as in cell_fwd_kernel)
+  const int q_begin = prm.skip_x ? nqx : 0;
+  const int NQ = nqx + kHidden / CHUNK;
   const long long num_m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
   const uint32_t rank = MC ? cluster_ctarank() : 0u;
   const long long num_tiles = (MC ? (num_m_tiles + 1) / 2 : num_m_tiles) * EW_N_TILES;
@@ -690,8 +702,8 @@ cell_fwd_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         const int half = nt & 1, tg0 = (nt >> 1) * 4;      // 32-row half and (tile, gate) index of gate 0
         for (int pass = 0; pass < 2; ++pass)
         for (int q = q_begin; q < NQ; ++q) {
-          const int c16 = q == 0 ? 0 : cxp + (q - 1) * CHUNK;
-          const int c8 = q == 0 ? 0 : 2 * cxp + (q - 1) * 2 * CHUNK;
+          const int c16 = q < nqx ? q * CHUNK : cxp + (q - nqx) * CHUNK;
+          const int c8 = f8_off(c16, 0, prm.cpad);
           const bool f8 = pass == 0;
           CELL_PROBED(kProbeAEmptyWait, mbar_wait(&aempty_bar[astage], aphase ^ 1));
           uint8_t* sa = smem_a + astage * a_stage_bytes;
@@ -758,7 +770,7 @@ cell_fwd_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           const uint32_t b_lo = smem_u32(smem_b + slot * EW_SLOT_BYTES) >> 4;
           wgmma_fence_regs(acc);
           wgmma_fence();
-          if (q > 0) {
+          if (q >= nqx) {
             if (f8) {
               for (int k = 0; k < 4; ++k) {           // [e0 (64 B) | e1 (64 B)]
                 wgmma_e4m3_n128(acc, desc_of(a_lo + 2 * k, kHi), desc_of(b_lo + 2 * k, kHi), fresh ^ 1u);
@@ -772,9 +784,9 @@ cell_fwd_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
               }
             }
           } else {
-            // ---- x chunk (only cells whose input is not folded): cxp = 32 or 64 channels ----
-            const int ks16 = cxp / MMA_K, ks8 = cxp / 32;
-            const uint32_t poff = (uint32_t)cxp >> 4;              // e1 sits cxp bytes after e0 in an fp8 row
+            // ---- x chunk (only cells whose input is not folded): 64 channels, or 32 for a trailing half chunk ----
+            int ks16, ks8; uint32_t poff;
+            x_chunk_steps(q, cxp, prm.cpad, ks16, ks8, poff);
             if (f8) {
               for (int pk = 0; pk < 2 * ks8; ++pk) {
                 const uint32_t o = (pk / ks8) * poff + (pk % ks8) * 2;
@@ -1291,7 +1303,9 @@ int cell_fwd(const CellStep& s, cudaStream_t stream) {
               "cell_fwd: fanout=%d needs the x-fold tables, c_in, h32_out, a [R,1024] fp32 workspace and no row_map / hp_out", s.fanout);
   MVB_REQUIRE(!s.xf_B || (s.xf_T2 && s.xf_ids && H >= 3 && W >= 3), "cell_fwd: x-fold needs its tables, ids and a grid of at least 3x3");
   MVB_REQUIRE((!s.xs_tab || s.xs_label) && (!s.xr_W || s.xr_in), "cell_fwd: the sparse x path needs its labels, the dense one its input");
-  MVB_REQUIRE(cpad == kHidden + XPAD || cpad == kHidden + 2 * XPAD, "cell_fwd: cpad=%d must be 288 or 320 (x block of 32 or 64 channels)", cpad);
+  MVB_REQUIRE(cpad % XPAD == 0 && cpad >= kHidden + XPAD && cpad <= kHidden + kMaxXBlock,
+              "cell_fwd: cpad=%d must be a multiple of %d from %d to %d (x block of 32 to %d channels)", cpad, XPAD,
+              kHidden + XPAD, kHidden + kMaxXBlock, kMaxXBlock);
   MVB_REQUIRE(NS > 0 && H > 0 && W > 0, "cell_fwd: bad sizes NS=%lld H=%d W=%d", NS, H, W);
   MVB_REQUIRE(s.xh && s.w && (s.bias || s.xf_B) && s.c_out, "cell_fwd: null pointer");
   if (s.hp_out) MVB_REQUIRE(s.cpad_out % 8 == 0 && s.ch_off_out % 8 == 0, "cell_fwd: hp_out pitch/offset must be multiples of 8");

@@ -88,8 +88,9 @@ __device__ __forceinline__ void split_planes(float v, __nv_bfloat16 (&out)[kBf16
 // instead of 3 at the accuracy class of the bf16 x 2-plane scheme.
 // Buffer layout for R rows of cpad channels: [fp16 R*cpad][fp8: R rows of 2*cpad bytes] = the bytes of two bf16
 // planes, so the same allocations serve both formats.  Inside an fp8 row the two planes are interleaved per K chunk
-// of the cell kernel, so that ONE 128-byte TMA row carries both (f8_off): [x block: e0 (cxp) | e1 (cxp)] then per
-// 64-channel chunk of the h block [e0 (64) | e1 (64)],  cxp = cpad - 256.
+// of the cell kernel, so that ONE 128-byte TMA row carries both (f8_off): per 64-channel chunk of the x block
+// [e0 (64) | e1 (64)], a trailing 32-channel chunk as [e0 (32) | e1 (32)], then per 64-channel chunk of the h block
+// [e0 (64) | e1 (64)],  cxp = cpad - 256 (a multiple of 32).  For cxp <= 64 the x block is [e0 (cxp) | e1 (cxp)].
 // ----------------------------------------------------------------------------------
 constexpr int kPlanesF16F8 = 16;
 constexpr float kF8ResidualScale = 4096.f;   // 2^12: residual of an fp16 rounding, brought into e4m3's range
@@ -101,7 +102,8 @@ inline bool valid_planes(int P) { return P == kBf16Planes || P == kPlanesF16F8; 
 __host__ __device__ __forceinline__ int f8_off(int c, int p, int cpad) {
   const int hoff = cpad - kHidden;
   if (c >= hoff) { const int cc = c - hoff; return 2 * hoff + (cc >> 6) * 128 + p * 64 + (cc & 63); }
-  return p * hoff + c;
+  const int c0 = c & ~63, width = hoff - c0 < 64 ? hoff - c0 : 64;     // c's x chunk: 64 channels, or a trailing 32
+  return 2 * c0 + p * width + (c & 63);
 }
 
 __device__ __forceinline__ uint8_t to_e4m3(float v) {

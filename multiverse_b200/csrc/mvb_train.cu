@@ -13,7 +13,8 @@
 //                    gate columns x N tiles of (tap, channel) units x k-splits; every (tile, k-split) adds into its
 //                    own fp32 slab of dW, which unpack_cell_wgrad sums (no atomics).
 // Both GEMMs use the forward kernel's bf16x2 operand format (products a0*b0 + a0*b1 + a1*b0) and the same
-// TMA / mbarrier pipeline with register accumulators.  dgrad tiles: two N tiles of cpad/2 when the x block is
+// TMA / mbarrier pipeline with register accumulators.  dgrad tiles: two N tiles of cpad/2 (cpad 288, 320) or of 192
+// / 256 columns (wider x blocks; the columns past cpad are zero-filled by TMA and not stored) when the x block is
 // needed, one N = 256 tile (h block only) when it is not (regression encoder).
 // Algorithmic FLOPs: dgrad = wgrad = forward (2*R*9*cpad*1024 each).
 #include "mvb_common.cuh"
@@ -47,7 +48,7 @@ struct GemmParams {
   int H, W;
   int cpad, bn;        // N tile
   int cxp;             // dgrad: width of the x block
-  int need_x;          // dgrad: 1 -> two N tiles of cpad/2 covering [0, cpad); 0 -> one N tile [cxp, cxp+256) (h only)
+  int need_x;          // dgrad: 1 -> two N tiles covering [0, cpad) (and up to 2 * bn); 0 -> one N tile [cxp, cxp+256) (h only)
   int num_kb;          // k-blocks per tile
   long long num_m_tiles;
   int num_n_tiles;
@@ -183,6 +184,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         const long long row = mt * G_BLOCK_M + 64 * c + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
         bool valid;
         float* dst;
+        int n_cols = BN;      // dgrad: columns of the tile inside [0, cpad)
         if (MODE == MODE_DGRAD) {
           valid = row < prm.R;
           if (valid) {
@@ -191,6 +193,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             valid = (x < g.W) && (y < g.H);
           }
           dst = prm.out + row * prm.cpad + (prm.need_x ? ntile * BN : prm.cxp);
+          n_cols = prm.need_x ? prm.cpad - ntile * BN : BN;
         } else {
           valid = row < kGates;
           dst = prm.out + (long long)(ntile % prm.ksplit) * kGates * 9LL * prm.cpad + row * (9LL * prm.cpad);
@@ -199,6 +202,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 #pragma unroll
         for (int i = 0; i < BN / 8; ++i) {
           const int col = 8 * i + 2 * (lane & 3);
+          if (MODE == MODE_DGRAD && col >= n_cols) continue;
           float2* d2 = reinterpret_cast<float2*>(dst + col);
           if (MN) {
             // column of the tile -> (unit, channel): dW[tap][chunk*ubn + c]; this (tile, k-split) owns its slab
@@ -378,6 +382,9 @@ static int launch_pgemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Ge
   return MVB_OK;
 }
 
+// x blocks of 32 to 256 channels
+static bool valid_gemm_cpad(int cpad) { return cpad % 32 == 0 && cpad >= kHidden + 32 && cpad <= 2 * kHidden; }
+
 static int num_sms_of_device(int* out) {
   int dev = 0;
   MVB_CHECK_CUDA(cudaGetDevice(&dev));
@@ -389,7 +396,7 @@ int cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, long lo
                int cpad, int P, int need_x, cudaStream_t stream) {
   MVB_REQUIRE(P == kBf16Planes, "cell_dgrad: planes P=%d must be 2 (the bf16x2 format)", P);
   MVB_REQUIRE(dg_planes && wd_planes && dxh && NS > 0, "cell_dgrad: bad args");
-  MVB_REQUIRE(cpad == 288 || cpad == 320, "cell_dgrad: cpad=%d unsupported", cpad);
+  MVB_REQUIRE(valid_gemm_cpad(cpad), "cell_dgrad: cpad=%d must be a multiple of 32 from 288 to 512", cpad);
   const int cxp = cpad - kHidden;
   const Grid g = make_grid(H, W);
   const long long R = NS * g.S;
@@ -398,8 +405,9 @@ int cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, long lo
                                (uint64_t)R * kGates * 2, G_BLOCK_K, G_BLOCK_M, kBf16Planes, 64);
   if (rc) return rc;
   const uint64_t ktot = 9ull * kGates;
-  // with the x block: two N tiles of cpad/2 (144 / 160); h only: one N tile of 256
-  const int bn = need_x ? cpad / 2 : 256;
+  // with the x block: two N tiles of cpad/2 (144 / 160), or of 192 (cpad <= 384) or 256 columns; h only: one N tile
+  // of 256
+  const int bn = !need_x ? 256 : cpad <= 320 ? cpad / 2 : cpad <= 384 ? 192 : 256;
   rc = encode_tmap_3d_bf16(&tmB, wd_planes, ktot, (uint64_t)cpad, kBf16Planes, ktot * 2, ktot * cpad * 2, G_BLOCK_K,
                            bn, kBf16Planes, 64);
   if (rc) return rc;
@@ -410,23 +418,42 @@ int cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, long lo
   prm.num_n_tiles = need_x ? 2 : 1;
   int sms = 0;
   if ((rc = num_sms_of_device(&sms))) return rc;
-  if (!need_x) return launch_pgemm<MODE_DGRAD, 256>(tmA, tmB, prm, sms, stream);
-  return cpad == 288 ? launch_pgemm<MODE_DGRAD, 144>(tmA, tmB, prm, sms, stream)
-                     : launch_pgemm<MODE_DGRAD, 160>(tmA, tmB, prm, sms, stream);
+  switch (bn) {
+    case 144: return launch_pgemm<MODE_DGRAD, 144>(tmA, tmB, prm, sms, stream);
+    case 160: return launch_pgemm<MODE_DGRAD, 160>(tmA, tmB, prm, sms, stream);
+    case 192: return launch_pgemm<MODE_DGRAD, 192>(tmA, tmB, prm, sms, stream);
+    default: return launch_pgemm<MODE_DGRAD, 256>(tmA, tmB, prm, sms, stream);
+  }
 }
 
-int cell_wgrad_mn_slabs(int cpad) { return cpad == 288 ? 5 : 2; }
+// K-split of the wgrad: every slab sums R / slabs halo rows, and the dW error grows with the rows a slab sums (1.5e-4
+// of the 2e-4 bar at 45 k rows: micro-batch 128 of 36x18 on 2 slabs).  cpad 288: 5 slabs (its N tiles are fewer);
+// cpad 320: 2; wider x blocks: 8.  At cpad 384 the whole-model gradient (summed over steps, scales and micro-batches)
+// measured 3.6e-4 on 2 slabs, 2.2e-4 on 5 and 1.5e-4 on 8 (H100, micro-batch 128 of 36x18).
+int cell_wgrad_mn_slabs(int cpad) { return cpad == 288 ? 5 : cpad == 320 ? 2 : 8; }
+
+// wgrad N tiles: units of ubn channels of one tap, upt units per tile.  cpad 288: two 96-wide units (N = 192 keeps the
+// MMA off the smem-bandwidth limit), cpad 320: one 160-wide unit; wider x blocks: the fewest units that fill a tile
+// of 256, 192 or 160 columns with a unit width (a multiple of 32) that divides cpad.  cpad 352 and 416 (11 and 13 x
+// 32) have no such unit wider than 32 channels: five 32-channel units per 160-column tile, i.e. five TMA boxes per
+// plane and stage instead of one or two (correct, its cost not measured separately).
+static void wgrad_units(int cpad, int* ubn, int* upt) {
+  static const int kWidths[3] = {256, 192, 160};
+  for (int u = 1; u <= 8; ++u)
+    for (int bn : kWidths)
+      if (bn % u == 0 && (bn / u) % 32 == 0 && cpad % (bn / u) == 0) { *ubn = bn / u; *upt = u; return; }
+  *ubn = 32; *upt = 8;
+}
 
 int cell_wgrad_mn(const void* dg_planes, const void* xh_planes, float* dwp, long long NS, int H, int W,
                   int cpad, int P, cudaStream_t stream) {
   MVB_REQUIRE(P == kBf16Planes, "cell_wgrad_mn: planes P=%d must be 2 (the bf16x2 format)", P);
   MVB_REQUIRE(dg_planes && xh_planes && dwp && NS > 0, "cell_wgrad_mn: bad args");
-  MVB_REQUIRE(cpad == 288 || cpad == 320, "cell_wgrad_mn: cpad=%d unsupported", cpad);
+  MVB_REQUIRE(valid_gemm_cpad(cpad), "cell_wgrad_mn: cpad=%d must be a multiple of 32 from 288 to 512", cpad);
   const Grid g = make_grid(H, W);
   const long long R = NS * g.S;
   GemmParams prm = {};
-  prm.ubn = cpad == 288 ? 96 : 160;
-  prm.upt = cpad == 288 ? 2 : 1;          // pair two 96-wide units: N = 192 keeps the MMA off the smem-bandwidth limit
+  wgrad_units(cpad, &prm.ubn, &prm.upt);
   prm.bn = prm.ubn * prm.upt;
   prm.nb = prm.ubn / 32; prm.n_per_tap = cpad / prm.ubn; prm.n_units = 9 * prm.n_per_tap;
   CUtensorMap tmA, tmB;
@@ -447,7 +474,7 @@ int cell_wgrad_mn(const void* dg_planes, const void* xh_planes, float* dwp, long
   prm.out = dwp; prm.R = R; prm.H = H; prm.W = W; prm.cpad = cpad;
   const long long kb_total = (R + G_BLOCK_K - 1) / G_BLOCK_K;
   // work items = 8 M tiles (128 gate columns) x unit groups x k-splits: cpad 288: 8 x 14 x 5 = 560; cpad 320:
-  // 8 x 18 x 2 = 288
+  // 8 x 18 x 2 = 288; wider x blocks 8 x (18 ... 27) x 8
   prm.ksplit = cell_wgrad_mn_slabs(cpad);
   prm.num_kb = (int)((kb_total + prm.ksplit - 1) / prm.ksplit);
   prm.num_m_tiles = kGates / G_BLOCK_M;
@@ -457,9 +484,11 @@ int cell_wgrad_mn(const void* dg_planes, const void* xh_planes, float* dwp, long
   int sms = 0;
   int rc = num_sms_of_device(&sms);
   if (rc) return rc;
-  // N tile: two 96-wide units (cpad 288) or one 160-wide unit (cpad 320)
-  return prm.bn == 192 ? launch_pgemm<MODE_WGRAD_MN, 192>(tmA, tmB, prm, sms, stream)
-                       : launch_pgemm<MODE_WGRAD_MN, 160>(tmA, tmB, prm, sms, stream);
+  switch (prm.bn) {
+    case 160: return launch_pgemm<MODE_WGRAD_MN, 160>(tmA, tmB, prm, sms, stream);
+    case 192: return launch_pgemm<MODE_WGRAD_MN, 192>(tmA, tmB, prm, sms, stream);
+    default: return launch_pgemm<MODE_WGRAD_MN, 256>(tmA, tmB, prm, sms, stream);
+  }
 }
 
 int lstm_gates_bwd(const float* gates, const float* c_prev, const float* c_new, const float* dh,

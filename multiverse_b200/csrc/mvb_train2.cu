@@ -240,85 +240,87 @@ head_bwd_kernel(const float* __restrict__ h32, const float* __restrict__ dout,
 // ------------------------------------------------------------------------------ emb backward
 // x = tanh(pre), pre = be + conv3x3(in, We);  dpre = dx * (1 - x^2)
 // one CTA per sample row.  ONEHOT (POUT == 1): in = one_hot(id);  else in = dense [HW][POUT] map (POUT = 1: the
-// class decoder's logits feedback, 2: the offset map).
+// class decoder's logits feedback, 2: the offset map).  The channels run in groups of EG whose dpre [HW][EG] fits in
+// shared memory; dbe and dWe of a channel are summed in the same order whatever the grouping, d_in adds the groups'
+// partial sums in channel order.
 template <int POUT, bool ONEHOT = (POUT == 1)>
 __global__ void __launch_bounds__(256)
 emb_bwd_kernel(const float* __restrict__ dxh, int cpad, const int* __restrict__ ids,
                const float* __restrict__ in_map, const float* __restrict__ We,
-               const float* __restrict__ be, int E, float* __restrict__ dWe, float* __restrict__ dbe,
+               const float* __restrict__ be, int E, int EG, float* __restrict__ dWe, float* __restrict__ dbe,
                float* __restrict__ d_in, int accumulate_din, Grid g) {
   extern __shared__ float sm[];
   const int hw = g.H * g.W;
   float* in_s = sm;                      // [HW][POUT] (dense input)
-  float* dpre_s = in_s + hw * 2;         // [HW][E]
-  float* accw = dpre_s + hw * E;         // [9][POUT][E]
-  float* accb = accw + 9 * POUT * E;     // [E]
+  float* dpre_s = in_s + hw * 2;         // [HW][eg]: the current channel group [e0, e0 + eg)
   const long long s = blockIdx.x;
   const int amax = ONEHOT ? ids[s] : 0;
   const int ay = amax / g.W, ax = amax % g.W;
   if (!ONEHOT)
     for (int i = threadIdx.x; i < hw * POUT; i += blockDim.x) in_s[i] = in_map[s * hw * POUT + i];
-  for (int i = threadIdx.x; i < 9 * POUT * E + E; i += blockDim.x) accw[i] = 0.f;
-  __syncthreads();
-  // pass 1: dpre for every (pixel, e)
-  for (int i = threadIdx.x; i < hw * E; i += blockDim.x) {
-    const int p = i / E, e = i % E;
-    const int y = p / g.W, x = p % g.W;
-    float pre = be[e];
-    if (ONEHOT) {
-      const int dy = ay - y, dx = ax - x;
-      if (dy >= -1 && dy <= 1 && dx >= -1 && dx <= 1) pre += We[((dy + 1) * 3 + (dx + 1)) * E + e];
-    } else {
+  for (int e0 = 0; e0 < E; e0 += EG) {
+    const int eg = E - e0 < EG ? E - e0 : EG;
+    __syncthreads();                     // in_s is loaded / the previous group's dpre has been read
+    // pass 1: dpre for every (pixel, e)
+    for (int i = threadIdx.x; i < hw * eg; i += blockDim.x) {
+      const int p = i / eg, e = e0 + i % eg;
+      const int y = p / g.W, x = p % g.W;
+      float pre = be[e];
+      if (ONEHOT) {
+        const int dy = ay - y, dx = ax - x;
+        if (dy >= -1 && dy <= 1 && dx >= -1 && dx <= 1) pre += We[((dy + 1) * 3 + (dx + 1)) * E + e];
+      } else {
 #pragma unroll
-      for (int t = 0; t < 9; ++t) {
-        const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
-        if (yy < 0 || yy >= g.H || xx < 0 || xx >= g.W) continue;
+        for (int t = 0; t < 9; ++t) {
+          const int yy = y + t / 3 - 1, xx = x + t % 3 - 1;
+          if (yy < 0 || yy >= g.H || xx < 0 || xx >= g.W) continue;
 #pragma unroll
-        for (int ci = 0; ci < POUT; ++ci) pre = fmaf(in_s[(yy * g.W + xx) * POUT + ci], We[(t * POUT + ci) * E + e], pre);
+          for (int ci = 0; ci < POUT; ++ci) pre = fmaf(in_s[(yy * g.W + xx) * POUT + ci], We[(t * POUT + ci) * E + e], pre);
+        }
       }
+      const float xv = tanhf(pre);
+      const long long row = s * g.S + (long long)y * g.Wp + x;
+      dpre_s[i] = dxh[row * cpad + e] * (1.f - xv * xv);
     }
-    const float xv = tanhf(pre);
-    const long long row = s * g.S + (long long)y * g.Wp + x;
-    dpre_s[i] = dxh[row * cpad + e] * (1.f - xv * xv);
-  }
-  __syncthreads();
-  // pass 2: dbe, dWe (thread per (tap, po, e)), d_in (thread per (pixel, po))
-  for (int i = threadIdx.x; i < E; i += blockDim.x) {
-    float a = 0.f;
-    for (int p = 0; p < hw; ++p) a += dpre_s[p * E + i];
-    atomicAdd(dbe + i, a);
-  }
-  for (int i = threadIdx.x; i < 9 * POUT * E; i += blockDim.x) {
-    const int e = i % E, po = (i / E) % POUT, t = i / (E * POUT);
-    float a = 0.f;
-    if (ONEHOT) {
-      // out[p] += onehot[p + off(t)] * We[t]  ->  only p = amax - off(t)
-      const int y = ay - (t / 3 - 1), x = ax - (t % 3 - 1);
-      if (y >= 0 && y < g.H && x >= 0 && x < g.W) a = dpre_s[(y * g.W + x) * E + e];
-    } else {
-      for (int p = 0; p < hw; ++p) {
-        const int yy = p / g.W + t / 3 - 1, xx = p % g.W + t % 3 - 1;
-        if (yy < 0 || yy >= g.H || xx < 0 || xx >= g.W) continue;
-        a = fmaf(in_s[(yy * g.W + xx) * POUT + po], dpre_s[p * E + e], a);
-      }
-    }
-    atomicAdd(dWe + (t * POUT + po) * E + e, a);
-  }
-  if (!ONEHOT && d_in) {
-    for (int i = threadIdx.x; i < hw * POUT; i += blockDim.x) {
-      const int q = i / POUT, po = i % POUT;
-      const int y = q / g.W, x = q % g.W;
+    __syncthreads();
+    // pass 2: dbe, dWe (thread per (tap, po, e)), d_in (thread per (pixel, po))
+    for (int i = threadIdx.x; i < eg; i += blockDim.x) {
       float a = 0.f;
-#pragma unroll
-      for (int t = 0; t < 9; ++t) {
-        const int py = y - (t / 3 - 1), px = x - (t % 3 - 1);   // out[p] uses in[p + off] -> p = q - off
-        if (py < 0 || py >= g.H || px < 0 || px >= g.W) continue;
-        const float* dp = dpre_s + (py * g.W + px) * E;
-        const float* wv = We + (t * POUT + po) * E;
-        for (int e = 0; e < E; ++e) a = fmaf(dp[e], wv[e], a);
+      for (int p = 0; p < hw; ++p) a += dpre_s[p * eg + i];
+      atomicAdd(dbe + e0 + i, a);
+    }
+    for (int i = threadIdx.x; i < 9 * POUT * eg; i += blockDim.x) {
+      const int el = i % eg, po = (i / eg) % POUT, t = i / (eg * POUT);
+      float a = 0.f;
+      if (ONEHOT) {
+        // out[p] += onehot[p + off(t)] * We[t]  ->  only p = amax - off(t)
+        const int y = ay - (t / 3 - 1), x = ax - (t % 3 - 1);
+        if (y >= 0 && y < g.H && x >= 0 && x < g.W) a = dpre_s[(y * g.W + x) * eg + el];
+      } else {
+        for (int p = 0; p < hw; ++p) {
+          const int yy = p / g.W + t / 3 - 1, xx = p % g.W + t % 3 - 1;
+          if (yy < 0 || yy >= g.H || xx < 0 || xx >= g.W) continue;
+          a = fmaf(in_s[(yy * g.W + xx) * POUT + po], dpre_s[p * eg + el], a);
+        }
       }
-      const long long o = s * hw * POUT + i;
-      d_in[o] = accumulate_din ? d_in[o] + a : a;
+      atomicAdd(dWe + (t * POUT + po) * E + e0 + el, a);
+    }
+    if (!ONEHOT && d_in) {
+      for (int i = threadIdx.x; i < hw * POUT; i += blockDim.x) {
+        const int q = i / POUT, po = i % POUT;
+        const int y = q / g.W, x = q % g.W;
+        float a = 0.f;
+#pragma unroll
+        for (int t = 0; t < 9; ++t) {
+          const int py = y - (t / 3 - 1), px = x - (t % 3 - 1);   // out[p] uses in[p + off] -> p = q - off
+          if (py < 0 || py >= g.H || px < 0 || px >= g.W) continue;
+          const float* dp = dpre_s + (py * g.W + px) * eg;
+          const float* wv = We + (t * POUT + po) * E + e0;
+          for (int e = 0; e < eg; ++e) a = fmaf(dp[e], wv[e], a);
+        }
+        const long long o = s * hw * POUT + i;
+        d_in[o] = (accumulate_din || e0 > 0) ? d_in[o] + a : a;
+      }
     }
   }
 }
@@ -711,15 +713,20 @@ int emb_bwd(const float* dxh, int cpad, const int* ids, const float* in_map, con
   MVB_REQUIRE((Pout == 1 && (ids || in_map)) || (Pout == 2 && in_map),
               "emb_bwd: need ids or in_map (Pout=1) or in_map (Pout=2)");
   const Grid g = make_grid(H, W);
-  const size_t smem = sizeof(float) * ((size_t)H * W * (2 + E) + 9 * Pout * E + E);
+  // channel group: all E channels where [HW][2 + E] floats fit, else the widest multiple of 8 that does
+  constexpr size_t kSmemMax = 160 * 1024;
+  const size_t hw = (size_t)H * W;
+  const long long fit = (long long)(kSmemMax / sizeof(float) / hw) - 2;
+  const int EG = fit >= E ? E : (int)(fit / 8 * 8);
+  MVB_REQUIRE(EG >= 8, "emb_bwd: grid %dx%d too large", H, W);
+  const size_t smem = sizeof(float) * hw * (2 + EG);
   static SmemOptIn opt1, opt1d, opt2;
-  MVB_CHECK_CUDA(smem_opt_in(opt1, emb_bwd_kernel<1>, 160 * 1024));
-  MVB_CHECK_CUDA(smem_opt_in(opt1d, emb_bwd_kernel<1, false>, 160 * 1024));
-  MVB_CHECK_CUDA(smem_opt_in(opt2, emb_bwd_kernel<2>, 160 * 1024));
-  MVB_REQUIRE(smem <= 160 * 1024, "emb_bwd: grid too large");
-  if (Pout == 1 && ids) emb_bwd_kernel<1><<<(unsigned)NS, 256, smem, stream>>>(dxh, cpad, ids, in_map, We, be, E, dWe, dbe, d_in, accumulate_din, g);
-  else if (Pout == 1) emb_bwd_kernel<1, false><<<(unsigned)NS, 256, smem, stream>>>(dxh, cpad, ids, in_map, We, be, E, dWe, dbe, d_in, accumulate_din, g);
-  else emb_bwd_kernel<2><<<(unsigned)NS, 256, smem, stream>>>(dxh, cpad, ids, in_map, We, be, E, dWe, dbe, d_in, accumulate_din, g);
+  MVB_CHECK_CUDA(smem_opt_in(opt1, emb_bwd_kernel<1>, kSmemMax));
+  MVB_CHECK_CUDA(smem_opt_in(opt1d, emb_bwd_kernel<1, false>, kSmemMax));
+  MVB_CHECK_CUDA(smem_opt_in(opt2, emb_bwd_kernel<2>, kSmemMax));
+  if (Pout == 1 && ids) emb_bwd_kernel<1><<<(unsigned)NS, 256, smem, stream>>>(dxh, cpad, ids, in_map, We, be, E, EG, dWe, dbe, d_in, accumulate_din, g);
+  else if (Pout == 1) emb_bwd_kernel<1, false><<<(unsigned)NS, 256, smem, stream>>>(dxh, cpad, ids, in_map, We, be, E, EG, dWe, dbe, d_in, accumulate_din, g);
+  else emb_bwd_kernel<2><<<(unsigned)NS, 256, smem, stream>>>(dxh, cpad, ids, in_map, We, be, E, EG, dWe, dbe, d_in, accumulate_din, g);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;

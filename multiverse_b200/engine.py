@@ -67,7 +67,7 @@ class ScaleWeights(object):
     # inference: class encoder with its one-cell scene-feature input added from per-sample table rows in the epilogue
     # (ops.cell_fwd_xsparse) instead of a K chunk of the GEMM
     self.enc_class_xs = None
-    if fast and weights[nm["enc_class"][0]].shape[2] == 64 + ops.HIDDEN:
+    if fast and scene_enc and weights[nm["enc_class"][0]].shape[2] == 64 + ops.HIDDEN:
       self.enc_class_xs = ops.XSparse(f(nm["enc_class"][0]))
     self.enc_reg_fast = self.enc_reg_xd = None
     if fast and weights[nm["enc_reg"][0]].shape[2] == 2 + ops.HIDDEN:
@@ -121,7 +121,6 @@ class ConvRNNEngine(object):
     assert cfg.enc_hidden_size == ops.HIDDEN and cfg.dec_hidden_size == ops.HIDDEN, \
         "the kernels are specialised for hidden size 256 (every published config)"
     assert cfg.convlstm_kernel == 3 and cfg.scene_conv_kernel == 3
-    assert cfg.use_scene_enc or cfg.emb_size == 32, "without use_scene_enc the class encoder's input is emb_size 32"
     assert cfg.scene_conv_dim == 64
     assert getattr(cfg, "activation_func", "tanh") in ("tanh",) or \
         getattr(cfg.activation_func, "__name__", "") == "tanh", "kernels implement tanh"

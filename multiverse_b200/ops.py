@@ -71,8 +71,8 @@ class PackedCell(object):
     assert kernel.dim() == 4 and kernel.shape[0] == 3 and kernel.shape[1] == 3
     assert kernel.shape[3] == 4 * HIDDEN
     self.cx = int(kernel.shape[2]) - HIDDEN
-    self.cxp = (self.cx + 31) // 32 * 32
-    self.cpad = self.cxp + HIDDEN
+    self.cpad = cell_cpad(self.cx)
+    self.cxp = self.cpad - HIDDEN
     self.planes = planes
     self.comp = bool(comp) and planes == PLANES_BF16X2 and 4 * self.cx <= self.cxp
     kernel = kernel.detach().to(torch.float32).contiguous()
@@ -124,12 +124,14 @@ def operand_values(xh):
   n = r * cpad
   a0 = raw[:2 * n].view(torch.float16).reshape(r, cpad).float()
   f8 = raw[2 * n:].view(torch.float8_e4m3fn).reshape(r, 2 * cpad).float()
-  # inside an fp8 row: [x block: e0 (cxp) | e1 (cxp)], then per 64 channels of the h block [e0 (64) | e1 (64)]
+  # inside an fp8 row, per 64-channel chunk of the x block [e0 (64) | e1 (64)] (a trailing 32-channel chunk:
+  # [e0 (32) | e1 (32)]), then per 64 channels of the h block [e0 (64) | e1 (64)] (mvb_common.cuh f8_off)
   cxp = cpad - HIDDEN
   c = torch.arange(cpad, device=xh.device)
-  cc = (c - cxp).clamp(min=0)
-  off0 = torch.where(c >= cxp, 2 * cxp + (cc // 64) * 128 + cc % 64, c)
-  off1 = torch.where(c >= cxp, off0 + 64, c + cxp)
+  c0 = torch.where(c >= cxp, cxp + (c - cxp) // 64 * 64, c // 64 * 64)     # first channel of c's chunk
+  width = torch.where(c >= cxp, 64, (cxp - c0).clamp(max=64))
+  off0 = 2 * c0 + (c - c0)
+  off1 = off0 + width
   return a0 + f8[:, off1] / 4096.0, f8[:, off0]
 
 

@@ -658,6 +658,9 @@ def _engine_config(config):
           "use_gnn use_beam_search beam_size diverse_beam diverse_gamma fix_num_timestep "
           "pred_len").split()
   d = {k: getattr(config, k) for k in keys}
+  if not (d["emb_size"] % 8 == 0 and 8 <= d["emb_size"] <= 256):
+    raise NotImplementedError("--emb_size %r: the kernels take a multiple of 8 from 8 to 256 (the reference's default "
+                              "is 128, the published commands pass 32)" % (d["emb_size"],))
   d["obs_len"] = getattr(config, "obs_len", None)    # multifuture_inference.py's Namespace has none (:419-452)
   d["activation_func"] = "tanh"
   for k, default in (("grid_loss_weight", 1.0), ("grid_reg_loss_weight", 0.1), ("wd", 0.0),
