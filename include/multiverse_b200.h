@@ -95,12 +95,15 @@ int mvb_convlstm_cell_fwd(const void* xh_planes, const void* w_planes, const flo
  * gate pre-activations is exactly two table rows per cell (mvb_cell_xfold_tables): the x chunks of
  * the K loop are skipped (1/9 of the MMAs) and the x block of xh_planes is never read.
  *   table_B  fp32 [9][1024]      (border class of the cell; biases folded in)
- *   table_T2 fp32 [9][25][1024]  (border class of ids[s]; 5x5 offset of the cell to ids[s]) */
+ *   table_T2 fp32 [9][25][1024]  (border class of ids[s]; 5x5 offset of the cell to ids[s])
+ * tiles / tile_count (or NULL: every row): a work list from mvb_beam_band, int32 [*tile_count][2] (m0, m_end) of
+ * GEMM rows; only the rows [m0, m_end) of its entries are computed and written. */
 int mvb_cell_xfold_tables(const float* kernel, const float* biases, const float* We, const float* be,
                           int E, float* table_B, float* table_T2, void* stream);
 int mvb_convlstm_cell_fwd_onehot(const void* xh_planes, const void* w_planes, const float* table_B,
                                  const float* table_T2, const int32_t* ids, const float* c_in,
-                                 const int32_t* row_map, float* c_out, float* h32_out, void* hp_out,
+                                 const int32_t* row_map, const int32_t* tiles, const int32_t* tile_count,
+                                 float* c_out, float* h32_out, void* hp_out,
                                  int64_t hp_plane_stride, int cpad_out, int ch_off_out, int64_t NS, int H,
                                  int W, int cpad, int planes, float forget_bias, void* stream);
 /* The cell of the regression encoder (code/pred_models.py:196-202, :232-234), whose 2-channel input holds raw pixel
@@ -136,6 +139,8 @@ int mvb_cell_xsparse_table(const float* scene_conv, const int32_t* frame_idx, co
  * NS sample rows; its raw accumulators go to `workspace`, fp32 [NS*S, 1024], caller-allocated) and a second,
  * HBM-bound kernel emits the K children (c_out, h32_out: NS*K sample rows, child-major within a sample): 1/K of the
  * MMAs, identical values. */
+/* xh_planes NULL: `workspace` already holds the accumulators of these parent rows (an earlier call on the same
+ * operands and weights): the GEMM is skipped and only the children are emitted (fanout >= 1). */
 int mvb_convlstm_cell_fwd_onehot_fanout(const void* xh_planes, const void* w_planes, const float* table_B,
                                         const float* table_T2, const int32_t* ids, const float* c_in,
                                         float* c_out, float* h32_out, float* workspace, int64_t NS, int fanout,
@@ -370,6 +375,22 @@ int mvb_beam_backtrace(const int32_t* step_ids, const int32_t* step_parents,
  * channel padding and halo rows are not written. */
 int mvb_beam_gather_h_f16f8(const float* h32, const int32_t* row_map, void* hp_out, int64_t hp_plane_stride,
                             int cpad_out, int64_t NS, int H, int W, void* stream);
+
+/* Image-row bands of the beam decoder (DESIGN.md 3.2).  Beam k's c and h equal those of its sample's base rollout
+ * (the same recurrence fed the no-selection input; ids outside the grid, e.g. (H+3)*W) outside the rows
+ *   band[k] = clamp(widen(band_in[parent(k)], radius) U [y(ids[k]) - 2, y(ids[k]) + 2])
+ * (radius 2 with the graph attention, 1 without; band_in NULL at the fan-out: no parent band).  ids, parents int32
+ * [NS] (NS = N*K; parents within the sample, as mvb_beam_step writes them), bands int32 [NS][2] (first, last row).
+ * Also writes the work list of the step's cell launch (mvb_convlstm_cell_fwd_onehot): int32 (m0, m_end) pairs of
+ * 128-row M tiles over the bands' GEMM rows, tiles_cap >= NS * (ceil((H+1)(W+1) / 128) + 1) of them, and their
+ * count.  Everything stays on the device. */
+int mvb_beam_band(const int32_t* ids, const int32_t* parents, const int32_t* band_in, int32_t* band_out,
+                  int32_t* tiles, int64_t tiles_cap, int32_t* tile_count, int64_t NS, int K, int radius, int H, int W,
+                  void* stream);
+/* c, h32 fp32 [NS*(H+1)*(W+1), 256] halo: the valid rows of beam k outside band[k] <- rows of sample k / K of the
+ * base rollout's base_c, base_h32 ([N*(H+1)*(W+1), 256]).  The rows inside the bands are not touched. */
+int mvb_beam_band_copy(const float* base_c, const float* base_h32, const int32_t* band, float* c, float* h32,
+                       int64_t NS, int K, int H, int W, void* stream);
 
 /* ---- f-1 (next row): feed generation on the device (multifuture_inference.py:115-156, preprocess.py:436-475):
  *      traj fp64 [NT,2] frame pixels, centers fp64 [H*W,2] (the caller's scene_grid_centers) ->

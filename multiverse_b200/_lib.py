@@ -34,7 +34,7 @@ SIGNATURES = {
     "mvb_cell_xsparse_weights": [_vp, _i, _vp, _vp],
     "mvb_cell_xsparse_table": [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp],
     "mvb_convlstm_cell_fwd_onehot_fanout": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _f, _vp],
-    "mvb_convlstm_cell_fwd_onehot": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i64,
+    "mvb_convlstm_cell_fwd_onehot": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i64,
                                      _i, _i, _i, _i, _f, _vp],
     "mvb_convlstm_cell_fwd_train": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _vp, _i64, _i, _i,
                                     _i, _i, _f, _vp],
@@ -80,6 +80,8 @@ SIGNATURES = {
     "mvb_beam_nll": [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _vp],
     "mvb_beam_backtrace": [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],
     "mvb_beam_gather_h_f16f8": [_vp, _vp, _vp, _i64, _i, _i64, _i, _i, _vp],
+    "mvb_beam_band": [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _vp],
+    "mvb_beam_band_copy": [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],
 }
 _RESTYPES = {"mvb_last_error": C.c_char_p, "mvb_launch_count": C.c_longlong, "mvb_cell_variants_seen": C.c_longlong,
              "mvb_reset_launch_count": None}

@@ -121,7 +121,7 @@ static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s)
 extern "C" {
 
 const char* mvb_last_error(void) { return get_error(); }
-int mvb_abi_version(void) { return 14; }
+int mvb_abi_version(void) { return 15; }
 int mvb_cell_last_variant(void) { return cell_last_variant(); }
 long long mvb_cell_variants_seen(int reset) { return (long long)cell_variants_seen(reset); }
 long long mvb_launch_count(void) { return g_launches; }
@@ -151,14 +151,15 @@ int mvb_cell_xfold_tables(const float* kernel, const float* biases, const float*
 }
 int mvb_convlstm_cell_fwd_onehot(const void* xh_planes, const void* w_planes, const float* table_B,
                                  const float* table_T2, const int32_t* ids, const float* c_in,
-                                 const int32_t* row_map, float* c_out, float* h32_out, void* hp_out,
+                                 const int32_t* row_map, const int32_t* tiles, const int32_t* tile_count,
+                                 float* c_out, float* h32_out, void* hp_out,
                                  int64_t hp_plane_stride, int cpad_out, int ch_off_out, int64_t NS, int H,
                                  int W, int cpad, int planes, float forget_bias, void* stream) {
   CellStep s{};
   s.xh = xh_planes; s.w = w_planes; s.xf_B = table_B; s.xf_T2 = table_T2; s.xf_ids = ids; s.c_in = c_in;
   s.row_map = row_map; s.c_out = c_out; s.h32_out = h32_out; s.hp_out = hp_out; s.hp_plane_stride = hp_plane_stride;
   s.cpad_out = cpad_out; s.ch_off_out = ch_off_out; s.NS = NS; s.H = H; s.W = W; s.cpad = cpad; s.planes = planes;
-  s.forget_bias = forget_bias;
+  s.forget_bias = forget_bias; s.tiles = tiles; s.tile_count = tile_count;
   return cell_fwd(s, S(stream));
 }
 int mvb_convlstm_cell_fwd_xdense(const void* xh_planes, const void* w_planes, const float* bias_packed,
@@ -415,6 +416,15 @@ int mvb_beam_backtrace(const int32_t* step_ids, const int32_t* step_parents,
 int mvb_beam_gather_h_f16f8(const float* h32, const int32_t* row_map, void* hp_out, int64_t hp_plane_stride,
                             int cpad_out, int64_t NS, int H, int W, void* stream) {
   return beam_gather_h(h32, row_map, hp_out, hp_plane_stride, cpad_out, NS, H, W, S(stream));
+}
+int mvb_beam_band(const int32_t* ids, const int32_t* parents, const int32_t* band_in, int32_t* band_out,
+                  int32_t* tiles, int64_t tiles_cap, int32_t* tile_count, int64_t NS, int K, int radius, int H, int W,
+                  void* stream) {
+  return beam_band(ids, parents, band_in, band_out, tiles, tiles_cap, tile_count, NS, K, radius, H, W, S(stream));
+}
+int mvb_beam_band_copy(const float* base_c, const float* base_h32, const int32_t* band, float* c, float* h32,
+                       int64_t NS, int K, int H, int W, void* stream) {
+  return beam_band_copy(base_c, base_h32, band, c, h32, NS, K, H, W, S(stream));
 }
 
 }  // extern "C"

@@ -321,6 +321,163 @@ int beam_gather_h(const float* h32, const int* row_map, void* hp_out, long long 
   return MVB_OK;
 }
 
+// ----------------------------------------------------------------------------------
+// Image-row bands of the beam decoder.  A beam's state differs from that of its sample's base rollout (the same
+// recurrence fed the no-selection input tanh(b) at every step) only near the cells its ancestry selected: the folded
+// one-hot input changes the pre-activations of the 5x5 cells around the selected cell, and each later step spreads
+// a difference by `radius` image rows (the 3x3 convolution, plus the 3x3 graph attention when it runs).  So
+//   band[k] = clamp(widen(band[parent(k)], radius) U [y(id_k) - 2, y(id_k) + 2])
+// and outside its band beam k's c and h are bit for bit the base's.  From the bands, the work list of the step's
+// beam cell launch: 128-row M tiles (m0, m_end) covering GEMM rows [lo (W+1), (hi+1) (W+1)) of every beam.  Bands
+// that meet across a sample boundary (one ends on the last image row, the next starts on the first: only the halo
+// row between them) form one run of rows, tiled as one, so full bands give the launch's own tiling.
+// One CTA: three block-wide scans over the beams (run start, run end, tile offset).
+// ----------------------------------------------------------------------------------
+constexpr int BAND_THREADS = 1024;
+
+static long long beam_band_capacity(long long NS, int H, int W) {
+  const Grid g = make_grid(H, W);
+  return NS * ((g.S + 127) / 128 + 1);     // tiles of a beam's own rows: at most one more than its span needs
+}
+
+// exclusive scan of v over the block's threads in the order of `slot`, with an associative op and its identity
+template <class Op>
+__device__ long long block_scan_excl(long long v, long long identity, int slot, long long* sh, Op op) {
+  long long x = v;
+  sh[slot] = x;
+  __syncthreads();
+  for (int o = 1; o < BAND_THREADS; o <<= 1) {
+    const long long u = slot >= o ? sh[slot - o] : identity;
+    __syncthreads();
+    x = op(u, x);
+    sh[slot] = x;
+    __syncthreads();
+  }
+  const long long r = slot ? sh[slot - 1] : identity;
+  __syncthreads();
+  return r;
+}
+
+__global__ void __launch_bounds__(BAND_THREADS)
+beam_band_kernel(const int* __restrict__ ids, const int* __restrict__ parents, const int* __restrict__ band_in,
+                 int* band_out, int* __restrict__ tiles, int* __restrict__ tile_count, int NS, int K, int radius,
+                 Grid g) {
+  __shared__ long long sh[BAND_THREADS];
+  const int t = threadIdx.x;
+  const int per = (NS + BAND_THREADS - 1) / BAND_THREADS;
+  const int k0 = min(NS, t * per), k1 = min(NS, k0 + per);
+  for (int k = k0; k < k1; ++k) {
+    const int y = ids[k] / g.W;
+    int lo = y - 2, hi = y + 2;
+    if (band_in) {
+      const int p = k - k % K + parents[k];
+      lo = min(lo, band_in[2 * p] - radius);
+      hi = max(hi, band_in[2 * p + 1] + radius);
+    }
+    band_out[2 * k] = max(lo, 0);
+    band_out[2 * k + 1] = min(hi, g.H - 1);
+  }
+  __syncthreads();      // every band is visible to the block
+  // beam k: GEMM rows [s_k, e_k) (through the trailing halo row when the band ends on the last image row); it
+  // continues the run of beam k - 1 when that one ends there and this one starts on the first image row
+  auto rows = [&](int k, long long& s, long long& e) {
+    const int lo = band_out[2 * k], hi = band_out[2 * k + 1];
+    s = (long long)k * g.S + (long long)lo * g.Wp;
+    e = hi == g.H - 1 ? (long long)(k + 1) * g.S : (long long)k * g.S + (long long)(hi + 1) * g.Wp;
+  };
+  auto continues = [&](int k) { return k > 0 && k < NS && band_out[2 * k] == 0 && band_out[2 * k - 1] == g.H - 1; };
+  auto lmax = [](long long a, long long b) { return a > b ? a : b; };
+  auto lmin = [](long long a, long long b) { return a < b ? a : b; };
+  auto lsum = [](long long a, long long b) { return a + b; };
+  // first row of each beam's run: max-scan of the run starts
+  long long agg = -1, s, e;
+  for (int k = k0; k < k1; ++k) if (!continues(k)) { rows(k, s, e); agg = s; }
+  const long long start_in = block_scan_excl(agg, -1LL, t, sh, lmax);
+  // end row of each beam's run: reverse min-scan of the first run end in each thread's beams
+  const long long kInf = 0x7fffffffffffffffLL;
+  agg = kInf;
+  for (int k = k0; k < k1; ++k) if (!continues(k + 1)) { rows(k, s, e); agg = e; break; }
+  const long long end_in = block_scan_excl(agg, kInf, BAND_THREADS - 1 - t, sh, lmin);
+  // a run's tiles start at its first row every 128 rows; beam k owns those whose m0 lies in [s_k, e_k)
+  auto own = [](long long s, long long e, long long rs, long long& j0, long long& j1) {
+    j0 = (s - rs + kCellTileRows - 1) / kCellTileRows; j1 = (e - rs + kCellTileRows - 1) / kCellTileRows;
+  };
+  long long rs = start_in, n = 0, j0, j1;
+  for (int k = k0; k < k1; ++k) {
+    rows(k, s, e);
+    if (!continues(k)) rs = s;
+    own(s, e, rs, j0, j1);
+    n += j1 - j0;
+  }
+  long long o = block_scan_excl(n, 0LL, t, sh, lsum);
+  if (t == BAND_THREADS - 1) *tile_count = (int)(o + n);
+  long long re = 0;
+  rs = start_in;
+  for (int k = k0; k < k1; ++k) {
+    rows(k, s, e);
+    if (!continues(k)) rs = s;
+    if (k == k0 || !continues(k)) {      // the last row of the run beam k belongs to
+      int j = k;
+      while (j + 1 < k1 && continues(j + 1)) ++j;
+      long long sj, ej;
+      rows(j, sj, ej);
+      re = (j + 1 == k1 && continues(k1)) ? end_in : ej;
+    }
+    own(s, e, rs, j0, j1);
+    for (long long j = j0; j < j1; ++j, ++o) {
+      const long long m0 = rs + j * kCellTileRows;
+      tiles[2 * o] = (int)m0;
+      tiles[2 * o + 1] = (int)lmin(m0 + kCellTileRows, re);
+    }
+  }
+}
+
+int beam_band(const int* ids, const int* parents, const int* band_in, int* band_out, int* tiles, long long tiles_cap,
+              int* tile_count, long long NS, int K, int radius, int H, int W, cudaStream_t stream) {
+  MVB_REQUIRE(ids && band_out && tiles && tile_count && (!band_in || parents), "beam_band: null pointer");
+  MVB_REQUIRE(band_in != band_out, "beam_band: the parents' bands and the new ones need separate buffers");
+  MVB_REQUIRE(NS > 0 && K > 0 && NS % K == 0 && H > 0 && W > 0 && radius >= 0,
+              "beam_band: bad sizes NS=%lld K=%d H=%d W=%d radius=%d", NS, K, H, W, radius);
+  const Grid g = make_grid(H, W);
+  MVB_REQUIRE(NS * g.S + kCellTileRows < 0x7fffffffLL, "beam_band: NS=%lld too large for int32 rows", NS);
+  MVB_REQUIRE(tiles_cap >= beam_band_capacity(NS, H, W), "beam_band: %lld tile entries, %lld needed", tiles_cap,
+              beam_band_capacity(NS, H, W));
+  beam_band_kernel<<<1, BAND_THREADS, 0, stream>>>(ids, parents, band_in, band_out, tiles, tile_count, (int)NS, K,
+                                                   radius, g);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
+// c and h32 of the base rollout (sample k / K) into the valid rows of beam k outside its band: one CTA per (beam,
+// image row), the row's W cells contiguous in both layouts.  The cell launch on the work list writes the other rows.
+__global__ void __launch_bounds__(256)
+beam_band_copy_kernel(const float4* __restrict__ base_c, const float4* __restrict__ base_h, const int* __restrict__ band,
+                      float4* __restrict__ c, float4* __restrict__ h, int K, Grid g) {
+  const long long k = blockIdx.x / g.H;
+  const int y = (int)(blockIdx.x - k * g.H);
+  if (y >= band[2 * k] && y <= band[2 * k + 1]) return;
+  constexpr int V = kHidden / 4;      // float4 per row
+  const long long src = ((k / K) * g.S + (long long)y * g.Wp) * V, dst = (k * g.S + (long long)y * g.Wp) * V;
+  for (int i = threadIdx.x; i < g.W * V; i += blockDim.x) {
+    c[dst + i] = __ldg(base_c + src + i);
+    h[dst + i] = __ldg(base_h + src + i);
+  }
+}
+
+int beam_band_copy(const float* base_c, const float* base_h32, const int* band, float* c, float* h32, long long NS,
+                   int K, int H, int W, cudaStream_t stream) {
+  MVB_REQUIRE(base_c && base_h32 && band && c && h32, "beam_band_copy: null pointer");
+  MVB_REQUIRE(NS > 0 && K > 0 && NS % K == 0 && H > 0 && W > 0 && NS * H < (1ll << 31),
+              "beam_band_copy: bad sizes NS=%lld K=%d H=%d W=%d", NS, K, H, W);
+  beam_band_copy_kernel<<<(unsigned)(NS * H), 256, 0, stream>>>(
+      reinterpret_cast<const float4*>(base_c), reinterpret_cast<const float4*>(base_h32), band,
+      reinterpret_cast<float4*>(c), reinterpret_cast<float4*>(h32), K, make_grid(H, W));
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
 int beam_backtrace(const int* step_ids, const int* step_parents, const float* step_logits,
                    int* out_ids, float* out_logits, long long N, int B, int Tp, int V,
                    cudaStream_t stream) {

@@ -29,7 +29,7 @@
 
 namespace mvb {
 
-constexpr int BLOCK_M = 128;
+constexpr int BLOCK_M = kCellTileRows;
 constexpr int BLOCK_N = 256;
 constexpr int XPAD = 32;      // the x block is zero-padded to a multiple of 32 channels (cpad = roundup(cx,32) + 256)
 constexpr int kMaxXBlock = 256;   // widest x block of the GEMM: four 64-channel chunks (emb_size up to 256)
@@ -141,6 +141,10 @@ struct CellParams {
   int cpad_out;             // row pitch of hp_out (elements)
   int ch_off_out;           // channel offset of the h block inside hp_out rows
   long long R;              // total halo rows
+  // work list (beam decoder, mvb_beam_band): M tiles (m0, m_end) pairs [*tile_count][2], or nullptr (the launch's
+  // 128-row blocks in order); a tile's stores are clipped to [m0, m_end)
+  const int* tiles;
+  const int* tile_count;
   int H, W;
   int cpad;                 // K channels per tap (multiple of 32)
   float forget_bias;
@@ -172,10 +176,10 @@ struct EpiRow {
   const float* xft;     // x-fold / sparse-x table row of this cell for its sample row, else nullptr
 };
 
-__device__ __forceinline__ EpiRow epi_row(const CellParams& prm, const Grid& g, long long row) {
+__device__ __forceinline__ EpiRow epi_row(const CellParams& prm, const Grid& g, long long row, long long m_end) {
   EpiRow r;
   r.row = row; r.src_row = row; r.psmp = 0; r.py = 0; r.px = 0; r.xfb = nullptr; r.xft = nullptr;
-  r.valid = row < prm.R;
+  r.valid = row < m_end;
   if (!r.valid) return r;
   const long long smp = row / g.S;
   const int rem = (int)(row - smp * g.S);
@@ -205,6 +209,18 @@ __device__ __forceinline__ EpiRow epi_row(const CellParams& prm, const Grid& g, 
     }
   }
   return r;
+}
+
+// M tiles of a launch, and the rows [m0, m_end) that tile i computes and stores: the launch's 128-row blocks in order,
+// or entry i of the work list.  An index past the list (rank 1 of a pair on an odd count) stores nothing.
+__device__ __forceinline__ long long m_tile_count(const CellParams& prm) {
+  return prm.tiles ? (long long)__ldg(prm.tile_count) : (prm.R + BLOCK_M - 1) / BLOCK_M;
+}
+__device__ __forceinline__ void m_tile_rows(const CellParams& prm, long long count, long long i, long long& m0,
+                                            long long& m_end) {
+  if (!prm.tiles) { m0 = i * BLOCK_M; m_end = prm.R; }
+  else if (i < count) { m0 = __ldg(prm.tiles + 2 * i); m_end = __ldg(prm.tiles + 2 * i + 1); }
+  else { m0 = 0; m_end = 0; }
 }
 
 // c of the row's channels ch, ch + 1 from the previous step (zero state without c_in).  The epilogue fetches all of
@@ -362,7 +378,7 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   // only their own small sum (~2^-11 of the result); the fp16 MMAs, exact in fp32, then add the main products.
   constexpr int NPASS = FMT ? 2 : 1;
   constexpr int NS = FMT ? 1 : kBf16Planes;    // B slots per (pass, chunk, tap)
-  const long long num_m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
+  const long long num_m_tiles = m_tile_count(prm);
   // work index w -> (m tile, n tile).  MC: the pair shares w; rank r takes m tile 2*(w / N_TILES) + r.
   const uint32_t rank = MC ? cluster_ctarank() : 0u;
   const long long num_tiles = (MC ? (num_m_tiles + 1) / 2 : num_m_tiles) * N_TILES;
@@ -374,7 +390,9 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   auto work_index = [&](long long it) -> long long {
     return prm.order ? (w_begin + (it / N_TILES) * w_step) * N_TILES + it % N_TILES : w_begin + it * w_step;
   };
-  auto tile_m0 = [&](long long w) -> long long { return ((w / N_TILES) * (MC ? 2 : 1) + rank) * BLOCK_M; };
+  auto tile_rows = [&](long long w, long long& m0, long long& m_end) {
+    m_tile_rows(prm, num_m_tiles, (w / N_TILES) * (MC ? 2 : 1) + rank, m0, m_end);
+  };
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA);
@@ -396,7 +414,8 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       int slot = 0, astage = 0; uint32_t phase = 0, aphase = 0;
       CELL_PROBE(const long long probe_t0 = clock64();)
       for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
-        const long long m0 = tile_m0(t);
+        long long m0, m_end;
+        tile_rows(t, m0, m_end);
         const int n0 = (int)(t % N_TILES) * BLOCK_N;
         // chunk-major K order: the x block - whose terms can be orders of magnitude larger than the h terms (raw
         // pixel offsets in the regression encoder) - is accumulated first, so the small h products are never added
@@ -458,7 +477,8 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     CELL_PROBE(const long long probe_t0 = clock64();)
     for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
       CELL_PROBE(++probe[kProbeTiles];)
-      const long long m0 = tile_m0(t);
+      long long m0, m_end;
+      tile_rows(t, m0, m_end);
       const int nt = (int)(t % N_TILES);
       uint32_t fresh = 1;                      // the tile's first MMA overwrites the accumulator
       auto mma16 = [&](uint32_t a_lo, uint32_t b_lo) {
@@ -533,7 +553,7 @@ cell_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       float2 cprev[2][8];
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
-        rows[hr] = epi_row(prm, g, rbase + 8 * hr);
+        rows[hr] = epi_row(prm, g, rbase + 8 * hr, m_end);
 #pragma unroll
         for (int ip = 0; ip < 8; ++ip) cprev[hr][ip] = epi_cprev(prm, rows[hr], nt * TILE_CH + 8 * ip + 2 * (lane & 3));
       }
@@ -667,7 +687,7 @@ cell_fwd_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   const int nqx = (cxp + CHUNK - 1) / CHUNK;   // x chunks, then the four h chunks (as in cell_fwd_kernel)
   const int q_begin = prm.skip_x ? nqx : 0;
   const int NQ = nqx + kHidden / CHUNK;
-  const long long num_m_tiles = (prm.R + BLOCK_M - 1) / BLOCK_M;
+  const long long num_m_tiles = m_tile_count(prm);
   const uint32_t rank = MC ? cluster_ctarank() : 0u;
   const long long num_tiles = (MC ? (num_m_tiles + 1) / 2 : num_m_tiles) * EW_N_TILES;
   const long long w_begin = MC ? (long long)(blockIdx.x >> 1) : (long long)blockIdx.x;
@@ -675,7 +695,9 @@ cell_fwd_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   auto work_index = [&](long long it) -> long long {      // as in cell_fwd_kernel, with eight N tiles per M tile
     return prm.order ? (w_begin + (it / EW_N_TILES) * w_step) * EW_N_TILES + it % EW_N_TILES : w_begin + it * w_step;
   };
-  auto tile_m0 = [&](long long w) -> long long { return ((w / EW_N_TILES) * (MC ? 2 : 1) + rank) * BLOCK_M; };
+  auto tile_rows = [&](long long w, long long& m0, long long& m_end) {
+    m_tile_rows(prm, num_m_tiles, (w / EW_N_TILES) * (MC ? 2 : 1) + rank, m0, m_end);
+  };
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA); prefetch_tmap(&tmB); prefetch_tmap(&tmA8); prefetch_tmap(&tmB8);
@@ -697,7 +719,8 @@ cell_fwd_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       int slot = 0, astage = 0; uint32_t phase = 0, aphase = 0;
       CELL_PROBE(const long long probe_t0 = clock64();)
       for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
-        const long long m0 = tile_m0(t);
+        long long m0, m_end;
+        tile_rows(t, m0, m_end);
         const int nt = (int)(t % EW_N_TILES);
         const int half = nt & 1, tg0 = (nt >> 1) * 4;      // 32-row half and (tile, gate) index of gate 0
         for (int pass = 0; pass < 2; ++pass)
@@ -850,7 +873,8 @@ cell_fwd_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     uint32_t staged_phase = 0;
     CELL_PROBE(const long long probe_t0 = clock64();)
     for (long long it = 0, t; (t = work_index(it)) < num_tiles; ++it) {
-      const long long m0 = tile_m0(t);
+      long long m0, m_end;
+      tile_rows(t, m0, m_end);
       const int nt = (int)(t % EW_N_TILES);
       const int tn = nt >> 1, jh = (nt & 1) * EW_TILE_CH;   // 256-column tile and this N tile's first channel in it
       const int rb = 32 * ew + (lane >> 2);
@@ -860,7 +884,7 @@ cell_fwd_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         float2 cprev[2][4];
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
-          rows[hr] = epi_row(prm, g, m0 + rb + 8 * (k2 + hr));
+          rows[hr] = epi_row(prm, g, m0 + rb + 8 * (k2 + hr), m_end);
 #pragma unroll
           for (int ip = 0; ip < 4; ++ip) cprev[hr][ip] = epi_cprev(prm, rows[hr], tn * TILE_CH + jh + 8 * ip + lc);
         }
@@ -1289,11 +1313,23 @@ static int launch_cell(const CellMaps& tm, const CellParams& prm_in, int num_sms
   return MVB_OK;
 }
 
+// fan-out stage 2: every parent row -> its K children (c_out / h32_out hold NS * fanout sample rows)
+static int fanout_children(const CellStep& s, const float* col_scale, const Grid& g, cudaStream_t stream) {
+  const unsigned blocks = (unsigned)((s.NS * g.H * g.W * 32 + 255) / 256);      // a warp per parent cell
+  auto children = col_scale ? fanout_children_kernel<1> : fanout_children_kernel<0>;
+  children<<<blocks, 256, 0, stream>>>(s.fanout_ws, col_scale, s.xf_B, s.xf_T2, s.xf_ids, s.c_in, s.c_out, s.h32_out,
+                                       s.NS, s.fanout, g, s.forget_bias);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
 int cell_fwd(const CellStep& s, cudaStream_t stream) {
   const int P = s.planes & 0xFF, P_out = (s.planes >> 8) ? (s.planes >> 8) : P;
   MVB_REQUIRE(valid_planes(P) && valid_planes(P_out), "cell_fwd: planes P=%d (output planes %d) not 2 or %d", P, P_out,
               kPlanesF16F8);
-  const bool mixed = P == kPlanesF16F8, fan = s.fanout > 1;
+  const bool mixed = P == kPlanesF16F8, fan = s.fanout > 1 || (s.fanout == 1 && !s.xh);
+  const bool children_only = fan && !s.xh;     // the accumulators of these parents are in fanout_ws already
   const int x_sources = !!s.xf_B + !!s.xs_tab + !!s.xr_W;
   const long long NS = s.NS; const int H = s.H, W = s.W, cpad = s.cpad;
   MVB_REQUIRE(!mixed || !s.gates_out, "cell_fwd: the f16f8 format is an inference format (no gates_out)");
@@ -1306,8 +1342,9 @@ int cell_fwd(const CellStep& s, cudaStream_t stream) {
   MVB_REQUIRE(cpad % XPAD == 0 && cpad >= kHidden + XPAD && cpad <= kHidden + kMaxXBlock,
               "cell_fwd: cpad=%d must be a multiple of %d from %d to %d (x block of 32 to %d channels)", cpad, XPAD,
               kHidden + XPAD, kHidden + kMaxXBlock, kMaxXBlock);
+  MVB_REQUIRE(!s.tiles || (s.tile_count && !fan), "cell_fwd: a work list needs its count and no fan-out");
   MVB_REQUIRE(NS > 0 && H > 0 && W > 0, "cell_fwd: bad sizes NS=%lld H=%d W=%d", NS, H, W);
-  MVB_REQUIRE(s.xh && s.w && (s.bias || s.xf_B) && s.c_out, "cell_fwd: null pointer");
+  MVB_REQUIRE((s.xh || children_only) && s.w && (s.bias || s.xf_B) && s.c_out, "cell_fwd: null pointer");
   if (s.hp_out) MVB_REQUIRE(s.cpad_out % 8 == 0 && s.ch_off_out % 8 == 0, "cell_fwd: hp_out pitch/offset must be multiples of 8");
   const Grid g = make_grid(H, W);
   const long long R = NS * g.S;
@@ -1323,6 +1360,11 @@ int cell_fwd(const CellStep& s, cudaStream_t stream) {
     if ((e && e[0] == '0') || (r && r[0] == '0')) return 0;
     return (e && e[0] == '1') ? 1 : 2;
   }();
+  if (children_only) {
+    const float* col_scale = mixed ? reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(s.w) +
+                                                                    4ull * kGates * 9 * cpad) : nullptr;
+    return fanout_children(s, col_scale, g, stream);
+  }
   CellMaps tm;
   const int P16 = mixed ? 1 : kBf16Planes;      // 16-bit "planes" the A / B maps describe
   const uint32_t ra8 = (uint32_t)((BLOCK_M + 2 * (W + 2) + 7) & ~7);      // rows of an A stage (see CellCfg)
@@ -1380,6 +1422,7 @@ int cell_fwd(const CellStep& s, cudaStream_t stream) {
   prm.hp_out = reinterpret_cast<__nv_bfloat16*>(s.hp_out);
   prm.hp_plane_stride = s.hp_plane_stride; prm.cpad_out = s.cpad_out; prm.ch_off_out = s.ch_off_out;
   prm.R = R; prm.H = H; prm.W = W; prm.cpad = cpad; prm.forget_bias = s.forget_bias;
+  prm.tiles = s.tiles; prm.tile_count = s.tile_count;
 
   int dev = 0, num_sms = 0;
   MVB_CHECK_CUDA(cudaGetDevice(&dev));
@@ -1387,14 +1430,7 @@ int cell_fwd(const CellStep& s, cudaStream_t stream) {
   rc = mixed ? launch_cell<1>(tm, prm, num_sms, multicast, epi_wg, stream)
              : launch_cell<0>(tm, prm, num_sms, multicast, 0, stream);
   if (rc || !fan) return rc;
-  // fan-out stage 2: every parent row -> its K children (c_out / h32_out hold NS * fanout sample rows)
-  const unsigned blocks = (unsigned)((NS * H * W * 32 + 255) / 256);      // a warp per parent cell
-  auto children = mixed ? fanout_children_kernel<1> : fanout_children_kernel<0>;
-  children<<<blocks, 256, 0, stream>>>(s.fanout_ws, col_scale, s.xf_B, s.xf_T2, s.xf_ids, s.c_in, s.c_out, s.h32_out,
-                                       NS, s.fanout, g, s.forget_bias);
-  MVB_CHECK_CUDA(cudaGetLastError());
-  count_launch(1);
-  return MVB_OK;
+  return fanout_children(s, col_scale, g, stream);
 }
 
 // ----------------------------------------------------------------------------------

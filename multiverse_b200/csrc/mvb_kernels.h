@@ -8,6 +8,7 @@ namespace mvb {
 void count_launch(int n);
 
 // mvb_cell.cu
+constexpr int kCellTileRows = 128;    // M rows of a cell kernel tile (and of a beam_band work-list entry at most)
 // One ConvLSTM cell step.  Callers value-initialise it (`CellStep s{};`) and set the fields they use; a null pointer is
 // an input not read or an output not written.  At most one x source (x-fold, sparse, dense) replaces the x block.
 struct CellStep {
@@ -24,7 +25,9 @@ struct CellStep {
   const float* xs_tab; const int* xs_label;       // sparse x: table rows [NS, 9, 1024]; label cells [NS]
   const float *xr_in, *xr_W;                      // dense x: raw input [NS, H, W, 2] fp32; weights [18][1024]
   int fanout;                     // > 1: each x-fold row is the parent of `fanout` child rows of c_out / h32_out,
-  float* fanout_ws;               // through the parents' raw accumulators [R, 1024] fp32
+  float* fanout_ws;               // through the parents' raw accumulators [R, 1024] fp32 (xh null: already there,
+                                  // from an earlier step on the same parents: the GEMM is skipped)
+  const int *tiles, *tile_count;  // work list of M tiles (m0, m_end) [*tile_count][2] (mvb_beam_band), or null
 };
 int cell_fwd(const CellStep& s, cudaStream_t stream);
 int cell_xdense_weights(const float* kernel, float* out, cudaStream_t stream);
@@ -85,6 +88,10 @@ int beam_backtrace(const int* step_ids, const int* step_parents, const float* st
                    cudaStream_t stream);
 int beam_gather_h(const float* h32, const int* row_map, void* hp_out, long long hp_plane_stride, int cpad_out,
                   long long NS, int H, int W, cudaStream_t stream);
+int beam_band(const int* ids, const int* parents, const int* band_in, int* band_out, int* tiles, long long tiles_cap,
+              int* tile_count, long long NS, int K, int radius, int H, int W, cudaStream_t stream);
+int beam_band_copy(const float* base_c, const float* base_h32, const int* band, float* c, float* h32, long long NS,
+                   int K, int H, int W, cudaStream_t stream);
 
 // mvb_metrics.cu
 int min_ade_fde(const float* pred, const float* gt, const int* gt_len, double* ade_err, int* ade_idx, double* fde,

@@ -23,6 +23,8 @@ through it into the cell's operands).
 """
 from __future__ import annotations
 
+import os
+
 import torch
 
 from . import ops
@@ -96,6 +98,11 @@ class ScaleWeights(object):
     if self._enc_class_xf is None:
       self._enc_class_xf = ops.XFold(*self._enc_cell, *self.enc_emb)
     return self._enc_class_xf
+
+
+def beam_band_on():
+  """MVB_BEAM_BAND=0 runs every row of the beam cell launches (decode_class_beam); read at every forward."""
+  return os.environ.get("MVB_BEAM_BAND", "1") != "0"
 
 
 class ConvRNNEngine(object):
@@ -365,6 +372,24 @@ class ConvRNNEngine(object):
                c_t0, h32_t0, None if cfg.use_gnn else xh1[1], h, w, n)
     ops.head_class_fwd(h32_t0, sw.head_class, logits_t0, None, None, None, None, h, w, n, planes=self.planes)
     step_logits[0].copy_(logits_t0.unsqueeze(1).expand(n, b, v))
+    # Image-row bands (ops.beam_band, DESIGN.md 3.2): outside rows band[k], beam k's c and h are bit for bit those of
+    # its sample's base rollout - the same recurrence, through the same kernels, fed the no-selection input (ids
+    # outside the grid) - so the beam cell computes only the bands' rows and the rest is copied from the base.
+    # MVB_BEAM_BAND=0 runs every row.
+    band = pred_len > 2 and beam_band_on()
+    if band:
+      bands = [self._buf(("beam_band", j, ns), lambda: torch.empty((ns, 2), dtype=torch.int32, device=dev))
+               for j in range(2)]
+      tiles = self._buf(("beam_band_tiles", ns, h, w), lambda: torch.empty(
+          (ops.beam_band_capacity(ns, h, w), 2), dtype=torch.int32, device=dev))
+      tile_count = torch.empty((pred_len,), dtype=torch.int32, device=dev)
+      base_xh = self._xh("beam_base", n, h, w, sw.dec_class.cpad, self.class_planes)[0]
+      base_c = [self._state("beam_base_c0", n, h, w), self._state("beam_base_c1", n, h, w)]
+      base_h32 = self._state("beam_base_h32", n, h, w)
+      no_ids = self._buf(("beam_base_ids", n, h, w), lambda: torch.full((n,), (h + 3) * w, dtype=torch.int32,
+                                                                        device=dev))
+      rows = self._buf(("beam_base_rows", n), lambda: torch.arange(n, dtype=torch.int32, device=dev))
+      radius = 2 if cfg.use_gnn else 1      # the graph attention spreads a difference by one more row per step
     h_src, c_src, cur_c = h32_t0, c_t0, 1
     for time in range(1, pred_len + 1):
       if time > 1:
@@ -377,6 +402,9 @@ class ConvRNNEngine(object):
                     gamma=cfg.diverse_gamma)
       if time == pred_len:
         break
+      if band:
+        ops.beam_band(step_ids[time - 1], step_par[time - 1], None if time == 1 else bands[time % 2],
+                      bands[1 - time % 2], tiles, tile_count[time:time + 1], b, radius, h, w)
       nxt = xh[time % 2]
       if time == 1:
         # every child's parent is its sample's single t0 row: the K children share the graph-attended h and c and
@@ -388,13 +416,26 @@ class ConvRNNEngine(object):
             (ops.halo_rows(n, h, w), 4 * ops.HIDDEN), dtype=torch.float32, device=dev))
         self._cell("beam_fanout", (h, w, n), ops.cell_fwd_onehot_fanout, xh1[1], sw.dec_class, xf,
                    step_ids[0].view(-1), c_t0, c[1 - cur_c], h32, h, w, n, b, workspace=ws)
+        if band:      # the base's first step: the same accumulators, no selection
+          ops.cell_fwd_onehot_fanout(None, sw.dec_class, xf, no_ids, c_t0, base_c[1], base_h32, h, w, n, 1,
+                                     workspace=ws)
       else:
+        if band:
+          if cfg.use_gnn:
+            ops.gnn_attend_fwd(base_h32, scene_mean, base_xh, h, w, n, beam=1, row_map=None)
+          else:
+            ops.beam_gather_h(base_h32, rows, base_xh, h, w, n)
+          self._cell("beam_base", (h, w, n), ops.cell_fwd_onehot, base_xh, sw.dec_class, xf, no_ids,
+                     base_c[(time - 1) % 2], base_c[time % 2], base_h32, None, h, w, n)
         if cfg.use_gnn:
           ops.gnn_attend_fwd(h_src, scene_mean, nxt, h, w, ns, beam=b, row_map=row_map)
         else:
           ops.beam_gather_h(h_src, row_map, nxt, h, w, ns)
         self._cell("beam", (h, w, ns), ops.cell_fwd_onehot, nxt, sw.dec_class, xf, step_ids[time - 1].view(-1), c_src,
-                   c[1 - cur_c], h32, None, h, w, ns, row_map=row_map)
+                   c[1 - cur_c], h32, None, h, w, ns, row_map=row_map,
+                   tiles=(tiles, tile_count[time:time + 1]) if band else None)
+        if band:
+          ops.beam_band_copy(base_c[time % 2], base_h32, bands[1 - time % 2], c[1 - cur_c], h32, b, h, w)
       cur_c = 1 - cur_c
       h_src, c_src = h32, c[cur_c]
     out_ids = torch.empty((n, b, pred_len), dtype=torch.int32, device=dev)
@@ -500,7 +541,8 @@ class ConvRNNEngine(object):
     sf = feeds["scene_feat"]
     f_pad = -(-int(sf.shape[0]) // 64) * 64
     flat = self._flat_feeds(feeds)
-    key = (tp, f_pad) + tuple((k, tuple(t.shape[1:] if k == "scene_feat" else t.shape), t.dtype) for k, t in flat)
+    key = (tp, f_pad) + tuple((k, tuple(t.shape[1:] if k == "scene_feat" else t.shape), t.dtype) for k, t in flat) + \
+        (("MVB_BEAM_BAND", beam_band_on()),)     # a graph holds one of the two beam paths
     ent = self._graphs.get(key)
     main = torch.cuda.current_stream(self.device)
     if ent is None:

@@ -205,19 +205,22 @@ class XFold(object):
 
 
 def cell_fwd_onehot(xh, packed, xf, ids, c_in, c_out, h32_out, xh_next, h, w, ns, row_map=None,
-                    forget_bias=1.0):
-  """Class-decoder step with the embedded one-hot input folded into table look-ups."""
+                    forget_bias=1.0, tiles=None):
+  """Class-decoder step with the embedded one-hot input folded into table look-ups.  tiles: (list, count) work list
+  of beam_band (only its rows are computed and written), or None (every row)."""
   hp = _hp_out(xh, packed, xh_next)
+  tl, tn = tiles if tiles is not None else (None, None)
   _lib.call("mvb_convlstm_cell_fwd_onehot", _p(xh), _p(packed.w), _p(xf.B), _p(xf.T2), _p(ids), _p(c_in),
-            _p(row_map), _p(c_out), _p(h32_out), *hp, ns, h, w, packed.cpad, _planes_arg(packed, xh_next),
-            float(forget_bias), _stream())
+            _p(row_map), _p(tl), _p(tn), _p(c_out), _p(h32_out), *hp, ns, h, w, packed.cpad,
+            _planes_arg(packed, xh_next), float(forget_bias), _stream())
 
 
 def cell_fwd_onehot_fanout(xh, packed, xf, ids, c_in, c_out, h32_out, h, w, ns, fanout, forget_bias=1.0,
                            workspace=None):
   """First K-row beam step: GEMM on the `ns` parent rows (raw accumulators to `workspace` fp32 [ns*S, 1024]), then
-  the children kernel emits ns*fanout child rows (ids [ns*fanout])."""
-  assert xh.shape[2] == packed.cpad and planes_of(xh) == packed.planes
+  the children kernel emits ns*fanout child rows (ids [ns*fanout]).  xh None: `workspace` holds the accumulators of
+  an earlier call on the same parents; only the children are emitted."""
+  assert xh is None and workspace is not None or xh.shape[2] == packed.cpad and planes_of(xh) == packed.planes
   if workspace is None:
     workspace = torch.empty((halo_rows(ns, h, w), 4 * HIDDEN), dtype=torch.float32, device=xh.device)
   assert workspace.numel() >= halo_rows(ns, h, w) * 4 * HIDDEN and workspace.dtype == torch.float32
@@ -330,6 +333,28 @@ def beam_gather_h(h32, row_map, xh_next, h, w, ns):
   assert xh_next.shape[1] == halo_rows(ns, h, w) and row_map.dtype == torch.int32 and row_map.numel() == ns
   _lib.call("mvb_beam_gather_h_f16f8", _p(h32), _p(row_map), _p(xh_next), xh_next.stride(0), xh_next.shape[2], ns,
             h, w, _stream())
+
+
+def beam_band_capacity(ns, h, w):
+  """Work-list entries beam_band may write for ns beam rows."""
+  return ns * (((h + 1) * (w + 1) + 127) // 128 + 1)
+
+
+def beam_band(ids, parents, band_in, band_out, tiles, tile_count, k, radius, h, w):
+  """Bands band_out int32 [ns, 2] (first, last image row where beam s may differ from its sample's base rollout) from
+  the step's ids / parents int32 [N, K] and the parents' bands band_in (None at the fan-out), and the work list of
+  the step's cell launch: tiles int32 [beam_band_capacity, 2] (m0, m_end) and tile_count int32 [1]."""
+  ns = ids.numel()
+  assert band_out.shape == (ns, 2) and band_out.dtype == torch.int32 and tiles.shape[1] == 2
+  _lib.call("mvb_beam_band", _p(ids), _p(parents), _p(band_in), _p(band_out), _p(tiles), tiles.shape[0],
+            _p(tile_count), ns, k, radius, h, w, _stream())
+
+
+def beam_band_copy(base_c, base_h32, band, c, h32, k, h, w):
+  """Valid rows of beam s outside band[s] <- the rows of sample s // k of the base rollout's state."""
+  ns = band.shape[0]
+  assert c.shape[0] == halo_rows(ns, h, w) and base_c.shape[0] * k == c.shape[0]
+  _lib.call("mvb_beam_band_copy", _p(base_c), _p(base_h32), _p(band), _p(c), _p(h32), ns, k, h, w, _stream())
 
 
 def beam_backtrace(step_ids, step_parents, step_logits, out_ids, out_logits):
