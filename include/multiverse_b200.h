@@ -367,6 +367,12 @@ int mvb_beam_nll(const float* logits, const float* logprobs, const int32_t* gt_i
 int mvb_beam_backtrace(const int32_t* step_ids, const int32_t* step_parents,
                        const float* step_logits, int32_t* out_ids, float* out_logits, int64_t N,
                        int B, int Tp, int V, void* stream);
+/* Back-trace of a batch whose rows end at their own lengths (1 <= lengths[n] <= Tp, int32 [N]): row n's trace starts
+ * at its own last step lengths[n] - 1, and out_ids / out_logits of row n at the steps t >= lengths[n] are zeros.
+ * Shapes as mvb_beam_backtrace; steps >= lengths[n] of the step buffers are not read for row n. */
+int mvb_beam_backtrace_ragged(const int32_t* step_ids, const int32_t* step_parents, const float* step_logits,
+                              const int32_t* lengths, int32_t* out_ids, float* out_logits, int64_t N, int B, int Tp,
+                              int V, void* stream);
 
 /* Parent-state gather of the beam decoder without graph attention (use_gnn off: pred_models.py:611-623, then the
  * gathered h goes straight into the cell): for every sample row s < NS and valid cell, the h block (channels
@@ -403,6 +409,11 @@ int mvb_traj_to_grid(const double* traj, const double* centers, double h_gap, do
  *      ids int32 [N,K,Tp]; offsets fp32 [Tp,N,V,2] (mvb_head_reg_fwd layout); centers fp32 [V,2]. */
 int mvb_decode_trajectories(const int32_t* ids, const float* offsets, const float* centers, float* out,
                             int64_t N, int K, int Tp, int V, void* stream);
+/* The fp32 offsets of the selected cells alone, for a caller that adds them to the centres in its own precision
+ * (multifuture_inference.py:495-517 in float64): out[n,k,t] = offsets[t,n,ids[n,k,t]] for t < lengths[n], zeros
+ * after.  ids int32 [N,K,Tp]; offsets fp32 [Tp,N,V,2]; lengths int32 [N] (1..Tp); out fp32 [N,K,Tp,2]. */
+int mvb_gather_offsets(const int32_t* ids, const float* offsets, const int32_t* lengths, float* out, int64_t N, int K,
+                       int Tp, int V, void* stream);
 
 #ifdef __cplusplus
 }

@@ -79,6 +79,8 @@ SIGNATURES = {
     "mvb_min_ade_fde": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp],
     "mvb_beam_nll": [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _vp],
     "mvb_beam_backtrace": [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],
+    "mvb_beam_backtrace_ragged": [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],
+    "mvb_gather_offsets": [_vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],
     "mvb_beam_gather_h_f16f8": [_vp, _vp, _vp, _i64, _i, _i64, _i, _i, _vp],
     "mvb_beam_band": [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i, _i, _i, _i, _vp],
     "mvb_beam_band_copy": [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],

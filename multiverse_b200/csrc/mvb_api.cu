@@ -413,6 +413,16 @@ int mvb_beam_backtrace(const int32_t* step_ids, const int32_t* step_parents,
   return beam_backtrace(step_ids, step_parents, step_logits, out_ids, out_logits, N, B, Tp, V,
                         S(stream));
 }
+int mvb_beam_backtrace_ragged(const int32_t* step_ids, const int32_t* step_parents, const float* step_logits,
+                              const int32_t* lengths, int32_t* out_ids, float* out_logits, int64_t N, int B, int Tp,
+                              int V, void* stream) {
+  return beam_backtrace_ragged(step_ids, step_parents, step_logits, lengths, out_ids, out_logits, N, B, Tp, V,
+                               S(stream));
+}
+int mvb_gather_offsets(const int32_t* ids, const float* offsets, const int32_t* lengths, float* out, int64_t N, int K,
+                       int Tp, int V, void* stream) {
+  return gather_offsets(ids, offsets, lengths, out, N, K, Tp, V, S(stream));
+}
 int mvb_beam_gather_h_f16f8(const float* h32, const int32_t* row_map, void* hp_out, int64_t hp_plane_stride,
                             int cpad_out, int64_t NS, int H, int W, void* stream) {
   return beam_gather_h(h32, row_map, hp_out, hp_plane_stride, cpad_out, NS, H, W, S(stream));

@@ -490,4 +490,78 @@ int beam_backtrace(const int* step_ids, const int* step_parents, const float* st
   return MVB_OK;
 }
 
+// The back-trace of a batch whose rows end at their own lengths: row n's trace starts at its last step
+// lengths[n] - 1 (its selections stop there; the step buffers of a ragged rollout hold nothing for it beyond), and
+// its outputs at the steps after it are zeros.
+__global__ void __launch_bounds__(256)
+beam_backtrace_ragged_kernel(const int* __restrict__ step_ids, const int* __restrict__ step_parents,
+                             const float* __restrict__ step_logits, const int* __restrict__ lengths,
+                             int* __restrict__ out_ids, float* __restrict__ out_logits, long long N, int B, int Tp,
+                             int V) {
+  extern __shared__ int src[];  // [Tp] source beam of each step for this (n, b)
+  const long long nb = blockIdx.x;
+  const long long n = nb / B;
+  const int b = (int)(nb - n * B);
+  const int len = lengths[n];
+  if (threadIdx.x == 0) {
+    int p = b;
+    for (int tau = len - 1; tau >= 0; --tau) {
+      const long long o = ((long long)tau * N + n) * B + p;
+      src[tau] = p;
+      out_ids[(n * B + b) * Tp + tau] = step_ids[o];
+      p = step_parents[o];
+    }
+  }
+  for (int tau = len + (int)threadIdx.x; tau < Tp; tau += blockDim.x) out_ids[(n * B + b) * Tp + tau] = 0;
+  __syncthreads();
+  for (int tau = 0; tau < Tp; ++tau) {
+    float* d = out_logits + ((n * B + b) * (long long)Tp + tau) * V;
+    if (tau < len) {
+      const float* s = step_logits + (((long long)tau * N + n) * B + src[tau]) * V;
+      for (int v = threadIdx.x; v < V; v += blockDim.x) d[v] = s[v];
+    } else {
+      for (int v = threadIdx.x; v < V; v += blockDim.x) d[v] = 0.f;
+    }
+  }
+}
+
+int beam_backtrace_ragged(const int* step_ids, const int* step_parents, const float* step_logits, const int* lengths,
+                          int* out_ids, float* out_logits, long long N, int B, int Tp, int V, cudaStream_t stream) {
+  MVB_REQUIRE(step_ids && step_parents && step_logits && lengths && out_ids && out_logits,
+              "beam_backtrace_ragged: null pointer");
+  MVB_REQUIRE(N > 0 && B >= 1 && Tp >= 1 && V >= 1, "beam_backtrace_ragged: bad sizes");
+  beam_backtrace_ragged_kernel<<<(unsigned)(N * B), 256, sizeof(int) * Tp, stream>>>(
+      step_ids, step_parents, step_logits, lengths, out_ids, out_logits, N, B, Tp, V);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
+// The fp32 offsets of the selected cells: out[n,k,t] = offs[t, n, ids[n,k,t]] for t < lengths[n], zeros after
+// (what a caller adds to the cell centres on the host, code/multifuture_inference.py:504-517, in its own precision).
+__global__ void gather_offsets_kernel(const int* __restrict__ ids, const float* __restrict__ offs,
+                                      const int* __restrict__ lengths, float* __restrict__ out, long long N, int K,
+                                      int Tp, int V) {
+  const long long total = N * K * Tp;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int t = (int)(i % Tp);
+    const long long n = i / ((long long)Tp * K);
+    float2 o = make_float2(0.f, 0.f);
+    if (t < lengths[n]) o = *reinterpret_cast<const float2*>(offs + (((long long)t * N + n) * V + ids[i]) * 2);
+    *reinterpret_cast<float2*>(out + 2 * i) = o;
+  }
+}
+
+int gather_offsets(const int* ids, const float* offs, const int* lengths, float* out, long long N, int K, int Tp,
+                   int V, cudaStream_t stream) {
+  MVB_REQUIRE(ids && offs && lengths && out && N > 0 && K > 0 && Tp > 0 && V > 0, "gather_offsets: bad args");
+  const long long total = N * K * Tp;
+  const int blocks = (int)((total + 255) / 256 < sm_count() * 8 ? (total + 255) / 256 : sm_count() * 8);
+  gather_offsets_kernel<<<blocks, 256, 0, stream>>>(ids, offs, lengths, out, N, K, Tp, V);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
 }  // namespace mvb

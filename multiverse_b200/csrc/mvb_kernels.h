@@ -86,6 +86,10 @@ int beam_step(const float* logits, const float* score_in, float* score_out, int*
 int beam_backtrace(const int* step_ids, const int* step_parents, const float* step_logits,
                    int* out_ids, float* out_logits, long long N, int B, int Tp, int V,
                    cudaStream_t stream);
+int beam_backtrace_ragged(const int* step_ids, const int* step_parents, const float* step_logits, const int* lengths,
+                          int* out_ids, float* out_logits, long long N, int B, int Tp, int V, cudaStream_t stream);
+int gather_offsets(const int* ids, const float* offs, const int* lengths, float* out, long long N, int K, int Tp,
+                   int V, cudaStream_t stream);
 int beam_gather_h(const float* h32, const int* row_map, void* hp_out, long long hp_plane_stride, int cpad_out,
                   long long NS, int H, int W, cudaStream_t stream);
 int beam_band(const int* ids, const int* parents, const int* band_in, int* band_out, int* tiles, long long tiles_cap,

@@ -286,8 +286,9 @@ class ConvRNNEngine(object):
                  c[(t + 1) % 2], h32 if last else None, xh_out if last else nxt, h, w, n)
     return c[t_len % 2], h32
 
-  def decode_class_greedy(self, i, c_enc, h32_enc, first_ids, scene_mean, pred_len):
-    """Greedy class decoder (:311-471, appendix A.1).  Returns logits [Tp,N,HW], ids [Tp,N]."""
+  def decode_class_greedy(self, i, c_enc, h32_enc, first_ids, scene_mean, pred_len, act=None):
+    """Greedy class decoder (:311-471, appendix A.1).  Returns logits [Tp,N,HW], ids [Tp,N].
+    act: ragged rollout (forward(pred_lengths=...)): step t runs the first act[t] rows only, the rest stay zero."""
     cfg = self.cfg
     h, w = cfg.scene_grids[i]
     n = first_ids.shape[0]
@@ -295,47 +296,64 @@ class ConvRNNEngine(object):
     xh = self._xh("dec_class", n, h, w, sw.dec_class.cpad, self.class_planes)
     c = [self._state("dec_c0", n, h, w), self._state("dec_c1", n, h, w)]
     h32 = self._state("dec_h32", n, h, w)
-    logits = torch.empty((pred_len, n, h * w), dtype=torch.float32, device=self.device)
-    ids = torch.empty((pred_len, n), dtype=torch.int32, device=self.device)
-    h_src, c_src, ids_prev = h32_enc, c_enc, first_ids
+    alloc = torch.empty if act is None else torch.zeros
+    logits = alloc((pred_len, n, h * w), dtype=torch.float32, device=self.device)
+    ids = alloc((pred_len, n), dtype=torch.int32, device=self.device)
+    h_src, c_src, ids_prev, m = h32_enc, c_enc, first_ids, n
     for t in range(pred_len):
       cur, nxt = xh[t % 2], xh[(t + 1) % 2]
+      if act is not None:     # operand planes as the kernels address them for the running rows (ops.operand_rows)
+        if not cfg.use_gnn:   # cur holds the previous step's h for its m rows
+          ops.operand_shrink(cur, m, act[t], h, w)
+        m = act[t]
+        cur, nxt = ops.operand_rows(cur, m, h, w), ops.operand_rows(nxt, m, h, w)
       if cfg.use_gnn:
-        ops.gnn_attend_fwd(h_src, scene_mean if self.gnn_scene_in_greedy else None, cur, h, w, n)
+        ops.gnn_attend_fwd(h_src, scene_mean if self.gnn_scene_in_greedy else None, cur, h, w, m)
       # (no attention: the planes of the previous h already sit in cur's h block)
       # the embedded one_hot(ids_prev) input is folded into table look-ups: nobody writes the x block
-      self._cell("dec_class", (h, w, n), ops.cell_fwd_onehot, cur, sw.dec_class, sw.dec_class_xf, ids_prev, c_src,
-                 c[(t + 1) % 2], h32, None if cfg.use_gnn else nxt, h, w, n)
+      self._cell("dec_class", (h, w, m), ops.cell_fwd_onehot, cur, sw.dec_class, sw.dec_class_xf, ids_prev, c_src,
+                 c[(t + 1) % 2], h32, None if cfg.use_gnn else nxt, h, w, m)
       c_src, h_src = c[(t + 1) % 2], h32
-      ops.head_class_fwd(h32, sw.head_class, logits[t], ids[t], None, None, None, h, w, n,
+      ops.head_class_fwd(h32, sw.head_class, logits[t], ids[t], None, None, None, h, w, m,
                          planes=self.planes)
       ids_prev = ids[t]
     return logits, ids
 
-  def decode_reg(self, i, c_enc, first_input, pred_len, xh):
+  def decode_reg(self, i, c_enc, first_input, pred_len, xh, act=None):
     """Regression decoder (:298-305): greedy, no attention, raw 2-channel feedback.  `xh` are
-    the decoder operand buffers whose xh[0] h block already holds the encoder state planes."""
+    the decoder operand buffers whose xh[0] h block already holds the encoder state planes.  act: as
+    decode_class_greedy."""
     h, w = self.cfg.scene_grids[i]
     n = first_input.shape[0]
     sw = self.scales[i]
     c = [self._state("decr_c0", n, h, w), self._state("decr_c1", n, h, w)]
     h32 = self._state("decr_h32", n, h, w)
-    offs = torch.empty((pred_len, n, h * w, 2), dtype=torch.float32, device=self.device)
+    offs = (torch.empty if act is None else torch.zeros)((pred_len, n, h * w, 2), dtype=torch.float32,
+                                                          device=self.device)
     We, be = sw.emb_reg
     ops.emb_dense_fwd(first_input, We, be, xh[0], h, w)
-    c_src = c_enc
+    c_src, m = c_enc, n
     for t in range(pred_len):
       cur, nxt = xh[t % 2], xh[(t + 1) % 2]
-      self._cell("dec_reg", (h, w, n), ops.cell_fwd, cur, sw.dec_reg, c_src, c[(t + 1) % 2], h32, nxt, h, w, n)
+      if act is not None:     # cur holds the previous step's h and fed-back offsets for its m rows
+        ops.operand_shrink(cur, m, act[t], h, w)
+        m = act[t]
+        cur, nxt = ops.operand_rows(cur, m, h, w), ops.operand_rows(nxt, m, h, w)
+      self._cell("dec_reg", (h, w, m), ops.cell_fwd, cur, sw.dec_reg, c_src, c[(t + 1) % 2], h32, nxt, h, w, m)
       c_src = c[(t + 1) % 2]
       last = t == pred_len - 1
       ops.head_reg_fwd(h32, sw.head_reg, offs[t], None if last else We, None if last else be,
-                       None if last else nxt, h, w, n, planes=self.planes)
+                       None if last else nxt, h, w, m, planes=self.planes)
     return offs
 
-  def decode_class_beam(self, i, c_enc, h32_enc, first_ids, scene_mean, pred_len):
+  def decode_class_beam(self, i, c_enc, h32_enc, first_ids, scene_mean, pred_len, act=None, lengths=None):
     """K-way beam decoder (:474-806, appendix A.2).  Returns (out_logits [N,B,Tp,V],
-    out_ids [N,B,Tp] int32, scores [N,B])."""
+    out_ids [N,B,Tp] int32, scores [N,B]).
+    Ragged rollout (forward(pred_lengths=...)): rows sorted by length, longest first; lengths int32 [N] on the device
+    and act[t] = number of rows longer than t.  The selection at time t runs the rows whose length is at least t,
+    the cell of time t (which feeds the selection at t + 1) only those longer than t: every launch takes a prefix of
+    the rows, and a row's outputs are those of a rollout of its own length.  Its scores are those after its own last
+    selection, its outputs after its length zeros."""
     cfg = self.cfg
     h, w = cfg.scene_grids[i]
     n, b, v = first_ids.shape[0], cfg.beam_size, h * w
@@ -377,6 +395,11 @@ class ConvRNNEngine(object):
     # outside the grid) - so the beam cell computes only the bands' rows and the rest is copied from the base.
     # MVB_BEAM_BAND=0 runs every row.
     band = pred_len > 2 and beam_band_on()
+    # samples in the selection (sel) and in the cell step (ncell) of each time, and the operand planes of ns rows as
+    # the kernels address them (ops.operand_rows)
+    sel = (lambda time: n) if act is None else (lambda time: act[time - 1])
+    ncell = (lambda time: n) if act is None else (lambda time: act[time])
+    rows_of = (lambda t, ns_: t) if act is None else (lambda t, ns_: ops.operand_rows(t, ns_, h, w))
     if band:
       bands = [self._buf(("beam_band", j, ns), lambda: torch.empty((ns, 2), dtype=torch.int32, device=dev))
                for j in range(2)]
@@ -392,57 +415,70 @@ class ConvRNNEngine(object):
       radius = 2 if cfg.use_gnn else 1      # the graph attention spreads a difference by one more row per step
     h_src, c_src, cur_c = h32_t0, c_t0, 1
     for time in range(1, pred_len + 1):
+      ms = sel(time)
       if time > 1:
         ops.head_class_fwd(h32, sw.head_class, step_logits[time - 1], None, None, None, None, h, w,
-                           ns, planes=self.planes)
+                           ms * b, planes=self.planes)
       s_in, s_out = scores[(time - 1) % 2], scores[time % 2]
       ops.beam_step(step_logits[time - 1], s_in, s_out, step_ids[time - 1], step_par[time - 1],
-                    row_map, n, b, v, first_step=(time <= 1),
+                    row_map, ms, b, v, first_step=(time <= 1),
                     zero_scores=(time <= cfg.fix_num_timestep), diverse=cfg.diverse_beam,
                     gamma=cfg.diverse_gamma)
       if time == pred_len:
         break
+      m = ncell(time)
       if band:
-        ops.beam_band(step_ids[time - 1], step_par[time - 1], None if time == 1 else bands[time % 2],
-                      bands[1 - time % 2], tiles, tile_count[time:time + 1], b, radius, h, w)
-      nxt = xh[time % 2]
+        ops.beam_band(step_ids[time - 1][:m], step_par[time - 1][:m], None if time == 1 else bands[time % 2],
+                      bands[1 - time % 2][:m * b], tiles, tile_count[time:time + 1], b, radius, h, w)
+      nxt = rows_of(xh[time % 2], m * b)
       if time == 1:
         # every child's parent is its sample's single t0 row: the K children share the graph-attended h and c and
         # differ only in the selected cell, i.e. in the folded table rows -> attention and GEMM once per sample,
         # the cell epilogue fans the K children out (ops.cell_fwd_onehot_fanout; 1/K of the step's MMAs)
+        if not cfg.use_gnn and act is not None:     # the time-0 cell wrote h for all rows
+          ops.operand_shrink(xh1[1], n, m, h, w)
+        x_t1 = rows_of(xh1[1], m)
         if cfg.use_gnn:
-          ops.gnn_attend_fwd(h32_t0, scene_mean, xh1[1], h, w, n, beam=1, row_map=None)
+          ops.gnn_attend_fwd(h32_t0, scene_mean, x_t1, h, w, m, beam=1, row_map=None)
         ws = self._buf(("beam_fanout_ws", n, h, w), lambda: torch.empty(
             (ops.halo_rows(n, h, w), 4 * ops.HIDDEN), dtype=torch.float32, device=dev))
-        self._cell("beam_fanout", (h, w, n), ops.cell_fwd_onehot_fanout, xh1[1], sw.dec_class, xf,
-                   step_ids[0].view(-1), c_t0, c[1 - cur_c], h32, h, w, n, b, workspace=ws)
+        self._cell("beam_fanout", (h, w, m), ops.cell_fwd_onehot_fanout, x_t1, sw.dec_class, xf,
+                   step_ids[0].view(-1), c_t0, c[1 - cur_c], h32, h, w, m, b, workspace=ws)
         if band:      # the base's first step: the same accumulators, no selection
-          ops.cell_fwd_onehot_fanout(None, sw.dec_class, xf, no_ids, c_t0, base_c[1], base_h32, h, w, n, 1,
+          ops.cell_fwd_onehot_fanout(None, sw.dec_class, xf, no_ids, c_t0, base_c[1], base_h32, h, w, m, 1,
                                      workspace=ws)
       else:
         if band:
+          x_base = rows_of(base_xh, m)
           if cfg.use_gnn:
-            ops.gnn_attend_fwd(base_h32, scene_mean, base_xh, h, w, n, beam=1, row_map=None)
+            ops.gnn_attend_fwd(base_h32, scene_mean, x_base, h, w, m, beam=1, row_map=None)
           else:
-            ops.beam_gather_h(base_h32, rows, base_xh, h, w, n)
-          self._cell("beam_base", (h, w, n), ops.cell_fwd_onehot, base_xh, sw.dec_class, xf, no_ids,
-                     base_c[(time - 1) % 2], base_c[time % 2], base_h32, None, h, w, n)
+            ops.beam_gather_h(base_h32, rows[:m], x_base, h, w, m)
+          self._cell("beam_base", (h, w, m), ops.cell_fwd_onehot, x_base, sw.dec_class, xf, no_ids,
+                     base_c[(time - 1) % 2], base_c[time % 2], base_h32, None, h, w, m)
         if cfg.use_gnn:
-          ops.gnn_attend_fwd(h_src, scene_mean, nxt, h, w, ns, beam=b, row_map=row_map)
+          ops.gnn_attend_fwd(h_src, scene_mean, nxt, h, w, m * b, beam=b, row_map=row_map)
         else:
-          ops.beam_gather_h(h_src, row_map, nxt, h, w, ns)
-        self._cell("beam", (h, w, ns), ops.cell_fwd_onehot, nxt, sw.dec_class, xf, step_ids[time - 1].view(-1), c_src,
-                   c[1 - cur_c], h32, None, h, w, ns, row_map=row_map,
+          ops.beam_gather_h(h_src, row_map[:m * b], nxt, h, w, m * b)
+        self._cell("beam", (h, w, m * b), ops.cell_fwd_onehot, nxt, sw.dec_class, xf, step_ids[time - 1].view(-1),
+                   c_src, c[1 - cur_c], h32, None, h, w, m * b, row_map=row_map,
                    tiles=(tiles, tile_count[time:time + 1]) if band else None)
         if band:
-          ops.beam_band_copy(base_c[time % 2], base_h32, bands[1 - time % 2], c[1 - cur_c], h32, b, h, w)
+          hr, hr_base = ops.halo_rows(m * b, h, w), ops.halo_rows(m, h, w)
+          ops.beam_band_copy(base_c[time % 2][:hr_base], base_h32[:hr_base], bands[1 - time % 2][:m * b],
+                             c[1 - cur_c][:hr], h32[:hr], b, h, w)
       cur_c = 1 - cur_c
       h_src, c_src = h32, c[cur_c]
     out_ids = torch.empty((n, b, pred_len), dtype=torch.int32, device=dev)
     out_logits = torch.empty((n, b, pred_len, v), dtype=torch.float32, device=dev)
-    ops.beam_backtrace(step_ids, step_par, step_logits, out_ids, out_logits)
-    return out_logits, out_ids, scores[pred_len % 2], dict(ids=step_ids, parents=step_par,
-                                                           logits=step_logits)
+    if act is None:
+      ops.beam_backtrace(step_ids, step_par, step_logits, out_ids, out_logits)
+      final = scores[pred_len % 2]
+    else:
+      ops.beam_backtrace_ragged(step_ids, step_par, step_logits, lengths, out_ids, out_logits)
+      # row j's last selection (time lengths[j]) wrote scores[lengths[j] % 2]; later selections skip it
+      final = torch.where((lengths % 2 == 0).unsqueeze(1), scores[0], scores[1])
+    return out_logits, out_ids, final, dict(ids=step_ids, parents=step_par, logits=step_logits)
 
   # ------------------------------------------------------------------ whole forward
   def branches(self):
@@ -450,7 +486,7 @@ class ConvRNNEngine(object):
     the scene CNN belongs to the class chains)."""
     return [(kind, i) for i in range(len(self.cfg.scene_grids)) if self.cfg.use_grids[i] for kind in ("class", "reg")]
 
-  def forward(self, feeds, pred_len=None, on_output=None, branches=None):
+  def forward(self, feeds, pred_len=None, on_output=None, branches=None, pred_lengths=None):
     """feeds: device tensors
          scene_feat fp32 [F,SH,SW,SC], obs_scene int32 [N,T],
          grid_obs_labels[i] int32 [N,T], grid_obs_regress[i] fp32 [N,T,h,w,2]
@@ -460,7 +496,13 @@ class ConvRNNEngine(object):
     on_output(name, index, tensor) is called as soon as a fetched tensor is complete on the current stream, so a
     caller can start its device->host copy on another stream while the remaining branches still run.
     `branches`: subset of self.branches() to run (forward_graph captures one graph per chain); the outputs of the
-    others are None."""
+    others are None.
+    `pred_lengths`: int [N], every L_i >= 1 (host array or tensor), decodes each row to its own length: the rollout
+    runs T = max L_i steps (pred_len is ignored), and row i's outputs at t < L_i are byte for byte those of a forward
+    of row i alone with pred_len = L_i, zeros at t >= L_i; beam_outputs[2][i] holds the scores after row i's own last
+    selection.  The rows are sorted by length, longest first, and every step launches only the rows still running
+    (the rollout of code/multifuture_inference.py, which decodes every trajectory alone to its own length, :311).
+    With all lengths equal this is forward(pred_len=T).  out["_lengths"]: the lengths, int32 on the device."""
     cfg = self.cfg
     emit = on_output if on_output is not None else (lambda *a: None)
     run = set(self.branches() if branches is None else branches)
@@ -468,8 +510,26 @@ class ConvRNNEngine(object):
     # FED pred_length (multifuture_inference.py feeds max_pred_lengths[idx], :311), not config.pred_len
     tp = int(pred_len) if pred_len else cfg.pred_len
     obs_scene = feeds["obs_scene"].to(torch.int32).contiguous()
-    obs_scene_t = obs_scene.t().contiguous()
     n = obs_scene.shape[0]
+    act = lengths = perm = inv = None
+    if pred_lengths is not None:
+      import numpy as np
+      lens = np.asarray(pred_lengths.cpu() if torch.is_tensor(pred_lengths) else pred_lengths).astype(np.int64)
+      lens = lens.reshape(-1)
+      if lens.size != n or lens.min() < 1:
+        raise ValueError("pred_lengths: one length >= 1 per row (%d rows), got %s" % (n, lens))
+      tp = int(lens.max())
+      if (lens != tp).any():
+        order = np.argsort(-lens, kind="stable")
+        act = [int((lens > t).sum()) for t in range(tp)]
+        perm = torch.from_numpy(order).to(self.device)
+        inv = torch.from_numpy(np.argsort(order)).to(self.device)
+        lengths = torch.from_numpy(lens[order].astype(np.int32)).to(self.device)
+        obs_scene = obs_scene.index_select(0, perm)
+    # rows back in the caller's order (ragged: they run sorted by length)
+    unsort = (lambda t, dim=0: t) if inv is None else (lambda t, dim=0: t.index_select(dim, inv))
+    sort = (lambda t: t) if perm is None else (lambda t: t.index_select(0, perm))
+    obs_scene_t = obs_scene.t().contiguous()
     convs = means = None
     if any(kind == "class" for kind, _ in run):
       convs, means = self.scene_cnn(feeds["scene_feat"].float().contiguous(), obs_scene)
@@ -482,7 +542,7 @@ class ConvRNNEngine(object):
       sw = self.scales[i]
       dec = reg = None
       if ("class", i) in run:
-        labels = feeds["grid_obs_labels"][i].to(torch.int32)
+        labels = sort(feeds["grid_obs_labels"][i].to(torch.int32))
         labels_t = labels.t().contiguous()
         # without the graph attention the encoder writes its last h straight into the decoder's first operands
         xh_dec = self._xh("beam_t0" if cfg.use_beam_search and not cfg.use_gnn else "dec_class", n, h, w,
@@ -491,26 +551,29 @@ class ConvRNNEngine(object):
                                      None if cfg.use_gnn else xh_dec[0])
         if cfg.use_beam_search:
           logits, ids, logprobs, _ = self.decode_class_beam(i, c_e, h_e, labels_t[-1].contiguous(),
-                                                            means[i], tp)
-          out["beam_outputs"] = [logits, ids, logprobs]
-          dec = logits[:, 0].reshape(n, tp, h, w, 1)                      # :799-803
+                                                            means[i], tp, act, lengths)
+          out["beam_outputs"] = [unsort(logits), unsort(ids), unsort(logprobs)]
+          dec = out["beam_outputs"][0][:, 0].reshape(n, tp, h, w, 1)     # :799-803
           for j, t in enumerate(out["beam_outputs"]):
             emit("beam_outputs", j, t)
         else:
-          lg, _ = self.decode_class_greedy(i, c_e, h_e, labels_t[-1].contiguous(), means[i], tp)
-          dec = lg.permute(1, 0, 2).reshape(n, tp, h, w, 1)
+          lg, _ = self.decode_class_greedy(i, c_e, h_e, labels_t[-1].contiguous(), means[i], tp, act)
+          dec = unsort(lg, 1).permute(1, 0, 2).reshape(n, tp, h, w, 1)
         emit("grid_pred_decoded", i, dec)
       if ("reg", i) in run:
-        obs_reg = feeds["grid_obs_regress"][i].float()
+        obs_reg = sort(feeds["grid_obs_regress"][i].float())
         obs_reg_t = obs_reg.transpose(0, 1).contiguous()
         xh_reg = self._xh("dec_reg", n, h, w, sw.dec_reg.cpad, self.fast_planes)
         c_r, _ = self.encode_reg(i, obs_reg_t, xh_reg[0])
-        offs = self.decode_reg(i, c_r, obs_reg_t[-1], tp, xh_reg)
+        offs = unsort(self.decode_reg(i, c_r, obs_reg_t[-1], tp, xh_reg, act), 1)
         reg = offs.permute(1, 0, 2, 3).reshape(n, tp, h, w, 2)
         emit("grid_pred_reg_decoded", i, reg)
         out.setdefault("_offs", {})[i] = offs           # engine layout [Tp,N,HW,2], for decode_trajectories
       out["grid_pred_decoded"].append(dec)
       out["grid_pred_reg_decoded"].append(reg)
+    if pred_lengths is not None:
+      out["_lengths"] = torch.full((n,), tp, dtype=torch.int32, device=self.device) if lengths is None \
+          else unsort(lengths)
     return out
 
   # ------------------------------------------------------------------ CUDA-graph replay of forward()

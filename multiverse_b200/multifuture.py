@@ -1,0 +1,195 @@
+# coding=utf-8
+"""Batched multi-future inference: what code/multifuture_inference.py computes, many trajectories per forward.
+
+That script decodes every trajectory alone (N=1 per `sess.run`, :460-472), each to its own length, the longest of
+its ground-truth futures (`max_pred_lengths`, :229-231, :311).  `infer` concatenates the script's own N=1 feeds into
+batches and decodes each batch with ConvRNNEngine.forward(pred_lengths=...), whose rows equal their batch-1 decodes
+byte for byte, so its `output_data` and `beam_prob` equal the script's loop in values, dtypes and structure.  From the
+device it fetches the selected cells and their fp32 offsets (ops.gather_offsets), and the beam logits only when the
+probabilities are asked for; the points `centre + offset` are formed in float64 on the host, as the script does
+(:495-517).
+
+Command line (the user's copy of the script, imported through the drop-in path, provides the argument parser, the
+data loading and the feeds):
+
+  python -m multiverse_b200.multifuture <path to code/multifuture_inference.py> <its arguments> [--batch_size N]
+"""
+from __future__ import annotations
+
+import argparse
+import glob
+import importlib.util
+import os
+import pickle
+import sys
+
+import numpy as np
+
+DEFAULT_BATCH = 256
+
+
+def batch_feeds(model, feeds):
+  """One feed dict of N rows from N of the script's N=1 feed dicts, and their lengths int32 [N]: the rows
+  concatenated, each feed's frames appended to scene_feat and its obs_scene indices offset to match."""
+  cfg = model.config
+  scene, obs_scene, frames = [], [], 0
+  for fd in feeds:
+    sf = np.asarray(fd[model.scene_feat])
+    scene.append(sf)
+    obs_scene.append(np.asarray(fd[model.obs_scene], dtype=np.int32) + frames)
+    frames += sf.shape[0]
+  out = {model.scene_feat: np.concatenate(scene), model.obs_scene: np.concatenate(obs_scene)}
+  for j in range(len(cfg.scene_grids)):
+    if cfg.use_grids[j]:
+      out[model.grid_obs_labels[j]] = np.concatenate([np.asarray(fd[model.grid_obs_labels[j]]) for fd in feeds])
+      out[model.grid_obs_regress[j]] = np.concatenate([np.asarray(fd[model.grid_obs_regress[j]]) for fd in feeds])
+  lengths = np.array([int(np.asarray(fd[model.pred_length]).reshape(-1)[0]) for fd in feeds], dtype=np.int32)
+  return out, lengths
+
+
+def trajectories(ids, offs, length, centers, num_out, greedy, center_only):
+  """One trajectory's entry of the script's output_data (:475-520): ids int [K,T] (greedy: [1,T]), offs fp32 [K,T,2]
+  of the selected cells, centers fp64 [HW,2]."""
+  if center_only:
+    points = [[centers[ids[k, t]] for t in range(length)] for k in range(ids.shape[0])]
+  else:
+    pts = centers[ids[:, :length]] + offs[:, :length]
+    points = [[pts[k, t] for t in range(length)] for k in range(ids.shape[0])]
+  if greedy:
+    return [points[0] for _ in range(num_out)]      # one list, num_out times (:498)
+  return points[:num_out]
+
+
+def infer(model, per_trajectory_feeds, batch_size, args, traj_ids, with_prob=False):
+  """(output_data, beam_prob) of the script's loop (:460-523) for its N=1 feeds `per_trajectory_feeds`
+  (PredictionModelInference.get_feed_dict) of the trajectories `traj_ids`, decoded `batch_size` trajectories per
+  forward.  `args`: the script's arguments after add_grid.  beam_prob (the beam logits and log-probabilities,
+  --save_prob_file) is fetched only with `with_prob`; it is {} otherwise."""
+  import torch
+  from . import ops
+  cfg = model.config
+  assert sum(cfg.use_grids) == 1, "multifuture inference decodes one scale (multifuture_inference.py:395)"
+  if with_prob and not cfg.use_beam_search:
+    raise ValueError("beam probabilities need beam search (the script's --greedy has no beam outputs)")
+  gi = list(cfg.use_grids).index(True)
+  centers = np.asarray(args.scene_grid_centers[gi]).reshape([-1, 2])
+  greedy = not cfg.use_beam_search
+  eng = model._ensure_engine()
+  output_data, beam_prob = {}, {}
+  with torch.cuda.device(eng.device):
+    for b0 in range(0, len(per_trajectory_feeds), batch_size):
+      chunk = per_trajectory_feeds[b0:b0 + batch_size]
+      # a short last batch is padded to the batch size with length-1 rows: the engine keeps its buffers per batch
+      # size, and a second set at batch 512 would not fit next to the first
+      pad = batch_size - len(chunk) if b0 > 0 else 0
+      feed, lengths = batch_feeds(model, chunk + chunk[-1:] * pad)
+      lengths[len(chunk):] = 1
+      n = len(lengths)
+      out = eng.forward(model._device_feeds(feed), pred_lengths=lengths)
+      if greedy:
+        ids = out["grid_pred_decoded"][gi].reshape(n, int(lengths.max()), -1).argmax(-1).to(torch.int32)
+        ids = ids.unsqueeze(1).contiguous()
+      else:
+        ids = out["beam_outputs"][1]
+      offs = ops.gather_offsets(ids, out["_offs"][gi].contiguous(), out["_lengths"])
+      ids_h, offs_h = ids.cpu().numpy(), offs.cpu().numpy()
+      if with_prob:
+        logits_h, logprobs_h = out["beam_outputs"][0].cpu().numpy(), out["beam_outputs"][2].cpu().numpy()
+      for r in range(len(chunk)):
+        tid, length = traj_ids[b0 + r], int(lengths[r])
+        output_data[tid] = trajectories(ids_h[r], offs_h[r], length, centers, args.num_out, greedy, args.center_only)
+        if with_prob:
+          beam_prob[tid] = (np.ascontiguousarray(logits_h[r:r + 1, :, :length]), logprobs_h[r:r + 1].copy())
+  return output_data, beam_prob
+
+
+def load_script(path):
+  """The user's code/multifuture_inference.py as a module, its `pred_models` and `tensorflow` the drop-in's."""
+  from . import pred_models  # noqa: F401  (puts the drop-in directory first on sys.path)
+  here = os.path.dirname(os.path.abspath(path))
+  if here not in sys.path:
+    sys.path.insert(1, here)         # after the drop-in: the script's own pred_utils
+  spec = importlib.util.spec_from_file_location("multifuture_inference", path)
+  mod = importlib.util.module_from_spec(spec)
+  spec.loader.exec_module(mod)
+  return mod
+
+
+def model_config(args, tf):
+  """The model Namespace of multifuture_inference.py:419-452."""
+  return argparse.Namespace(
+      modelname="model", batch_size=1,
+      beam_size=args.num_out, use_beam_search=args.use_beam_search, diverse_beam=args.diverse_beam,
+      diverse_gamma=args.diverse_gamma, fix_num_timestep=args.fix_num_timestep,
+      use_teacher_forcing=False, is_train=False,
+      scene_h=args.scene_h, scene_w=args.scene_w, scene_class=args.scene_class,
+      use_soft_grid_class=args.use_soft_grid_class, use_single_decoder=args.use_single_decoder,
+      pred_len=12, emb_size=args.emb_size, enc_hidden_size=args.enc_hidden_size,
+      dec_hidden_size=args.dec_hidden_size, activation_func=tf.nn.tanh, scene_conv_kernel=args.scene_conv_kernel,
+      use_scene_enc=args.use_scene_enc, scene_conv_dim=args.scene_conv_dim, convlstm_kernel=args.convlstm_kernel,
+      use_gnn=args.use_gnn, keep_prob=1.0, scene_grid_strides=args.scene_grid_strides,
+      scene_grids=args.scene_grids, use_grids=args.use_grids)
+
+
+def prepare(script_path, script_argv, load_weights=True):
+  """The script's set-up (:389-461) through its own functions: returns (args, traj_ids, model, per-trajectory
+  feeds).  load_weights=False leaves the model's initial weights (no checkpoint read)."""
+  mod = load_script(script_path)
+  tf = sys.modules["tensorflow"]
+  args = mod.parser.parse_args(script_argv)
+  mod.add_grid(args)
+  args.use_beam_search = not args.greedy
+  assert sum(args.use_grids) == 1
+  traj_files = glob.glob(os.path.join(args.traj_path, "*.txt"))
+  traj_ids = [os.path.splitext(os.path.basename(one))[0] for one in traj_files]
+  gt_trajs = {}
+  for traj_id in traj_ids:
+    with open(os.path.join(args.multifuture_path, "%s.p" % traj_id), "rb") as f:
+      gt_trajs[traj_id] = pickle.load(f)
+  inputs = mod.get_inputs(args, traj_files, gt_trajs)
+  cfg = model_config(args, tf)
+  with tf.device("/gpu:%s" % args.gpuid):
+    model = mod.PredictionModelInference(cfg, cfg.modelname)
+  model.gpuid = args.gpuid
+  if load_weights:
+    with tf.Session() as sess:
+      mod.load_model_weights(args.model_path, sess, top_scope="person_pred")
+  feeds = [model.get_feed_dict(inputs, args, i) for i in range(len(traj_ids))]
+  return args, traj_ids, model, feeds
+
+
+def split_argv(argv):
+  """(script path, the script's arguments, batch size) from this module's command line."""
+  if not argv or argv[0].startswith("-"):
+    raise SystemExit("usage: python -m multiverse_b200.multifuture <multifuture_inference.py> <its arguments> "
+                     "[--batch_size N]")
+  rest, batch, i = [], DEFAULT_BATCH, 1
+  while i < len(argv):
+    a = argv[i]
+    if a == "--batch_size":
+      batch, i = int(argv[i + 1]), i + 2
+      continue
+    if a.startswith("--batch_size="):
+      batch = int(a.split("=", 1)[1])
+    else:
+      rest.append(a)
+    i += 1
+  if batch < 1:
+    raise SystemExit("--batch_size must be at least 1")
+  return argv[0], rest, batch
+
+
+def main(argv=None):
+  script, script_argv, batch = split_argv(sys.argv[1:] if argv is None else argv)
+  args, traj_ids, model, feeds = prepare(script, script_argv)
+  with_prob = args.save_prob_file is not None
+  output_data, beam_prob = infer(model, feeds, batch, args, traj_ids, with_prob=with_prob)
+  with open(args.output_file, "wb") as f:
+    pickle.dump(output_data, f)
+  if with_prob:
+    with open(args.save_prob_file, "wb") as f:
+      pickle.dump(beam_prob, f)
+
+
+if __name__ == "__main__":
+  main()

@@ -364,6 +364,16 @@ def beam_backtrace(step_ids, step_parents, step_logits, out_ids, out_logits):
             _p(out_logits), n, b, tp, v, _stream())
 
 
+def beam_backtrace_ragged(step_ids, step_parents, step_logits, lengths, out_ids, out_logits):
+  """beam_backtrace of rows that end at their own lengths int32 [N] (1..Tp): row n's trace starts at step
+  lengths[n] - 1, and its outputs at the steps after are zeros."""
+  tp, n, b = step_ids.shape
+  v = step_logits.shape[-1]
+  assert lengths.dtype == torch.int32 and lengths.numel() == n
+  _lib.call("mvb_beam_backtrace_ragged", _p(step_ids), _p(step_parents), _p(step_logits), _p(lengths), _p(out_ids),
+            _p(out_logits), n, b, tp, v, _stream())
+
+
 # --------------------------------------------------------------------------- training (BPTT) ops
 def cell_fwd_train(xh, packed, c_in, c_out, h32_out, xh_next, gates_out, h, w, ns, forget_bias=1.0):
   """cell_fwd that also stores the activated gates [R,1024] for the backward pass."""
@@ -497,6 +507,40 @@ def decode_trajectories(ids, offs, centers, out):
   n, k, tp = ids.shape
   _lib.call("mvb_decode_trajectories", _p(ids), _p(offs), _p(centers), _p(out), n, k, tp, offs.shape[2],
             _stream())
+
+
+def gather_offsets(ids, offs, lengths):
+  """ids int32 [N,K,Tp], offs fp32 [Tp,N,V,2], lengths int32 [N] -> fp32 [N,K,Tp,2]: the offsets of the selected
+  cells for t < lengths[n], zeros after."""
+  n, k, tp = ids.shape
+  assert offs.shape[:2] == (tp, n) and lengths.dtype == torch.int32 and lengths.numel() == n
+  out = torch.empty((n, k, tp, 2), dtype=torch.float32, device=ids.device)
+  _lib.call("mvb_gather_offsets", _p(ids), _p(offs), _p(lengths), _p(out), n, k, tp, offs.shape[2], _stream())
+  return out
+
+
+def operand_rows(xh, ns, h, w):
+  """The operand planes of the first ns sample rows of an alloc_xh buffer, as the kernels address them: a
+  [2, halo_rows(ns), cpad] view of its leading bytes (the cell kernels find the second plane halo_rows(ns) rows after
+  the first).  Halo cells and padding are zero in every such view: the plane boundary falls on a sample boundary."""
+  r, cpad = halo_rows(ns, h, w), xh.shape[2]
+  if r == xh.shape[1]:
+    return xh
+  v = xh.view(-1)[:2 * r * cpad].view(2, r, cpad)
+  if planes_of(xh) == PLANES_F16F8:
+    v.mvb_planes = PLANES_F16F8
+  return v
+
+
+def operand_shrink(xh, ns_from, ns_to, h, w):
+  """Re-lays operand planes written for ns_from sample rows (operand_rows(xh, ns_from)) for their first ns_to rows:
+  the second plane's first rows move to their place in operand_rows(xh, ns_to)."""
+  if ns_to == ns_from:
+    return
+  cpad = xh.shape[2]
+  r0, r1 = halo_rows(ns_from, h, w), halo_rows(ns_to, h, w)
+  flat = xh.view(-1)
+  flat[r1 * cpad:2 * r1 * cpad].copy_(flat[r0 * cpad:(r0 + r1) * cpad].clone())
 
 
 def adv_step(x, adv, grad, out, eps, step):
