@@ -209,6 +209,27 @@ int mvb_fg_count(const float* soft_labels, const int32_t* labels, int64_t rows, 
 int mvb_masked_huber_fwd_bwd(const float* reg, const float* target, float* dreg, const float* soft_labels,
                              const int32_t* labels, int64_t rows, int V, const double* fg_count, float reg_weight,
                              float* loss_out, void* stream);
+/* The same losses with their targets and label maps computed where they are read (f-1, training), so that no
+ * dense target or label map exists:  reg / dreg fp32 [Tp,N,H*W,2]; pred_traj fp64 [N,Tp,2] frame pixels; centers
+ * fp64 [H*W,2]; labels int32 [Tp,N] label cells.  The target of cell v of row (t, n) is
+ * float32(pred_traj[n,t] - centers[v]) computed in fp64 (as mvb_traj_to_grid); the label map of a row is that of
+ * --use_soft_grid_class with --soft_grid `soft_grid` (1-7: the 3x3 / 5x5 tables of pred_models.py:1085-1136 around the
+ * label cell, a negative label counted from the end), or the one-hot map of an in-range label for soft_grid 0.
+ * Each equals the dense entry point above fed the tensors the host builds from the same data, bit for bit in
+ * every element (the loss sums are accumulated across blocks in no fixed order, as there):
+ *   mvb_huber_traj_fwd_bwd        = the Huber half of mvb_loss_fwd_bwd (nreg = N*Tp*H*W*2 = Tp*N*V*2)
+ *   mvb_soft_ce_label_fwd_bwd     = mvb_soft_ce_fwd_bwd (rows = Tp*N, V = H*W; soft_grid 1-7)
+ *   mvb_fg_count_label            = mvb_fg_count (soft_grid 0-7; rows = Tp*N label cells)
+ *   mvb_masked_huber_traj_fwd_bwd = mvb_masked_huber_fwd_bwd (soft_grid 0-7) */
+int mvb_huber_traj_fwd_bwd(const float* reg, const double* pred_traj, const double* centers, float* dreg, int64_t N,
+                           int Tp, int V, float reg_weight, float* loss_out, void* stream);
+int mvb_soft_ce_label_fwd_bwd(const float* logits, const int32_t* labels, int soft_grid, float* dlogits, int64_t rows,
+                              int H, int W, float cls_weight, float* loss_out, void* stream);
+int mvb_fg_count_label(const int32_t* labels, int soft_grid, int64_t rows, int H, int W, double* fg_count,
+                       void* stream);
+int mvb_masked_huber_traj_fwd_bwd(const float* reg, const double* pred_traj, const double* centers, float* dreg,
+                                  const int32_t* labels, int soft_grid, int64_t N, int Tp, int H, int W,
+                                  const double* fg_count, float reg_weight, float* loss_out, void* stream);
 /* ---- a13: backward of the heads / embedding / attention / scene CNN (tf.gradients :1698) ----
  * hidden2grid: dWo[3,3,256,Pout] += ..., dh[NS*S,256] (=|+=) conv3x3^T(dout[NS,HW,Pout], Wo). */
 int mvb_head_bwd(const float* h32, const float* dout, const float* Wo, int Pout, float* dWo,
@@ -403,6 +424,11 @@ int mvb_beam_band_copy(const float* base_c, const float* base_h32, const int32_t
  *      labels int32 [NT] (cell of every point), regress fp32 [NT,H,W,2] (point - centre of every cell). */
 int mvb_traj_to_grid(const double* traj, const double* centers, double h_gap, double w_gap, int32_t* labels,
                      float* regress, int64_t NT, int H, int W, void* stream);
+/* The regression encoder's input from the trajectories (training): = mvb_nhwc_to_planes(src, ..., ch_off 0, C 2,
+ * bf16x2 planes, comp) of src[s,y,x] = float32(traj[s * traj_stride + (0,1)] - centers[y*W+x]) (fp64 difference),
+ * without src: traj fp64 points of NS rows, traj_stride >= 2 doubles apart (one time step of [N,T,2]). */
+int mvb_traj_to_planes(const double* traj, int64_t traj_stride, const double* centers, void* dst_planes,
+                       int64_t plane_stride, int cpad, int64_t NS, int H, int W, int comp, void* stream);
 
 /* ---- f-3 (next row): post-decode on the device (multifuture_inference.py:504-517,
  *      pred_utils.py:460-492): out[n,k,t] = centers[ids[n,k,t]] + offsets[t,n,ids[n,k,t]].

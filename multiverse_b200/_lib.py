@@ -48,6 +48,10 @@ SIGNATURES = {
     "mvb_soft_ce_fwd_bwd": [_vp, _vp, _vp, _i64, _i, _f, _vp, _vp],
     "mvb_fg_count": [_vp, _vp, _i64, _i, _vp, _vp],
     "mvb_masked_huber_fwd_bwd": [_vp, _vp, _vp, _vp, _vp, _i64, _i, _vp, _f, _vp, _vp],
+    "mvb_huber_traj_fwd_bwd": [_vp, _vp, _vp, _vp, _i64, _i, _i, _f, _vp, _vp],
+    "mvb_soft_ce_label_fwd_bwd": [_vp, _vp, _i, _vp, _i64, _i, _i, _f, _vp, _vp],
+    "mvb_fg_count_label": [_vp, _i, _i64, _i, _i, _vp, _vp],
+    "mvb_masked_huber_traj_fwd_bwd": [_vp, _vp, _vp, _vp, _vp, _i, _i64, _i, _i, _i, _vp, _f, _vp, _vp],
     "mvb_head_bwd": [_vp, _vp, _vp, _i, _vp, _vp, _i, _i64, _i, _i, _vp],
     "mvb_emb_bwd": [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _i, _i64, _i, _i, _vp],
     "mvb_gnn_attend_bwd": [_vp, _vp, _vp, _vp, _vp, _i, _vp, _i64, _i, _i, _vp],
@@ -69,6 +73,7 @@ SIGNATURES = {
     "mvb_emb_dense_fwd": [_vp, _vp, _vp, _i, _vp, _i64, _i, _i64, _i, _i, _i, _vp],
     "mvb_beam_step": [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _f, _vp],
     "mvb_traj_to_grid": [_vp, _vp, C.c_double, C.c_double, _vp, _vp, _i64, _i, _i, _vp],
+    "mvb_traj_to_planes": [_vp, _i64, _vp, _vp, _i64, _i, _i64, _i, _i, _i, _vp],
     "mvb_decode_trajectories": [_vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],
     "mvb_clip_update": [_vp, _vp, _vp, _vp, _i64, _i, _f, _f, _f, _f, _f, _f, _f, _vp],
     "mvb_adv_step": [_vp, _vp, _vp, _vp, _f, _f, _i64, _vp],

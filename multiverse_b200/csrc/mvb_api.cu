@@ -121,7 +121,7 @@ static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s)
 extern "C" {
 
 const char* mvb_last_error(void) { return get_error(); }
-int mvb_abi_version(void) { return 15; }
+int mvb_abi_version(void) { return 16; }
 int mvb_cell_last_variant(void) { return cell_last_variant(); }
 long long mvb_cell_variants_seen(int reset) { return (long long)cell_variants_seen(reset); }
 long long mvb_launch_count(void) { return g_launches; }
@@ -260,6 +260,24 @@ int mvb_masked_huber_fwd_bwd(const float* reg, const float* target, float* dreg,
   return masked_huber_fwd_bwd(reg, target, dreg, soft_labels, labels, rows, V, fg_count, reg_weight, loss_out,
                               S(stream));
 }
+int mvb_huber_traj_fwd_bwd(const float* reg, const double* pred_traj, const double* centers, float* dreg, int64_t N,
+                           int Tp, int V, float reg_weight, float* loss_out, void* stream) {
+  return huber_traj_fwd_bwd(reg, pred_traj, centers, dreg, N, Tp, V, reg_weight, loss_out, S(stream));
+}
+int mvb_soft_ce_label_fwd_bwd(const float* logits, const int32_t* labels, int soft_grid, float* dlogits, int64_t rows,
+                              int H, int W, float cls_weight, float* loss_out, void* stream) {
+  return soft_ce_label_fwd_bwd(logits, labels, soft_grid, dlogits, rows, H, W, cls_weight, loss_out, S(stream));
+}
+int mvb_fg_count_label(const int32_t* labels, int soft_grid, int64_t rows, int H, int W, double* fg_count,
+                       void* stream) {
+  return fg_count_label(labels, soft_grid, rows, H, W, fg_count, S(stream));
+}
+int mvb_masked_huber_traj_fwd_bwd(const float* reg, const double* pred_traj, const double* centers, float* dreg,
+                                  const int32_t* labels, int soft_grid, int64_t N, int Tp, int H, int W,
+                                  const double* fg_count, float reg_weight, float* loss_out, void* stream) {
+  return masked_huber_traj_fwd_bwd(reg, pred_traj, centers, dreg, labels, soft_grid, N, Tp, H, W, fg_count,
+                                   reg_weight, loss_out, S(stream));
+}
 int mvb_head_bwd(const float* h32, const float* dout, const float* Wo, int Pout, float* dWo,
                  float* dh, int accumulate_dh, int64_t NS, int H, int W, void* stream) {
   return head_bwd(h32, dout, Wo, Pout, dWo, dh, accumulate_dh, NS, H, W, S(stream));
@@ -303,6 +321,10 @@ int mvb_nhwc_to_planes(const float* src, void* dst_planes, int64_t plane_stride,
 int mvb_traj_to_grid(const double* traj, const double* centers, double h_gap, double w_gap, int32_t* labels,
                      float* regress, int64_t NT, int H, int W, void* stream) {
   return traj_to_grid(traj, centers, h_gap, w_gap, labels, regress, NT, H, W, S(stream));
+}
+int mvb_traj_to_planes(const double* traj, int64_t traj_stride, const double* centers, void* dst_planes,
+                       int64_t plane_stride, int cpad, int64_t NS, int H, int W, int comp, void* stream) {
+  return traj_to_planes(traj, traj_stride, centers, dst_planes, plane_stride, cpad, NS, H, W, comp, S(stream));
 }
 int mvb_nhwc_to_halo(const float* src, float* dst, int64_t NS, int H, int W, int C, void* stream) {
   return nhwc_halo_copy(src, dst, NS, H, W, C, 0, S(stream));

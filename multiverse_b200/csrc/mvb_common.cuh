@@ -68,6 +68,64 @@ __host__ __device__ inline Grid make_grid(int H, int W) {
 }
 
 // ----------------------------------------------------------------------------------
+// Inputs of the training step (SURVEY.md §8 row f-1), read either from dense fp32 tensors or computed where they are
+// consumed from the trajectories: kernels that take one of these as a template parameter run the same arithmetic on
+// the same values either way.
+// ----------------------------------------------------------------------------------
+// dense fp32 offsets: element i of [rows, V, 2], or cell i of [rows, V] as a pair
+struct DenseOffsets {
+  const float* p;
+  __device__ __forceinline__ float operator()(long long i) const { return p[i]; }
+  __device__ __forceinline__ float2 cell(long long i) const { return reinterpret_cast<const float2*>(p)[i]; }
+};
+// float32(point - centre) computed in double, as traj_to_grid and the host's float64 preprocessing cast to float32.
+// Row r of [rows, H*W, 2] is the point traj + (r % n) * row_stride + (r / n) * step_stride (in doubles); centers
+// fp64 [H*W, 2].
+struct TrajOffsets {
+  const double* traj;
+  const double* centers;
+  long long n, row_stride, step_stride;
+  int hw;
+  __device__ __forceinline__ float2 cell(long long i) const {
+    const long long r = i / hw;
+    const int v = (int)(i - r * hw);
+    const double* p = traj + (r % n) * row_stride + (r / n) * step_stride;
+    return make_float2((float)(p[0] - centers[2 * v]), (float)(p[1] - centers[2 * v + 1]));
+  }
+  __device__ __forceinline__ float operator()(long long i) const {
+    const float2 o = cell(i >> 1);
+    return (i & 1) ? o.y : o.x;
+  }
+};
+
+// Grid-class label of cell v for the label cell `lab` under --soft_grid `mode` (code/pred_models.py:1085-1136, as
+// pred_models._soft_labels builds the maps): the 3x3 (modes 1-6) or 5x5 (mode 7) kernel value at the cell's offset
+// from the label cell, 0 outside the kernel; a negative label indexes from the end, as numpy's m[cls] does.
+// mode 0: the one-hot map of a label in [0, H*W).  Values are float32 of the float64 table entries.
+__device__ __forceinline__ float grid_label(int lab, int v, int mode, int H, int W) {
+  const int hw = H * W;
+  if (mode == 0) return lab == v ? 1.f : 0.f;
+  if (lab < -hw || lab >= hw) return 0.f;
+  const int cell = lab < 0 ? lab + hw : lab;
+  const int r = mode == 7 ? 2 : 1;
+  const int dy = v / W - cell / W + r, dx = v % W - cell % W + r;
+  if (dy < 0 || dy > 2 * r || dx < 0 || dx > 2 * r) return 0.f;
+  if (mode == 7) {
+    if (dy == 2 && dx == 2) return (float)0.8;
+    return (dy >= 1 && dy <= 3 && dx >= 1 && dx <= 3) ? (float)0.0125 : (float)0.0625;
+  }
+  const bool centre = dy == 1 && dx == 1;
+  switch (mode) {
+    case 1: return centre ? (float)1.0 : (float)0.1;
+    case 2: return centre ? (float)1.0 : (float)0.01;
+    case 3: return centre ? (float)1.0 : (float)0.05;
+    case 4: return centre ? (float)0.9 : (float)0.0125;
+    case 5: return centre ? (float)0.6 : (float)0.05;
+    default: return centre ? (float)0.2 : (float)0.1;
+  }
+}
+
+// ----------------------------------------------------------------------------------
 // "bf16x2" operand format (planes code kBf16Planes): v = p0 + p1 + O(2^-18 |v|), both planes bf16; the product
 // of two such operands is accumulated as a0*b0 + a0*b1 + a1*b0 (a1*b1, 2^-18 of the result, is dropped).
 // A plane tensor is [2][rows][cpad] bf16.

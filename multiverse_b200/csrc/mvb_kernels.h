@@ -46,6 +46,8 @@ int nhwc_to_planes(const float* src, void* dst_planes, long long plane_stride, i
                    long long NS, int H, int W, int C, int P, int comp, cudaStream_t stream);
 int traj_to_grid(const double* traj, const double* centers, double h_gap, double w_gap, int* labels,
                  float* regress, long long NT, int H, int W, cudaStream_t stream);
+int traj_to_planes(const double* traj, long long traj_stride, const double* centers, void* dst_planes,
+                   long long plane_stride, int cpad, long long NS, int H, int W, int comp, cudaStream_t stream);
 int nhwc_halo_copy(const float* src, float* dst, long long NS, int H, int W, int C, int to_nhwc,
                    cudaStream_t stream);
 int enc_class_input(const float* scene_conv, const int* frame_idx, const int* label,
@@ -126,6 +128,14 @@ int fg_count(const float* soft, const int* labels, long long rows, int V, double
 int masked_huber_fwd_bwd(const float* reg, const float* target, float* dreg, const float* soft, const int* labels,
                          long long rows, int V, const double* count, float reg_scale, float* loss_out,
                          cudaStream_t stream);
+int huber_traj_fwd_bwd(const float* reg, const double* pred_traj, const double* centers, float* dreg, long long N,
+                       int Tp, int V, float reg_scale, float* loss_out, cudaStream_t stream);
+int soft_ce_label_fwd_bwd(const float* logits, const int* labels, int mode, float* dlogits, long long rows, int H,
+                          int W, float cls_scale, float* loss_out, cudaStream_t stream);
+int fg_count_label(const int* labels, int mode, long long rows, int H, int W, double* count, cudaStream_t stream);
+int masked_huber_traj_fwd_bwd(const float* reg, const double* pred_traj, const double* centers, float* dreg,
+                              const int* labels, int mode, long long N, int Tp, int H, int W, const double* count,
+                              float reg_scale, float* loss_out, cudaStream_t stream);
 int head_bwd(const float* h32, const float* dout, const float* Wo, int Pout, float* dWo, float* dh,
              int accumulate_dh, long long NS, int H, int W, cudaStream_t stream);
 int emb_bwd(const float* dxh, int cpad, const int* ids, const float* in_map, const float* We,

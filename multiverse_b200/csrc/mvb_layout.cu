@@ -7,8 +7,8 @@
 namespace mvb {
 
 // One thread per (pixel, channel); channel fastest so reads and writes coalesce.  FMT = 1: f16f8 operand format.
-template <int FMT>
-__global__ void nhwc_to_planes_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst,
+template <int FMT, class Src>
+__global__ void nhwc_to_planes_kernel(const Src src, __nv_bfloat16* __restrict__ dst,
                                       long long plane_stride, int cpad, int ch_off, long long NS,
                                       Grid g, int C, int comp) {
   const long long total = NS * g.H * g.W * C;
@@ -21,7 +21,7 @@ __global__ void nhwc_to_planes_kernel(const float* __restrict__ src, __nv_bfloat
     const int y = (int)(t % g.H);
     const long long s = t / g.H;
     const long long row = s * g.S + (long long)y * g.Wp + x;
-    const float v = src[i];
+    const float v = src(i);
     if (FMT) {      // f16f8 operand format (mvb_common.cuh)
       store_f16f8(dst, plane_stride, row, ch_off + c, cpad, v);
       continue;
@@ -159,8 +159,28 @@ int nhwc_to_planes(const float* src, void* dst_planes, long long plane_stride, i
   const int threads = 256;
   const int blocks = (int)((total + threads - 1) / threads < sm_count() * 16 ? (total + threads - 1) / threads : sm_count() * 16);
   __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst_planes);
-  if (P == kPlanesF16F8) nhwc_to_planes_kernel<1><<<blocks, threads, 0, stream>>>(src, d, plane_stride, cpad, ch_off, NS, g, C, 0);
-  else nhwc_to_planes_kernel<0><<<blocks, threads, 0, stream>>>(src, d, plane_stride, cpad, ch_off, NS, g, C, comp);
+  const DenseOffsets s{src};
+  if (P == kPlanesF16F8) nhwc_to_planes_kernel<1><<<blocks, threads, 0, stream>>>(s, d, plane_stride, cpad, ch_off, NS, g, C, 0);
+  else nhwc_to_planes_kernel<0><<<blocks, threads, 0, stream>>>(s, d, plane_stride, cpad, ch_off, NS, g, C, comp);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
+// nhwc_to_planes of the offsets float32(traj[s] - centre) [NS,H,W,2] into channels [0, 2) of the bf16x2 planes (and
+// the compensation channels [2, 8) under comp), computed in the kernel instead of read from a dense tensor: the
+// regression encoder's input straight from the observed trajectories (point s at traj + s * traj_stride doubles).
+int traj_to_planes(const double* traj, long long traj_stride, const double* centers, void* dst_planes,
+                   long long plane_stride, int cpad, long long NS, int H, int W, int comp, cudaStream_t stream) {
+  MVB_REQUIRE(traj && centers && dst_planes && NS > 0 && H > 0 && W > 0 && traj_stride >= 2 &&
+              (comp ? 8 : 2) <= cpad - kHidden, "traj_to_planes: bad args");
+  const Grid g = make_grid(H, W);
+  const long long total = NS * H * W * 2;
+  const int threads = 256;
+  const int blocks = (int)((total + threads - 1) / threads < sm_count() * 16 ? (total + threads - 1) / threads : sm_count() * 16);
+  const TrajOffsets s{traj, centers, NS, traj_stride, 0, H * W};
+  nhwc_to_planes_kernel<0><<<blocks, threads, 0, stream>>>(s, reinterpret_cast<__nv_bfloat16*>(dst_planes),
+                                                           plane_stride, cpad, 0, NS, g, 2, comp);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;

@@ -4,6 +4,8 @@
 //   soft_ce_fwd_bwd     the --use_soft_grid_class CE (:986-989) against dense label maps
 //   fg_count, masked_huber_fwd_bwd
 //                       the --mask_grid_regression Huber (:999-1018): over the cells whose label is > 0 only
+//   huber_traj_fwd_bwd, soft_ce_label_fwd_bwd, fg_count_label, masked_huber_traj_fwd_bwd
+//                       the same losses with targets and label maps computed from the trajectories and label cells
 //   head_bwd            hidden2grid (:925-959): dWo, dh
 //   emb_onehot_bwd      grid_emb on a one-hot input (:442-446): dWe, dbe (no input gradient)
 //   emb_dense_bwd       grid_emb on the 2-channel offset map: dWe, dbe, d(input)
@@ -63,14 +65,15 @@ ce_loss_kernel(const float* __restrict__ logits, const int* __restrict__ labels,
   if (threadIdx.x == 0) atomicAdd(loss_sum, lab_ok ? (logf(s) + m - lg[lab]) * scale : NAN);
 }
 
+template <class Target>
 __global__ void __launch_bounds__(256)
-huber_loss_kernel(const float* __restrict__ pred, const float* __restrict__ target,
+huber_loss_kernel(const float* __restrict__ pred, const Target target,
                   float* __restrict__ dpred, float* __restrict__ loss_sum, long long n, float scale) {
   __shared__ float red[8];
   float acc = 0.f;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x) {
-    const float e = pred[i] - target[i];
+    const float e = pred[i] - target(i);
     const float a = fabsf(e);
     acc += (a <= 1.f) ? 0.5f * e * e : a - 0.5f;
     dpred[i] = fminf(fmaxf(e, -1.f), 1.f) * scale;
@@ -81,15 +84,27 @@ huber_loss_kernel(const float* __restrict__ pred, const float* __restrict__ targ
 
 // one CTA per (n,t) row: softmax_cross_entropy_with_logits against a dense label row y[V]:
 //   loss = sum_v y_v (lse - l_v),  grad = (sum(y) softmax - y) * scale
-// (the soft maps of :1085-1136 do not sum to one, and lose mass where the kernel is clipped at the border)
+// (the soft maps of :1085-1136 do not sum to one, and lose mass where the kernel is clipped at the border).
+// y(r, v): a dense map (DenseMaps) or the rule of grid_label (LabelMaps)
+struct DenseMaps {
+  const float* y;
+  int V;
+  __device__ __forceinline__ float operator()(long long r, int v) const { return y[r * V + v]; }
+};
+struct LabelMaps {
+  const int* labels;
+  int mode, H, W;
+  __device__ __forceinline__ float operator()(long long r, int v) const { return grid_label(labels[r], v, mode, H, W); }
+};
+
+template <class Maps>
 __global__ void __launch_bounds__(256)
-soft_ce_loss_kernel(const float* __restrict__ logits, const float* __restrict__ labels,
+soft_ce_loss_kernel(const float* __restrict__ logits, const Maps y,
                     float* __restrict__ dlogits, float* __restrict__ loss_sum, int V, float scale) {
   __shared__ float red[8];
   __shared__ float bc[3];
   const long long r = blockIdx.x;
   const float* lg = logits + r * V;
-  const float* y = labels + r * V;
   float m = -INFINITY;
   for (int v = threadIdx.x; v < V; v += blockDim.x) m = fmaxf(m, lg[v]);
   m = warp_max(m);
@@ -107,7 +122,7 @@ soft_ce_loss_kernel(const float* __restrict__ logits, const float* __restrict__ 
   const float lse = logf(s) + m;
   float sy = 0.f, l = 0.f;
   for (int v = threadIdx.x; v < V; v += blockDim.x) {
-    const float yv = y[v];
+    const float yv = y(r, v);
     sy += yv;
     l = fmaf(yv, lse - lg[v], l);
   }
@@ -118,19 +133,43 @@ soft_ce_loss_kernel(const float* __restrict__ logits, const float* __restrict__ 
   sy = bc[2];
   const float inv = 1.0f / s;
   for (int v = threadIdx.x; v < V; v += blockDim.x)
-    dlogits[r * V + v] = (sy * (expf(lg[v] - m) * inv) - y[v]) * scale;
+    dlogits[r * V + v] = (sy * (expf(lg[v] - m) * inv) - y(r, v)) * scale;
   if (threadIdx.x == 0) atomicAdd(loss_sum, l * scale);
 }
 
-// foreground of the masked regression loss: cells with label > 0 (dense maps) or the label cell of each row
-// (tf.one_hot of an in-range sparse label); count += their number
+// foreground of the masked regression loss: cells with label > 0 (dense maps, or the maps of grid_label) or the
+// label cell of each row (tf.one_hot of an in-range sparse label).  fg(i) over the cells [rows, V] of the maps
+struct SoftFg {
+  const float* soft;
+  __device__ __forceinline__ bool operator()(long long i) const { return soft[i] > 0.f; }
+};
+struct SparseFg {
+  const int* labels;
+  int V;
+  __device__ __forceinline__ bool operator()(long long i) const { return labels[i / V] == (int)(i % V); }
+};
+struct LabelFg {
+  const int* labels;
+  int mode, H, W;
+  __device__ __forceinline__ bool operator()(long long i) const {
+    const int hw = H * W;
+    return grid_label(labels[i / hw], (int)(i % hw), mode, H, W) > 0.f;
+  }
+};
+// ... or over the rows [rows] of sparse labels
+struct RowFg {
+  const int* labels;
+  int V;
+  __device__ __forceinline__ bool operator()(long long i) const { return labels[i] >= 0 && labels[i] < V; }
+};
+
+// count += the number of i in [0, n) with fg(i)
+template <class Fg>
 __global__ void __launch_bounds__(256)
-fg_count_kernel(const float* __restrict__ soft, const int* __restrict__ labels, long long rows, int V,
-                double* __restrict__ count) {
-  const long long n = soft ? rows * V : rows;
+fg_count_kernel(const Fg fg, long long n, double* __restrict__ count) {
   unsigned c = 0;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    c += soft ? (soft[i] > 0.f) : (labels[i] >= 0 && labels[i] < V);
+    c += fg(i);
   c = __reduce_add_sync(0xffffffffu, c);
   if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, (double)c);       // integers: exact up to 2^53
 }
@@ -138,21 +177,19 @@ fg_count_kernel(const float* __restrict__ soft, const int* __restrict__ labels, 
 // Huber(delta=1) over the foreground cells only (tf.where + tf.gather, Reduction.MEAN over the 2K gathered
 // elements, div_no_nan: 0 when K = 0); dpred = 0 off the foreground.  K is read from the device: the count
 // of the whole batch, which a micro-batch may be only a part of.
+template <class Target, class Fg>
 __global__ void __launch_bounds__(256)
-masked_huber_kernel(const float2* __restrict__ pred, const float2* __restrict__ target, float2* __restrict__ dpred,
-                    const float* __restrict__ soft, const int* __restrict__ labels,
-                    const double* __restrict__ fg_count, float* __restrict__ loss_sum, long long cells,
-                    int V, float weight) {
+masked_huber_kernel(const float2* __restrict__ pred, const Target target, float2* __restrict__ dpred, const Fg is_fg,
+                    const double* __restrict__ fg_count, float* __restrict__ loss_sum, long long cells, float weight) {
   __shared__ float red[8];
   const double K = *fg_count;
   const float scale = K > 0.0 ? (float)(weight / (2.0 * K)) : 0.f;
   float acc = 0.f;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < cells;
        i += (long long)gridDim.x * blockDim.x) {
-    const bool fg = soft ? soft[i] > 0.f : labels[i / V] == (int)(i % V);
     float2 d = make_float2(0.f, 0.f);
-    if (fg) {
-      const float2 p = pred[i], t = target[i];
+    if (is_fg(i)) {
+      const float2 p = pred[i], t = target.cell(i);
       const float e0 = p.x - t.x, e1 = p.y - t.y, a0 = fabsf(e0), a1 = fabsf(e1);
       acc += ((a0 <= 1.f) ? 0.5f * e0 * e0 : a0 - 0.5f) + ((a1 <= 1.f) ? 0.5f * e1 * e1 : a1 - 0.5f);
       d = make_float2(fminf(fmaxf(e0, -1.f), 1.f) * scale, fminf(fmaxf(e1, -1.f), 1.f) * scale);
@@ -648,7 +685,8 @@ int loss_fwd_bwd(const float* logits, const int* labels, float* dlogits, long lo
   }
   if (reg) {
     MVB_REQUIRE(target && dreg && nreg > 0, "loss_fwd_bwd: bad Huber args");
-    huber_loss_kernel<<<grid_for(nreg, 256), 256, 0, stream>>>(reg, target, dreg, loss_out + 1, nreg, reg_scale / (float)nreg);
+    huber_loss_kernel<<<grid_for(nreg, 256), 256, 0, stream>>>(reg, DenseOffsets{target}, dreg, loss_out + 1, nreg,
+                                                               reg_scale / (float)nreg);
     MVB_CHECK_CUDA(cudaGetLastError());
     count_launch(1);
   }
@@ -658,7 +696,8 @@ int loss_fwd_bwd(const float* logits, const int* labels, float* dlogits, long lo
 int soft_ce_fwd_bwd(const float* logits, const float* labels, float* dlogits, long long rows, int V, float cls_scale,
                     float* loss_out, cudaStream_t stream) {
   MVB_REQUIRE(logits && labels && dlogits && loss_out && rows > 0 && V > 0, "soft_ce_fwd_bwd: bad args");
-  soft_ce_loss_kernel<<<(unsigned)rows, 256, 0, stream>>>(logits, labels, dlogits, loss_out, V, cls_scale / (float)rows);
+  soft_ce_loss_kernel<<<(unsigned)rows, 256, 0, stream>>>(logits, DenseMaps{labels, V}, dlogits, loss_out, V,
+                                                           cls_scale / (float)rows);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;
@@ -666,8 +705,62 @@ int soft_ce_fwd_bwd(const float* logits, const float* labels, float* dlogits, lo
 
 int fg_count(const float* soft, const int* labels, long long rows, int V, double* count, cudaStream_t stream) {
   MVB_REQUIRE((soft || labels) && count && rows > 0 && V > 0, "fg_count: bad args");
-  fg_count_kernel<<<grid_for(soft ? rows * V : rows, 256), 256, 0, stream>>>(
-      soft, soft ? nullptr : labels, rows, V, count);
+  if (soft) fg_count_kernel<<<grid_for(rows * V, 256), 256, 0, stream>>>(SoftFg{soft}, rows * V, count);
+  else fg_count_kernel<<<grid_for(rows, 256), 256, 0, stream>>>(RowFg{labels, V}, rows, count);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
+// ---- the same losses with their targets and label maps computed from the trajectories and the label cells
+// (SURVEY.md §8 row f-1): reg fp32 [Tp,N,H*W,2]; pred_traj fp64 [N,Tp,2]; centers fp64 [H*W,2]; labels int32 [Tp,N];
+// mode: --soft_grid 1-7, or 0 for the sparse labels
+static inline TrajOffsets pred_offsets(const double* traj, const double* centers, long long N, int Tp, int hw) {
+  return TrajOffsets{traj, centers, N, 2LL * Tp, 2, hw};
+}
+
+int huber_traj_fwd_bwd(const float* reg, const double* pred_traj, const double* centers, float* dreg, long long N,
+                       int Tp, int V, float reg_scale, float* loss_out, cudaStream_t stream) {
+  MVB_REQUIRE(reg && pred_traj && centers && dreg && loss_out && N > 0 && Tp > 0 && V > 0,
+              "huber_traj_fwd_bwd: bad args");
+  const long long nreg = N * Tp * V * 2;
+  huber_loss_kernel<<<grid_for(nreg, 256), 256, 0, stream>>>(reg, pred_offsets(pred_traj, centers, N, Tp, V), dreg,
+                                                             loss_out + 1, nreg, reg_scale / (float)nreg);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
+int soft_ce_label_fwd_bwd(const float* logits, const int* labels, int mode, float* dlogits, long long rows, int H,
+                          int W, float cls_scale, float* loss_out, cudaStream_t stream) {
+  MVB_REQUIRE(logits && labels && dlogits && loss_out && rows > 0 && H > 0 && W > 0 && mode >= 1 && mode <= 7,
+              "soft_ce_label_fwd_bwd: bad args (mode %d)", mode);
+  soft_ce_loss_kernel<<<(unsigned)rows, 256, 0, stream>>>(logits, LabelMaps{labels, mode, H, W}, dlogits, loss_out,
+                                                           H * W, cls_scale / (float)rows);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
+int fg_count_label(const int* labels, int mode, long long rows, int H, int W, double* count, cudaStream_t stream) {
+  MVB_REQUIRE(labels && count && rows > 0 && H > 0 && W > 0 && mode >= 0 && mode <= 7,
+              "fg_count_label: bad args (mode %d)", mode);
+  const long long cells = rows * H * W;
+  fg_count_kernel<<<grid_for(cells, 256), 256, 0, stream>>>(LabelFg{labels, mode, H, W}, cells, count);
+  MVB_CHECK_CUDA(cudaGetLastError());
+  count_launch(1);
+  return MVB_OK;
+}
+
+int masked_huber_traj_fwd_bwd(const float* reg, const double* pred_traj, const double* centers, float* dreg,
+                              const int* labels, int mode, long long N, int Tp, int H, int W, const double* count,
+                              float reg_scale, float* loss_out, cudaStream_t stream) {
+  MVB_REQUIRE(reg && pred_traj && centers && dreg && labels && count && loss_out && N > 0 && Tp > 0 && H > 0 &&
+              W > 0 && mode >= 0 && mode <= 7, "masked_huber_traj_fwd_bwd: bad args (mode %d)", mode);
+  const long long cells = N * Tp * H * W;
+  masked_huber_kernel<<<grid_for(cells, 256), 256, 0, stream>>>(
+      reinterpret_cast<const float2*>(reg), pred_offsets(pred_traj, centers, N, Tp, H * W),
+      reinterpret_cast<float2*>(dreg), LabelFg{labels, mode, H, W}, count, loss_out + 1, cells, reg_scale);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;
@@ -679,10 +772,15 @@ int masked_huber_fwd_bwd(const float* reg, const float* target, float* dreg, con
   MVB_REQUIRE(reg && target && dreg && (soft || labels) && count && loss_out && rows > 0 && V > 0,
               "masked_huber_fwd_bwd: bad args");
   const long long cells = rows * V;
-  masked_huber_kernel<<<grid_for(cells, 256), 256, 0, stream>>>(
-      reinterpret_cast<const float2*>(reg), reinterpret_cast<const float2*>(target), reinterpret_cast<float2*>(dreg),
-      soft, soft ? nullptr : labels, count, loss_out + 1, cells, V,
-      reg_scale);
+  const DenseOffsets tg{target};
+  float2* d = reinterpret_cast<float2*>(dreg);
+  if (soft)
+    masked_huber_kernel<<<grid_for(cells, 256), 256, 0, stream>>>(reinterpret_cast<const float2*>(reg), tg, d,
+                                                                  SoftFg{soft}, count, loss_out + 1, cells, reg_scale);
+  else
+    masked_huber_kernel<<<grid_for(cells, 256), 256, 0, stream>>>(reinterpret_cast<const float2*>(reg), tg, d,
+                                                                  SparseFg{labels, V}, count, loss_out + 1, cells,
+                                                                  reg_scale);
   MVB_CHECK_CUDA(cudaGetLastError());
   count_launch(1);
   return MVB_OK;

@@ -235,6 +235,15 @@ def nhwc_to_planes(src, xh, ch_off, h, w, comp=False):
             c, planes_of(xh), int(comp), _stream())
 
 
+def traj_to_planes(traj, t, centers, xh, h, w, comp=False):
+  """nhwc_to_planes(float32(traj[:, t] - centers), xh, 0, h, w, comp) without the dense offsets: traj fp64 [N,T,2],
+  centers fp64 [h,w,2], xh bf16x2 planes."""
+  assert planes_of(xh) == PLANES_BF16X2 and 0 <= t < traj.shape[1]
+  _, c = _traj_args(traj, centers, h, w)
+  _lib.call("mvb_traj_to_planes", C.c_void_p(traj[:, t].data_ptr()), traj.stride(0), c, _p(xh), xh.stride(0),
+            xh.shape[2], traj.shape[0], h, w, int(comp), _stream())
+
+
 def nhwc_to_halo(src, dst, h, w):
   _lib.call("mvb_nhwc_to_halo", _p(src), _p(dst), src.shape[0], h, w, src.shape[-1], _stream())
 
@@ -452,6 +461,46 @@ def masked_huber_fwd_bwd(reg, target, dreg, labels, count, reg_weight, loss_out)
   assert count.dtype == torch.float64 and (labels.numel() == rows * v if soft else labels.numel() == rows)
   _lib.call("mvb_masked_huber_fwd_bwd", _p(reg), _p(target), _p(dreg), _p(labels) if soft else None,
             None if soft else _p(labels), rows, v, _p(count), float(reg_weight), _p(loss_out), _stream())
+
+
+def _traj_args(traj, centers, h, w):
+  assert traj.dtype == torch.float64 and traj.shape[-1] == 2 and traj.is_contiguous()
+  assert centers.dtype == torch.float64 and centers.numel() == 2 * h * w
+  return _p(traj), _p(centers)
+
+
+def huber_traj_fwd_bwd(reg, pred_traj, centers, dreg, reg_weight, loss_out):
+  """The Huber half of loss_fwd_bwd against the targets float32(pred_traj[n,t] - centers[v]) (fp64 difference),
+  computed in the kernel: reg / dreg fp32 [Tp,N,V,2], pred_traj fp64 [N,Tp,2], centers fp64 [h,w,2]."""
+  tp, n, v = reg.shape[0], reg.shape[1], reg.shape[2]
+  assert tuple(pred_traj.shape) == (n, tp, 2)
+  traj, c = _traj_args(pred_traj, centers, 1, v)
+  _lib.call("mvb_huber_traj_fwd_bwd", _p(reg), traj, c, _p(dreg), n, tp, v, float(reg_weight), _p(loss_out), _stream())
+
+
+def soft_ce_label_fwd_bwd(logits, labels, soft_grid, h, w, dlogits, cls_weight, loss_out):
+  """soft_ce_fwd_bwd against the --soft_grid label maps of the int32 label cells `labels` [...] (one per logits row),
+  computed in the kernel."""
+  assert labels.dtype == torch.int32 and labels.numel() * h * w == logits.numel()
+  _lib.call("mvb_soft_ce_label_fwd_bwd", _p(logits), _p(labels), int(soft_grid), _p(dlogits), labels.numel(), h, w,
+            float(cls_weight), _p(loss_out), _stream())
+
+
+def fg_count_label(labels, soft_grid, h, w, count):
+  """fg_count of the label maps of the int32 label cells `labels` under --soft_grid (0: the sparse labels)."""
+  assert labels.dtype == torch.int32
+  _lib.call("mvb_fg_count_label", _p(labels), int(soft_grid), labels.numel(), h, w, _p(count), _stream())
+
+
+def masked_huber_traj_fwd_bwd(reg, pred_traj, centers, dreg, labels, soft_grid, h, w, count, reg_weight, loss_out):
+  """masked_huber_fwd_bwd with the targets of huber_traj_fwd_bwd and the foreground of the label maps of
+  fg_count_label; labels int32 [Tp,N]."""
+  tp, n = reg.shape[0], reg.shape[1]
+  assert tuple(pred_traj.shape) == (n, tp, 2) and reg.shape[2] == h * w and tuple(labels.shape) == (tp, n)
+  assert count.dtype == torch.float64 and labels.dtype == torch.int32
+  traj, c = _traj_args(pred_traj, centers, h, w)
+  _lib.call("mvb_masked_huber_traj_fwd_bwd", _p(reg), traj, c, _p(dreg), _p(labels), int(soft_grid), n, tp, h, w,
+            _p(count), float(reg_weight), _p(loss_out), _stream())
 
 
 def head_bwd(h32, dout, Wo, dWo, dh, accumulate_dh, h, w, ns):

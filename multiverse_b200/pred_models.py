@@ -118,6 +118,10 @@ class Model(object):
     # bus instead of 41 KB per trajectory and scale.  get_feed_dict uses them when the batch carries both.
     self.obs_traj = ph("obs_traj")
     self.grid_centers = [ph("grid_centers", i) for i, _ in enumerate(config.scene_grids)]
+    # Training batches also feed the future trajectories [N,Tp,2] float64 and int32 label cells in grid_pred_labels_T,
+    # instead of grid_obs_regress, grid_pred_regress and (--use_soft_grid_class) the soft label maps: the training
+    # step's kernels compute the offsets, regression targets and label maps where they read them.
+    self.pred_traj = ph("pred_traj")
     # SimAug's Model (SimAug/code/pred_models.py:225-267): the other camera views of every sample
     if getattr(config, "multiview_train", False):
       self.obs_scene_extra = ph("obs_scene_extra")
@@ -212,10 +216,13 @@ class Model(object):
     self.loss = Handle(self, "fetch", "loss")
 
   # ---------------------------------------------------------------- feeds
-  def get_feed_dict(self, batch, is_train=False):
+  def get_feed_dict(self, batch, is_train=False, train_traj=False):
     """code/pred_models.py:1042-1194, vectorised.  `batch` is a pred_utils.Dataset whose
     `.data` holds obs_grid_class / pred_grid_class [num_scale,T], obs/pred_grid_target_all_<j>
-    [T,h,w,2], batch_scene_feat [F,SH,SW,SC] and batch_obs_scene [[idx],...]."""
+    [T,h,w,2], batch_scene_feat [F,SH,SW,SC] and batch_obs_scene [[idx],...].
+    train_traj (Trainer.step): a training batch that carries its trajectories and grid centres is fed as those
+    (_train_traj_feeds) - no dense offset, target or soft label map is built; without it a training feed dict is
+    the reference's."""
     cfg = self.config
     N, T_in, T_pred = self.N, cfg.obs_len, cfg.pred_len
     data = batch.data
@@ -223,12 +230,17 @@ class Model(object):
           self.pred_length: np.full((N,), T_pred, dtype="int32"),
           self.is_train: is_train}
     n_have = len(data["obs_grid_class"])
+    traj = self._train_traj_feeds(batch, n_have) if is_train and train_traj else None
     for j, (h, w) in enumerate(cfg.scene_grids):
       labels = np.zeros((N, T_in), dtype="int32")
       if n_have:
         labels[:n_have] = np.stack([np.asarray(a)[j, :] for a in data["obs_grid_class"]])
       fd[self.grid_obs_labels[j]] = labels           # :1186-1191 (every scale, used or not)
       if not cfg.use_grids[j]:
+        continue
+      if traj is not None:
+        fd[self.grid_pred_labels_T[j]] = np.stack([np.asarray(a)[j, :] for a in data["pred_grid_class"]]).astype("int32")
+        fd[self.grid_centers[j]] = traj[2][j]
         continue
       obs_reg = np.zeros((N, T_in, h, w, 2), dtype="float32")
       obs_reg[:n_have] = np.stack(data["obs_grid_target_all_%d" % j])
@@ -280,8 +292,60 @@ class Model(object):
         fd[self.grid_pred_regress_extra[j]] = pred_reg
         fd[self.grid_obs_regress_extra[j]] = obs_reg
       fd[self.obs_scene_extra] = np.squeeze(data["batch_extra_obs_scene"])
+    if traj is not None:
+      fd[self.obs_traj], fd[self.pred_traj] = traj[0], traj[1]
     self._compact_grid_feeds(fd, batch, n_have, is_train)
     return fd
+
+  def _train_traj_feeds(self, batch, n_have):
+    """Row f-1 for training: (obs_traj [N,T,2], pred_traj [N,Tp,2], {scale: centres [h,w,2]}, all float64) when a
+    training batch can be fed as trajectories, else None and the batch keeps the dense feeds.  That needs a full batch
+    (pred_utils pads the last one with its last item; padded rows of a dense feed are zeros no trajectory gives),
+    data["obs_traj"] / data["pred_traj"] and shared["grid_center_<j>"] of every used scale (pred_utils.read_data puts
+    them there), label cells that index the grid under --use_soft_grid_class (as _soft_labels' numpy indexing needs),
+    and dense offsets that agree with float32(trajectory - centre) on 32 sampled cells per scale, observed and future,
+    as in _compact_grid_feeds.  SimAug's adversarial and multiview training keep the dense feeds."""
+    cfg = self.config
+    N, T, Tp = self.N, cfg.obs_len, cfg.pred_len
+    if not getattr(cfg, "device_grid_feeds", True) or n_have != N:
+      return None
+    if getattr(cfg, "multiview_train", False) or getattr(cfg, "adv_train", False):
+      return None
+    data, shared = batch.data, getattr(batch, "shared", None)
+    if shared is None or "obs_traj" not in data or "pred_traj" not in data:
+      return None
+    soft = bool(getattr(cfg, "use_soft_grid_class", False))
+    if soft and getattr(cfg, "soft_grid", None) not in range(1, 8):
+      return None
+    try:
+      obs = np.stack([np.asarray(t, dtype=np.float64) for t in data["obs_traj"]])[:, :T]
+      pred = np.stack([np.asarray(t, dtype=np.float64) for t in data["pred_traj"]])[:, :Tp]
+    except Exception:
+      return None
+    if obs.shape != (N, T, 2) or pred.shape != (N, Tp, 2):
+      return None
+    rng = np.random.default_rng(0)
+    centers = {}
+    for j, (h, w) in enumerate(cfg.scene_grids):
+      if not cfg.use_grids[j]:
+        continue
+      c = shared.get("grid_center_%d" % j)
+      if c is None or np.shape(c) != (h, w, 2):
+        return None
+      centers[j] = np.ascontiguousarray(c, dtype=np.float64)
+      cls = np.stack([np.asarray(a)[j, :] for a in data["pred_grid_class"]])
+      if soft and not ((cls >= -h * w) & (cls < h * w)).all():
+        return None
+      for key, tr, steps in (("obs_grid_target_all_%d" % j, obs, T), ("pred_grid_target_all_%d" % j, pred, Tp)):
+        ii, tt = rng.integers(0, N, 32), rng.integers(0, steps, 32)
+        yy, xx = rng.integers(0, h, 32), rng.integers(0, w, 32)
+        try:
+          dense = np.array([np.asarray(data[key][i][t, y, x], dtype=np.float32) for i, t, y, x in zip(ii, tt, yy, xx)])
+        except Exception:
+          return None
+        if not np.array_equal(dense, (tr[ii, tt] - centers[j][yy, xx]).astype(np.float32)):
+          return None
+    return obs, pred, centers
 
   def _compact_grid_feeds(self, fd, batch, n_have, is_train):
     """Row f-1: when the batch carries the observed trajectories and the grid centres the dense offsets were
@@ -289,7 +353,7 @@ class Model(object):
     instead of the dense [N,T,h,w,2] arrays; the engine regenerates the arrays on the device.  Guarded by a
     sampled consistency check - dense == float32(trajectory - centre) on 32 random cells per scale - so a batch
     whose dense targets were edited independently keeps the dense path.  config.device_grid_feeds=False turns it
-    off; training keeps the dense path (its loss also needs the dense prediction targets)."""
+    off.  Training batches are decided before any dense array is built (_train_traj_feeds)."""
     cfg = self.config
     if is_train or not getattr(cfg, "device_grid_feeds", True) or not n_have:
       return
@@ -347,7 +411,9 @@ class Model(object):
       self._stale = False
     return self._engine
 
-  def _device_feeds(self, feed):
+  def _device_feeds(self, feed, train_traj=False):
+    """The feeds of the engine on its device.  train_traj: a training feed of trajectories (obs_traj, pred_traj,
+    grid_centers): they go to the device as feeds["traj"] (TrainEngine.loss_and_grads) and no dense offset is built."""
     import torch
     eng = self._ensure_engine()
     dev = eng.device
@@ -361,7 +427,12 @@ class Model(object):
                grid_obs_labels=[None] * len(cfg.scene_grids),
                grid_obs_regress=[None] * len(cfg.scene_grids))
     regress = None
-    if self.obs_traj in feed:       # row f-1: dense offsets built on the device from the trajectories
+    if train_traj:
+      out["traj"] = dict(obs=up(feed[self.obs_traj], np.float64), pred=up(feed[self.pred_traj], np.float64),
+                         centers=[up(feed[self.grid_centers[i]], np.float64) if cfg.use_grids[i] else None
+                                  for i in range(len(cfg.scene_grids))],
+                         soft_grid=int(cfg.soft_grid) if getattr(cfg, "use_soft_grid_class", False) else 0)
+    elif self.obs_traj in feed:     # row f-1: dense offsets built on the device from the trajectories
       centers = [feed.get(self.grid_centers[i]) for i in range(len(cfg.scene_grids))]
       _, regress = eng.grid_feeds_from_traj(np.asarray(feed[self.obs_traj], dtype=np.float64), centers=centers)
     for i in range(len(cfg.scene_grids)):
@@ -371,7 +442,7 @@ class Model(object):
           out["grid_obs_regress"][i] = up(feed[self.grid_obs_regress[i]], np.float32)
         elif regress is not None:
           out["grid_obs_regress"][i] = regress[i]
-        else:
+        elif not train_traj:
           raise KeyError("feed neither grid_obs_regress[%d] nor obs_traj + grid_centers[%d]" % (i, i))
     return out
 
@@ -518,14 +589,17 @@ class Model(object):
       raise NotImplementedError("SimAug's model ignores --use_soft_grid_class; this combination is not implemented")
     eng = self._ensure_engine()
     dev = eng.device
-    feeds = self._device_feeds(feed)
+    train_traj = self.pred_traj in feed          # get_feed_dict's trajectory feeds (_train_traj_feeds)
+    feeds = self._device_feeds(feed, train_traj)
     up = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev, non_blocking=True)
     feeds["grid_pred_labels"] = [None] * len(cfg.scene_grids)
     feeds["grid_pred_regress"] = [None] * len(cfg.scene_grids)
     for i in range(len(cfg.scene_grids)):
       if cfg.use_grids[i]:
-        feeds["grid_pred_labels"][i] = up(feed[self.grid_pred_labels_T[i]], np.float32 if soft else np.int32)
-        feeds["grid_pred_regress"][i] = up(feed[self.grid_pred_regress[i]], np.float32)
+        feeds["grid_pred_labels"][i] = up(feed[self.grid_pred_labels_T[i]],
+                                          np.float32 if soft and not train_traj else np.int32)
+        if not train_traj:
+          feeds["grid_pred_regress"][i] = up(feed[self.grid_pred_regress[i]], np.float32)
     feeds = self._simaug_feeds(eng, feeds, feed)
     step = int(self.global_step.value)
     if apply:
@@ -721,7 +795,7 @@ class Trainer(object):
 
   def step(self, sess, batch):
     _, batch_data = batch
-    feed_dict = self.model.get_feed_dict(batch_data, is_train=True)
+    feed_dict = self.model.get_feed_dict(batch_data, is_train=True, train_traj=True)
     outputs = sess.run([self.loss, self.train_op, self.wd_loss, self.model.pred_grid_loss],
                        feed_dict=feed_dict)
     loss, train_op, wd_loss, pred_grid_loss = outputs

@@ -96,7 +96,8 @@ class TrainEngine(ConvRNNEngine):
     T, Tp = cfg.obs_len, cfg.pred_len
     labels_t = feeds["grid_obs_labels"][i].to(torch.int32).t().contiguous()
     obs_scene_t = feeds["obs_scene"].to(torch.int32).t().contiguous()
-    obs_reg_t = feeds["grid_obs_regress"][i].float().transpose(0, 1).contiguous()
+    tr = feeds.get("traj")
+    obs_reg_t = None if tr is not None else feeds["grid_obs_regress"][i].float().transpose(0, 1).contiguous()
     n = labels_t.shape[1]
     mix = feeds.get("mixup")
     labels2_t = mix["obs_labels2"][i].to(torch.int32).t().contiguous() if mix is not None else None
@@ -104,7 +105,7 @@ class TrainEngine(ConvRNNEngine):
     st = lambda tag, cnt: self._steps((tag, i, n), cnt, lambda: ops.alloc_state(n, h, w, dev))
     gt = lambda tag, cnt: self._steps((tag, i, n), cnt, lambda: torch.zeros((R, 4 * HID), device=dev))
     xs = lambda tag, cnt, cpad: self._steps((tag, i, n), cnt, lambda: ops.alloc_xh(n, h, w, cpad, P, dev))
-    S = dict(n=n, h=h, w=w, labels_t=labels_t, obs_scene_t=obs_scene_t, obs_reg_t=obs_reg_t)
+    S = dict(n=n, h=h, w=w, labels_t=labels_t, obs_scene_t=obs_scene_t)
     # ---- class encoder
     xh = xs("xh_ec", T, sw.enc_class.cpad); c = st("c_ec", T); g = gt("g_ec", T)
     h32_last = self._one(("h32_ec", i, n), lambda: ops.alloc_state(n, h, w, dev))
@@ -167,7 +168,10 @@ class TrainEngine(ConvRNNEngine):
     xh_dr = xs("xh_dr", Tp, sw.dec_reg.cpad)
     xh[0][:, :, sw.enc_reg.cxp:].zero_()
     for t in range(T):
-      ops.nhwc_to_planes(obs_reg_t[t], xh[t], 0, h, w, comp=sw.enc_reg.comp)
+      if tr is None:
+        ops.nhwc_to_planes(obs_reg_t[t], xh[t], 0, h, w, comp=sw.enc_reg.comp)
+      else:
+        ops.traj_to_planes(tr["obs"], t, tr["centers"][i], xh[t], h, w, comp=sw.enc_reg.comp)
       last = t == T - 1
       ops.cell_fwd_train(xh[t], sw.enc_reg, None if t == 0 else c[t - 1], c[t], None,
                          xh_dr[0] if last else xh[t + 1], g[t], h, w, n)
@@ -176,7 +180,16 @@ class TrainEngine(ConvRNNEngine):
     c = st("c_dr", Tp); g = gt("g_dr", Tp); h32 = st("h32_dr", Tp)
     offs = self._one(("offs", i, n), lambda: torch.empty((Tp, n, h * w, 2), device=dev))
     We, be = sw.emb_reg
-    ops.emb_dense_fwd(obs_reg_t[-1], We, be, xh_dr[0], h, w)
+    if tr is None:
+      obs_last = obs_reg_t[-1].reshape(n, h * w, 2)
+    else:
+      # the last observed offsets [n,HW,2]: the decoder's first input, and what emb_bwd reads for its weight gradient
+      obs_last = self._one(("obs_last", i, n), lambda: torch.empty((n, h * w, 2), device=dev))
+      scratch = self._one(("obs_last_cell", i, n), lambda: torch.empty((n,), dtype=torch.int32, device=dev))
+      vh, vw = getattr(cfg, "video_h", 1080), getattr(cfg, "video_w", 1920)
+      ops.traj_to_grid(tr["obs"][:, -1].contiguous(), tr["centers"][i], vh * 1.0 / h, vw * 1.0 / w, scratch, obs_last,
+                       h, w)
+    ops.emb_dense_fwd(obs_last, We, be, xh_dr[0], h, w)
     for t in range(Tp):
       c_prev = S["c_er"][T - 1] if t == 0 else c[t - 1]
       last = t == Tp - 1
@@ -184,7 +197,7 @@ class TrainEngine(ConvRNNEngine):
                          g[t], h, w, n)
       ops.head_reg_fwd(h32[t], sw.head_reg, offs[t], None if last else We, None if last else be,
                        None if last else xh_dr[t + 1], h, w, n, planes=P)
-    S.update(xh_dr=xh_dr, c_dr=c, g_dr=g, h32_dr=h32, offs=offs)
+    S.update(xh_dr=xh_dr, c_dr=c, g_dr=g, h32_dr=h32, offs=offs, obs_last=obs_last)
     return S
 
   # ------------------------------------------------------------------ backward helpers
@@ -218,17 +231,30 @@ class TrainEngine(ConvRNNEngine):
     dh = self._one(("dh", i, n), lambda: ops.alloc_state(n, h, w, dev))
     # ---- losses and their gradients (Model.build_loss :988-1027)
     lab_in = feeds["grid_pred_labels"][i]
-    soft = lab_in.dim() > 2                                                        # [N,Tp,h,w,1] label maps
+    tr = feeds.get("traj")         # trajectory feeds: targets and label maps are computed in the loss kernels
+    soft = tr is None and lab_in.dim() > 2                                         # [N,Tp,h,w,1] label maps
     if soft:
       lab = lab_in.float().reshape(n, Tp, h * w).transpose(0, 1).contiguous()   # [Tp,N,HW]
     else:
       lab = lab_in.to(torch.int32).t().contiguous()                              # [Tp,N]
-    tgt = feeds["grid_pred_regress"][i].float().transpose(0, 1).reshape(Tp, n, h * w, 2).contiguous()
+    tgt = None if tr is not None else \
+        feeds["grid_pred_regress"][i].float().transpose(0, 1).reshape(Tp, n, h * w, 2).contiguous()
     dlogits = self._one(("dlogits", i, n), lambda: torch.empty_like(S["logits"]))
     doffs = self._one(("doffs", i, n), lambda: torch.empty_like(S["offs"]))
     mix = S["mix"]
     assert mix is None or not (soft or fg is not None), "soft labels / masked regression with SimAug's mixup"
-    if mix is None and not soft and fg is None:
+    assert mix is None or tr is None, "SimAug's mixup keeps the dense feeds"
+    if tr is not None:
+      mode, pred, centers = tr["soft_grid"], tr["pred"], tr["centers"][i]
+      if mode:
+        ops.soft_ce_label_fwd_bwd(S["logits"], lab, mode, h, w, dlogits, cw, loss_out)
+      else:
+        ops.loss_fwd_bwd(S["logits"], lab, dlogits, cw, None, None, None, 0.0, loss_out)
+      if fg is not None:
+        ops.masked_huber_traj_fwd_bwd(S["offs"], pred, centers, doffs, lab, mode, h, w, fg[0], fg[1], loss_out)
+      else:
+        ops.huber_traj_fwd_bwd(S["offs"], pred, centers, doffs, rw, loss_out)
+    elif mix is None and not soft and fg is None:
       ops.loss_fwd_bwd(S["logits"], lab, dlogits, cw, S["offs"], tgt, doffs, rw, loss_out)
     elif mix is None:
       if soft:
@@ -312,7 +338,7 @@ class TrainEngine(ConvRNNEngine):
       c_prev = S["c_er"][T - 1] if t == 0 else S["c_dr"][t - 1]
       dxh, dc = self._cell_bwd(S, i, sw.dec_reg, cgr["dec_reg"], S["xh_dr"][t], S["g_dr"][t], c_prev,
                                S["c_dr"][t], dh, dc)
-      in_map = S["obs_reg_t"][-1].reshape(n, h * w, 2) if t == 0 else S["offs"][t - 1]
+      in_map = S["obs_last"] if t == 0 else S["offs"][t - 1]
       ops.emb_bwd(dxh, None, in_map, We, be, G[nm["emb_reg"][0]], G[nm["emb_reg"][1]],
                   None if t == 0 else doffs[t - 1], True, h, w, n)
       dh.copy_(dxh[:, sw.dec_reg.cxp:])
@@ -332,12 +358,17 @@ class TrainEngine(ConvRNNEngine):
   # ------------------------------------------------------------------ public
   def fg_counts(self, feeds):
     """Foreground size K of the masked regression loss per scale (fp64 [scales] on the device, no host sync): the
-    cells whose label is > 0 of the soft maps, or the in-range label cells of sparse labels."""
+    cells whose label is > 0 of the soft maps, or the in-range label cells of sparse labels.  With trajectory feeds
+    the soft maps are those of the label cells under feeds["traj"]["soft_grid"]."""
     cfg = self.cfg
     K = torch.zeros((len(cfg.scene_grids),), dtype=torch.float64, device=self.device)
+    tr = feeds.get("traj")
     for i, (h, w) in enumerate(cfg.scene_grids):
       if cfg.use_grids[i]:
         lab = feeds["grid_pred_labels"][i]
+        if tr is not None and tr["soft_grid"]:
+          ops.fg_count_label(lab.to(torch.int32).contiguous(), tr["soft_grid"], h, w, K[i:i + 1])
+          continue
         lab = lab.float().contiguous() if lab.dim() > 2 else lab.to(torch.int32).contiguous()
         ops.fg_count(lab, h * w, K[i:i + 1])
     return K
@@ -345,7 +376,11 @@ class TrainEngine(ConvRNNEngine):
   def loss_and_grads(self, feeds, loss_scale=1.0, zero=True, dscene_out=None, cls_weight=None, reg_weight=None,
                      fg_count=None):
     """Forward + loss + backward.  feeds additionally needs grid_pred_labels[i] int32 [N,Tp] and
-    grid_pred_regress[i] fp32 [N,Tp,h,w,2].  Returns (losses fp32 tensor [2*scales] on device in
+    grid_pred_regress[i] fp32 [N,Tp,h,w,2] - or, instead of grid_obs_regress and grid_pred_regress, the trajectory
+    feeds feeds["traj"] = dict(obs fp64 [N,T,2], pred fp64 [N,Tp,2], centers [scale] fp64 [h,w,2] (None for an unused
+    scale), soft_grid: the --soft_grid mode of the label maps, 0 for sparse labels) with int32 label cells in
+    grid_pred_labels: the offsets, targets and label maps are then computed by the kernels that read them, bit-identical
+    to the dense feeds float32(trajectory - centre) and pred_models._soft_labels.  Returns (losses fp32 tensor [2*scales] on device in
     the reference's order cls_0, reg_0, cls_1, ..., wd_loss tensor); gradients are ADDED into
     self.grads (TF variable names; zeroed first unless zero=False), WITHOUT the weight-decay term
     (added by the optimizer).  loss_scale weights this call's batch inside a larger one
@@ -443,6 +478,8 @@ class TrainEngine(ConvRNNEngine):
       part = dict(scene_feat=feeds["scene_feat"][uniq.long()].contiguous(), obs_scene=inv.to(torch.int32))
       for key in ("grid_obs_labels", "grid_obs_regress", "grid_pred_labels", "grid_pred_regress"):
         part[key] = [None if a is None else a[sl] for a in feeds[key]]
+      if feeds.get("traj") is not None:
+        part["traj"] = dict(feeds["traj"], obs=feeds["traj"]["obs"][sl], pred=feeds["traj"]["pred"][sl])
       if feeds.get("mixup") is not None:
         mx = feeds["mixup"]
         part["mixup"] = dict(beta=mx["beta"], obs_labels2=[None if a is None else a[sl] for a in mx["obs_labels2"]],
