@@ -382,6 +382,30 @@ int mvb_min_ade_fde(const float* pred, const float* gt, const int32_t* gt_len, d
  *   logits fp32 [N,K,Tp,V] and logprobs fp32 [N,K] = beam_outputs[0], [2]; gt_idx int32 [N,J,G]; steps int32 [J]. */
 int mvb_beam_nll(const float* logits, const float* logprobs, const int32_t* gt_idx, const int32_t* steps, double* nll,
                  int32_t* count, int64_t N, int K, int Tp, int V, int J, int G, void* stream);
+/* mvb_beam_nll of a batch whose rows end at their own lengths (lengths int32 [N], the decode's out["_lengths"]):
+ * logits [N,K,Tp,V] as the ragged decode leaves them (zeros after each row's length), and a step steps[j] >=
+ * lengths[n] is not evaluated for row n (count 0).  With every length Tp it equals mvb_beam_nll bit for bit. */
+int mvb_beam_nll_ragged(const float* logits, const float* logprobs, const int32_t* lengths, const int32_t* gt_idx,
+                        const int32_t* steps, double* nll, int32_t* count, int64_t N, int K, int Tp, int V, int J,
+                        int G, void* stream);
+/* mvb_min_ade_fde on the decode's selections instead of fp32 points: prediction k's point at step t is
+ *   centers[ids[n,k,t]] + (double)offsets[n,k,t]    (center_only: centers[ids[n,k,t]])
+ * one fp64 add, as multifuture_inference.py:504-517 forms it on float64 centres, against fp64 ground truth
+ * gt [N,G,Tg,2] (gt_len [N,G], 0 = absent).  Same selections and errors as mvb_min_ade_fde (shared code); greedy
+ * decodes are K = 1.  ids int32 [N,K,Tp] (beam_outputs[1] or the arg-max), offsets fp32 [N,K,Tp,2]
+ * (mvb_gather_offsets; unread with center_only, may be NULL), centers fp64 [V,2], lengths int32 [N] (the rows'
+ * prediction lengths).  *err |= 1 for a future longer than its row's predictions (or a row longer than Tp), |= 2 for
+ * an id outside [0, V); such futures are not scored (index -1).  err is not cleared. */
+int mvb_min_ade_fde_cells(const int32_t* ids, const float* offsets, const double* centers, int center_only,
+                          const int32_t* lengths, const double* gt, const int32_t* gt_len, double* ade_err,
+                          int32_t* ade_idx, double* fde, int32_t* fde_idx, int32_t* err, int64_t N, int G, int K,
+                          int Tp, int V, int Tg, void* stream);
+/* xys_to_indexes of code/multifuture_eval_trajs_prob.py:45-63: points fp64 [P,2] frame pixels -> cells int32 [P] =
+ * y * scene_w + x of the grid cell, per axis ceil(c / gap) with gap = video / scene in fp64, 0 counted as 1, minus
+ * one, negative indices wrapped as numpy indexes.  An index outside [-size, size) sets *err = 1 (numpy's IndexError)
+ * and that cell to -1.  err is not cleared. */
+int mvb_points_to_cells(const double* points, int32_t* cells, int32_t* err, int64_t P, int scene_h, int scene_w,
+                        int video_h, int video_w, void* stream);
 
 /* Back-trace (pred_models.py:689-764): step_ids/step_parents int32 [Tp,N,B], step_logits fp32
  * [Tp,N,B,V] -> out_ids int32 [N,B,Tp], out_logits fp32 [N,B,Tp,V]. */

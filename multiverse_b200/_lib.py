@@ -83,6 +83,10 @@ SIGNATURES = {
     "mvb_mix": [_vp, _vp, _vp, _f, _i64, _vp],
     "mvb_min_ade_fde": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp],
     "mvb_beam_nll": [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _vp],
+    "mvb_beam_nll_ragged": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i, _vp],
+    "mvb_min_ade_fde_cells": [_vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _i, _i,
+                              _vp],
+    "mvb_points_to_cells": [_vp, _vp, _vp, _i64, _i, _i, _i, _i, _vp],
     "mvb_beam_backtrace": [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],
     "mvb_beam_backtrace_ragged": [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],
     "mvb_gather_offsets": [_vp, _vp, _vp, _vp, _i64, _i, _i, _i, _vp],

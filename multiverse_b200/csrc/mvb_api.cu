@@ -121,7 +121,7 @@ static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s)
 extern "C" {
 
 const char* mvb_last_error(void) { return get_error(); }
-int mvb_abi_version(void) { return 16; }
+int mvb_abi_version(void) { return 17; }
 int mvb_cell_last_variant(void) { return cell_last_variant(); }
 long long mvb_cell_variants_seen(int reset) { return (long long)cell_variants_seen(reset); }
 long long mvb_launch_count(void) { return g_launches; }
@@ -427,7 +427,24 @@ int mvb_min_ade_fde(const float* pred, const float* gt, const int32_t* gt_len, d
 }
 int mvb_beam_nll(const float* logits, const float* logprobs, const int32_t* gt_idx, const int32_t* steps, double* nll,
                  int32_t* count, int64_t N, int K, int Tp, int V, int J, int G, void* stream) {
-  return beam_nll(logits, logprobs, gt_idx, steps, nll, count, N, K, Tp, V, J, G, S(stream));
+  return beam_nll(logits, logprobs, nullptr, gt_idx, steps, nll, count, N, K, Tp, V, J, G, S(stream));
+}
+int mvb_beam_nll_ragged(const float* logits, const float* logprobs, const int32_t* lengths, const int32_t* gt_idx,
+                        const int32_t* steps, double* nll, int32_t* count, int64_t N, int K, int Tp, int V, int J,
+                        int G, void* stream) {
+  MVB_REQUIRE(lengths, "beam_nll_ragged: null lengths");
+  return beam_nll(logits, logprobs, lengths, gt_idx, steps, nll, count, N, K, Tp, V, J, G, S(stream));
+}
+int mvb_min_ade_fde_cells(const int32_t* ids, const float* offsets, const double* centers, int center_only,
+                          const int32_t* lengths, const double* gt, const int32_t* gt_len, double* ade_err,
+                          int32_t* ade_idx, double* fde, int32_t* fde_idx, int32_t* err, int64_t N, int G, int K,
+                          int Tp, int V, int Tg, void* stream) {
+  return min_ade_fde_cells(ids, offsets, centers, center_only, lengths, gt, gt_len, ade_err, ade_idx, fde, fde_idx,
+                           err, N, G, K, Tp, V, Tg, S(stream));
+}
+int mvb_points_to_cells(const double* points, int32_t* cells, int32_t* err, int64_t P, int scene_h, int scene_w,
+                        int video_h, int video_w, void* stream) {
+  return points_to_cells(points, cells, err, P, scene_h, scene_w, video_h, video_w, S(stream));
 }
 int mvb_beam_backtrace(const int32_t* step_ids, const int32_t* step_parents,
                        const float* step_logits, int32_t* out_ids, float* out_logits, int64_t N,

@@ -102,8 +102,14 @@ int beam_band_copy(const float* base_c, const float* base_h32, const int* band, 
 // mvb_metrics.cu
 int min_ade_fde(const float* pred, const float* gt, const int* gt_len, double* ade_err, int* ade_idx, double* fde,
                 int* fde_idx, long long N, int G, int K, int Tp, int Tg, cudaStream_t stream);
-int beam_nll(const float* logits, const float* logprobs, const int* gt_idx, const int* steps, double* nll, int* count,
-             long long N, int K, int Tp, int V, int J, int G, cudaStream_t stream);
+int min_ade_fde_cells(const int* ids, const float* offs, const double* centers, int center_only, const int* lengths,
+                      const double* gt, const int* gt_len, double* ade_err, int* ade_idx, double* fde, int* fde_idx,
+                      int* err, long long N, int G, int K, int Tp, int V, int Tg, cudaStream_t stream);
+int points_to_cells(const double* points, int* cells, int* err, long long P, int scene_h, int scene_w, int video_h,
+                    int video_w, cudaStream_t stream);
+// lengths [N] may be NULL (every row Tp steps)
+int beam_nll(const float* logits, const float* logprobs, const int* lengths, const int* gt_idx, const int* steps,
+             double* nll, int* count, long long N, int K, int Tp, int V, int J, int G, cudaStream_t stream);
 
 // mvb_train.cu
 int cell_dgrad(const void* dg_planes, const void* wd_planes, float* dxh, long long NS, int H, int W,

@@ -13,6 +13,11 @@ Command line (the user's copy of the script, imported through the drop-in path, 
 data loading and the feeds):
 
   python -m multiverse_b200.multifuture <path to code/multifuture_inference.py> <its arguments> [--batch_size N]
+      [--eval]
+
+--eval also scores every batch on the device against the ground truth the script loaded (multifuture_eval.Evaluation)
+and prints what code/multifuture_eval_trajs.py and, for a beam decode, code/multifuture_eval_trajs_prob.py print for
+the pickles; the beam logits stay on the device unless --save_prob_file asks for them.
 """
 from __future__ import annotations
 
@@ -60,11 +65,12 @@ def trajectories(ids, offs, length, centers, num_out, greedy, center_only):
   return points[:num_out]
 
 
-def infer(model, per_trajectory_feeds, batch_size, args, traj_ids, with_prob=False):
+def infer(model, per_trajectory_feeds, batch_size, args, traj_ids, with_prob=False, evaluation=None):
   """(output_data, beam_prob) of the script's loop (:460-523) for its N=1 feeds `per_trajectory_feeds`
   (PredictionModelInference.get_feed_dict) of the trajectories `traj_ids`, decoded `batch_size` trajectories per
   forward.  `args`: the script's arguments after add_grid.  beam_prob (the beam logits and log-probabilities,
-  --save_prob_file) is fetched only with `with_prob`; it is {} otherwise."""
+  --save_prob_file) is fetched only with `with_prob`; it is {} otherwise.  `evaluation` (a multifuture_eval.Evaluation)
+  is given every batch's selections, offsets and beam outputs on the device."""
   import torch
   from . import ops
   cfg = model.config
@@ -92,6 +98,10 @@ def infer(model, per_trajectory_feeds, batch_size, args, traj_ids, with_prob=Fal
       else:
         ids = out["beam_outputs"][1]
       offs = ops.gather_offsets(ids, out["_offs"][gi].contiguous(), out["_lengths"])
+      if evaluation is not None:
+        m, bo = len(chunk), out.get("beam_outputs")
+        evaluation.add(traj_ids[b0:b0 + m], ids[:m], offs[:m], out["_lengths"][:m],
+                       bo[0][:m] if bo is not None else None, bo[2][:m] if bo is not None else None)
       ids_h, offs_h = ids.cpu().numpy(), offs.cpu().numpy()
       if with_prob:
         logits_h, logprobs_h = out["beam_outputs"][0].cpu().numpy(), out["beam_outputs"][2].cpu().numpy()
@@ -131,9 +141,10 @@ def model_config(args, tf):
       scene_grids=args.scene_grids, use_grids=args.use_grids)
 
 
-def prepare(script_path, script_argv, load_weights=True):
+def prepare(script_path, script_argv, load_weights=True, return_gt=False):
   """The script's set-up (:389-461) through its own functions: returns (args, traj_ids, model, per-trajectory
-  feeds).  load_weights=False leaves the model's initial weights (no checkpoint read)."""
+  feeds), and with return_gt the ground truth it loaded (gt_trajs: traj id -> future dict) after them.
+  load_weights=False leaves the model's initial weights (no checkpoint read)."""
   mod = load_script(script_path)
   tf = sys.modules["tensorflow"]
   args = mod.parser.parse_args(script_argv)
@@ -155,6 +166,8 @@ def prepare(script_path, script_argv, load_weights=True):
     with tf.Session() as sess:
       mod.load_model_weights(args.model_path, sess, top_scope="person_pred")
   feeds = [model.get_feed_dict(inputs, args, i) for i in range(len(traj_ids))]
+  if return_gt:
+    return args, traj_ids, model, feeds, gt_trajs
   return args, traj_ids, model, feeds
 
 
@@ -179,16 +192,39 @@ def split_argv(argv):
   return argv[0], rest, batch
 
 
+def split_eval(argv):
+  """(argv without --eval, whether it was given)."""
+  rest = [a for a in argv if a != "--eval"]
+  return rest, len(rest) != len(argv)
+
+
+def make_evaluation(model, args, gt_trajs):
+  """The multifuture_eval.Evaluation of this decode: the decoded scale's centres and grid, the script's frame size;
+  NLL only for a beam decode (the greedy one has no beam logits)."""
+  from . import multifuture_eval
+  cfg = model.config
+  gi = list(cfg.use_grids).index(True)
+  return multifuture_eval.Evaluation(gt_trajs, args.scene_grid_centers[gi], args.center_only, cfg.scene_grids[gi],
+                                     (args.video_h, args.video_w), with_nll=bool(cfg.use_beam_search))
+
+
 def main(argv=None):
-  script, script_argv, batch = split_argv(sys.argv[1:] if argv is None else argv)
-  args, traj_ids, model, feeds = prepare(script, script_argv)
+  argv, evaluate = split_eval(sys.argv[1:] if argv is None else argv)
+  script, script_argv, batch = split_argv(argv)
+  args, traj_ids, model, feeds, gt_trajs = prepare(script, script_argv, return_gt=True)
   with_prob = args.save_prob_file is not None
-  output_data, beam_prob = infer(model, feeds, batch, args, traj_ids, with_prob=with_prob)
+  evaluation = make_evaluation(model, args, gt_trajs) if evaluate else None
+  if evaluate and not args.use_beam_search:
+    print("--eval: no NLL for --greedy (it has no beam logits)", file=sys.stderr)
+  output_data, beam_prob = infer(model, feeds, batch, args, traj_ids, with_prob=with_prob, evaluation=evaluation)
   with open(args.output_file, "wb") as f:
     pickle.dump(output_data, f)
   if with_prob:
     with open(args.save_prob_file, "wb") as f:
       pickle.dump(beam_prob, f)
+  if evaluation is not None:
+    for line in evaluation.lines():
+      print(line)
 
 
 if __name__ == "__main__":

@@ -638,6 +638,52 @@ def beam_nll(logits, logprobs, gt_idx, steps):
   return nll, cnt
 
 
+def beam_nll_ragged(logits, logprobs, lengths, gt_idx, steps):
+  """beam_nll of a ragged decode: logits fp32 [N,K,Tmax,V] and logprobs fp32 [N,K] as forward(pred_lengths=...) returns
+  them, lengths int32 [N] (its out["_lengths"]); a step at or past a row's length is not evaluated (count 0)."""
+  n, k, tp, v = logits.shape
+  j, g = gt_idx.shape[1], gt_idx.shape[2]
+  assert lengths.dtype == torch.int32 and lengths.numel() == n
+  nll = torch.empty((n, j), dtype=torch.float64, device=logits.device)
+  cnt = torch.empty((n, j), dtype=torch.int32, device=logits.device)
+  _lib.call("mvb_beam_nll_ragged", _p(logits), _p(logprobs), _p(lengths), _p(gt_idx), _p(steps), _p(nll), _p(cnt), n,
+            k, tp, v, j, g, _stream())
+  return nll, cnt
+
+
+def min_ade_fde_cells(ids, offs, centers, lengths, gt, gt_len, center_only=False):
+  """ids int32 [N,K,Tp], offs fp32 [N,K,Tp,2] (gather_offsets), centers fp64 [V,2], lengths int32 [N], gt fp64
+  [N,G,Tg,2], gt_len int32 [N,G] -> (ade_err fp64 [N,G,Tg], ade_idx, fde fp64 [N,G], fde_idx, err int32 [1]):
+  min_ade_fde on the points centre + offset formed in fp64 (centre alone with center_only).  err bit 1: a future
+  longer than its row's predictions; bit 2: a cell id outside the centres."""
+  n, k, tp = ids.shape
+  g, tg = gt.shape[1], gt.shape[2]
+  assert offs.shape == (n, k, tp, 2) and centers.dtype == torch.float64 and gt.dtype == torch.float64
+  assert lengths.dtype == torch.int32 and gt_len.dtype == torch.int32 and ids.dtype == torch.int32
+  dev = ids.device
+  ade_err = torch.empty((n, g, tg), dtype=torch.float64, device=dev)
+  ade_idx = torch.empty((n, g), dtype=torch.int32, device=dev)
+  fde = torch.empty((n, g), dtype=torch.float64, device=dev)
+  fde_idx = torch.empty((n, g), dtype=torch.int32, device=dev)
+  err = torch.zeros(1, dtype=torch.int32, device=dev)
+  _lib.call("mvb_min_ade_fde_cells", _p(ids), _p(offs), _p(centers), int(bool(center_only)), _p(lengths), _p(gt),
+            _p(gt_len), _p(ade_err), _p(ade_idx), _p(fde), _p(fde_idx), _p(err), n, g, k, tp, centers.shape[0], tg,
+            _stream())
+  return ade_err, ade_idx, fde, fde_idx, err
+
+
+def points_to_cells(points, scene_h, scene_w, video_h, video_w):
+  """points fp64 [..., 2] frame pixels -> (cells int32 [...], err int32 [1]): xys_to_indexes of
+  code/multifuture_eval_trajs_prob.py:45-63 (err 1: an index numpy would refuse; that cell is -1)."""
+  assert points.dtype == torch.float64 and points.shape[-1] == 2
+  cells = torch.empty(points.shape[:-1], dtype=torch.int32, device=points.device)
+  err = torch.zeros(1, dtype=torch.int32, device=points.device)
+  if cells.numel():
+    _lib.call("mvb_points_to_cells", _p(points), _p(cells), _p(err), cells.numel(), int(scene_h), int(scene_w),
+              int(video_h), int(video_w), _stream())
+  return cells, err
+
+
 def traj_to_grid(traj, centers, h_gap, w_gap, labels, regress, h, w):
   """traj fp64 [...,2], centers fp64 [h*w,2] -> labels int32 [...], regress fp32 [...,h,w,2]."""
   _lib.call("mvb_traj_to_grid", _p(traj), _p(centers), float(h_gap), float(w_gap), _p(labels), _p(regress),
