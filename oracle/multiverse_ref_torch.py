@@ -97,15 +97,17 @@ def decoder_greedy(first, state, tp, cell_w, emb_w, head_w, scene_mean, mask, us
 
 
 def decoder_beam(first, state, tp, b, cell_w, emb_w, head_w, scene_mean, mask, diverse, gamma,
-                 fix_num_timestep, margins=None):
+                 fix_num_timestep, margins=None, trace=None):
   """Model.grid_decoder_beam_search, code/pred_models.py:474-806 (diverse rank through a full
-  sort, as add_div_penalty :1197-1223 does)."""
+  sort, as add_div_penalty :1197-1223 does).  Runs on the device of `state`; scene_mean None: the attention sees h
+  alone (models without scene encoding).  trace: a list that receives (ids, parents, logits) of every step."""
   c0, h0 = state
   n, hh, ww, _ = h0.shape
   v = hh * ww
-  rep = lambda t: t.repeat_interleave(b, dim=0)
+  dev = h0.device
+  rep = lambda t: None if t is None else t.repeat_interleave(b, dim=0)
   c, h, inp, sm = rep(c0), rep(h0), rep(first), rep(scene_mean)
-  score = torch.zeros(n, b, dtype=h0.dtype)
+  score = torch.zeros(n, b, dtype=h0.dtype, device=dev)
   ids_l, par_l, log_l = [], [], []
 
   def step(inp, c, h):
@@ -118,7 +120,7 @@ def decoder_beam(first, state, tp, b, cell_w, emb_w, head_w, scene_mean, mask, d
     if diverse:
       order = torch.argsort(lp, dim=-1, descending=True, stable=True)
       rank = torch.empty_like(order)
-      rank.scatter_(-1, order, torch.arange(v).expand_as(order))
+      rank.scatter_(-1, order, torch.arange(v, device=dev).expand_as(order))
       lp = lp + math.log(gamma) * rank.to(lp.dtype)
     cand = lp.reshape(n, b * v) if time > 1 else lp[:, 0]
     sc, idx = torch.topk(cand, b, dim=-1, sorted=True)
@@ -129,17 +131,19 @@ def decoder_beam(first, state, tp, b, cell_w, emb_w, head_w, scene_mean, mask, d
       sc = torch.zeros_like(sc)
     ids, par = idx % v, idx // v
     ids_l.append(ids); par_l.append(par); log_l.append(logits)
+    if trace is not None:
+      trace.append((ids, par, logits))
     score = sc
-    flat = (par + (torch.arange(n) * b)[:, None]).reshape(-1)
+    flat = (par + (torch.arange(n, device=dev) * b)[:, None]).reshape(-1)
     c, h = c[flat], h[flat]
     inp = one_hot_map(ids.reshape(-1), hh, ww, h0.dtype)
     if time == tp:
       break
     c, h = step(inp, c, h)
-  parents = torch.arange(b)[None].repeat(n, 1)
-  rows = torch.arange(n)[:, None]
-  out_ids = torch.zeros(n, b, tp, dtype=torch.long)
-  out_logits = torch.zeros(n, b, tp, v, dtype=h0.dtype)
+  parents = torch.arange(b, device=dev)[None].repeat(n, 1)
+  rows = torch.arange(n, device=dev)[:, None]
+  out_ids = torch.zeros(n, b, tp, dtype=torch.long, device=dev)
+  out_logits = torch.zeros(n, b, tp, v, dtype=h0.dtype, device=dev)
   for tau in range(tp - 1, -1, -1):
     out_ids[:, :, tau] = ids_l[tau][rows, parents]
     out_logits[:, :, tau] = log_l[tau][rows, parents]

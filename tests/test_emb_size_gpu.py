@@ -19,6 +19,7 @@ import pytest
 import torch
 
 import test_kernels_atsize_gpu as K
+from beam_truth import beam_replay
 from test_beam_no_gnn_gpu import rel, to_dev
 
 pytestmark = pytest.mark.gpu
@@ -281,51 +282,6 @@ def test_rollout_greedy_two_scale_wide_emb(dev, emb):
     errs["offsets_%d" % i] = rel(_np(out["grid_pred_reg_decoded"][i]), _np(ref["grid_pred_reg_decoded"][i]))
   print("greedy emb %d: cell variants %s, rel errs %s" % (emb, sorted(seen), {k: "%.1e" % v for k, v in errs.items()}))
   assert max(errs.values()) < 1e-4, errs
-
-
-def beam_replay(cfg, weights, feeds, i, step_ids, step_par, device):
-  """The fp64 truth of the beam decoder of scale i (RT.decoder_beam's steps) with its selections given: the cells
-  step_ids[t] and parent beams step_par[t] [N,K] of every step, e.g. an engine's trace.  Returns the logits [Tp,N,K,V]
-  every live beam row computes along those selections.  Without scene encoding: no_scene_enc_ref.beam_replay."""
-  import torch.nn.functional as F
-  import no_scene_enc_ref as NS
-  from oracle import multiverse_ref as R
-  from oracle import multiverse_ref_torch as RT
-  if not cfg.use_scene_enc:
-    return NS.beam_replay(cfg, weights, feeds, i, step_ids, step_par, device=device)
-  dt = torch.float64
-  w = {k: torch.from_numpy(np.ascontiguousarray(v)).to(device=device, dtype=dt) for k, v in weights.items()}
-  n, b = cfg.batch_size, cfg.beam_size
-  h, ww = cfg.scene_grids[i]
-  x = torch.from_numpy(feeds["scene_feat"]).to(device=device, dtype=dt)[torch.from_numpy(feeds["obs_scene"]).long()
-                                                                          .reshape(-1).to(device)]
-  for j in range(i + 1):
-    x = torch.tanh(RT.conv2d_same(x, w["person_pred/scene_conv%d/W" % (j + 1)], 2) + w["person_pred/scene_conv%d/b" % (j + 1)])
-  conv = x.reshape((n, -1) + tuple(x.shape[1:]))
-  sw = R.scale_weights(w, i)
-  labels = torch.from_numpy(np.asarray(feeds["grid_obs_labels"][i])).to(device).long()
-  obs = F.one_hot(labels, h * ww).to(dt).reshape(n, -1, h, ww, 1)
-  c, hs = RT.encoder(conv * obs, sw.enc_class[0], sw.enc_class[1], cfg.enc_hidden_size, device)
-  mask = RT.neighbour_mask(h, ww, dt, device) if cfg.use_gnn else None
-  sm = conv.mean(1)
-
-  def step(inp, c, hs, sm):
-    h_in = RT.gnn_dense(hs, sm, mask) if cfg.use_gnn else hs
-    return RT.convlstm_cell(RT.grid_emb(inp, *sw.emb_class), c, h_in, *sw.dec_class)
-
-  c, hs = step(obs[:, -1], c, hs, sm)                      # time 0: the K beams of a sample are identical
-  c, hs, sm = c.repeat_interleave(b, 0), hs.repeat_interleave(b, 0), sm.repeat_interleave(b, 0)
-  base = torch.arange(n, device=device)[:, None] * b
-  out = []
-  for t in range(len(step_ids)):
-    out.append(RT.conv2d_same(hs, sw.head_class).reshape(n, b, -1))
-    flat = (torch.as_tensor(np.asarray(step_par[t])).to(device).long() + base).reshape(-1)
-    c, hs = c[flat], hs[flat]
-    if t == len(step_ids) - 1:
-      break
-    inp = RT.one_hot_map(torch.as_tensor(np.asarray(step_ids[t])).reshape(-1), h, ww, dt, device)
-    c, hs = step(inp, c, hs, sm)
-  return torch.stack(out).cpu().numpy()
 
 
 def golden_case(name):
