@@ -34,8 +34,10 @@ DEFAULT_BATCH = 256
 
 
 def batch_feeds(model, feeds):
-  """One feed dict of N rows from N of the script's N=1 feed dicts, and their lengths int32 [N]: the rows
-  concatenated, each feed's frames appended to scene_feat and its obs_scene indices offset to match."""
+  """One feed dict of N rows from the feed dicts `feeds` (the script's N=1 feeds, or get_feed_dict's batches), and
+  their lengths int32 [N]: the rows concatenated, each feed's frames appended to scene_feat and its obs_scene indices
+  offset to match.  Feeds that carry their observed trajectories (obs_traj + grid_centers, get_feed_dict's row f-1
+  path) are concatenated as those; all feeds must then carry them, with the same centres."""
   cfg = model.config
   scene, obs_scene, frames = [], [], 0
   for fd in feeds:
@@ -44,12 +46,24 @@ def batch_feeds(model, feeds):
     obs_scene.append(np.asarray(fd[model.obs_scene], dtype=np.int32) + frames)
     frames += sf.shape[0]
   out = {model.scene_feat: np.concatenate(scene), model.obs_scene: np.concatenate(obs_scene)}
+  traj = [model.obs_traj in fd for fd in feeds]
+  if any(traj) and not all(traj):
+    raise ValueError("batch_feeds: feeds with dense offsets and feeds with trajectories cannot share a forward")
+  if all(traj):
+    out[model.obs_traj] = np.concatenate([np.asarray(fd[model.obs_traj]) for fd in feeds])
   for j in range(len(cfg.scene_grids)):
     if cfg.use_grids[j]:
       out[model.grid_obs_labels[j]] = np.concatenate([np.asarray(fd[model.grid_obs_labels[j]]) for fd in feeds])
-      out[model.grid_obs_regress[j]] = np.concatenate([np.asarray(fd[model.grid_obs_regress[j]]) for fd in feeds])
-  lengths = np.array([int(np.asarray(fd[model.pred_length]).reshape(-1)[0]) for fd in feeds], dtype=np.int32)
-  return out, lengths
+      if all(traj):
+        c = feeds[0][model.grid_centers[j]]
+        if any(fd[model.grid_centers[j]] is not c and not np.array_equal(fd[model.grid_centers[j]], c) for fd in feeds):
+          raise ValueError("batch_feeds: the feeds' grid centres of scale %d differ" % j)
+        out[model.grid_centers[j]] = c
+      else:
+        out[model.grid_obs_regress[j]] = np.concatenate([np.asarray(fd[model.grid_obs_regress[j]]) for fd in feeds])
+  lengths = np.concatenate([np.broadcast_to(np.asarray(fd[model.pred_length]).reshape(-1),
+                                            (np.asarray(fd[model.obs_scene]).shape[0],)) for fd in feeds])
+  return out, lengths.astype(np.int32)
 
 
 def trajectories(ids, offs, length, centers, num_out, greedy, center_only):
@@ -113,16 +127,23 @@ def infer(model, per_trajectory_feeds, batch_size, args, traj_ids, with_prob=Fal
   return output_data, beam_prob
 
 
-def load_script(path):
-  """The user's code/multifuture_inference.py as a module, its `pred_models` and `tensorflow` the drop-in's."""
+def load_script(path, name="multifuture_inference"):
+  """The user's script at `path` as a module named `name` (run as the script with name "__main__"), its
+  `pred_models` and `tensorflow` the drop-in's and its own directory next on sys.path (its pred_utils)."""
   from . import pred_models  # noqa: F401  (puts the drop-in directory first on sys.path)
-  here = os.path.dirname(os.path.abspath(path))
-  if here not in sys.path:
-    sys.path.insert(1, here)         # after the drop-in: the script's own pred_utils
-  spec = importlib.util.spec_from_file_location("multifuture_inference", path)
+  add_script_dir(path)
+  spec = importlib.util.spec_from_file_location(name, path)
   mod = importlib.util.module_from_spec(spec)
   spec.loader.exec_module(mod)
   return mod
+
+
+def add_script_dir(path):
+  """The script's directory on sys.path right after the drop-in's, so that its own modules (pred_utils) import."""
+  from . import pred_models  # noqa: F401
+  here = os.path.dirname(os.path.abspath(path))
+  if here not in sys.path:
+    sys.path.insert(1, here)         # after the drop-in: the script's own pred_utils
 
 
 def model_config(args, tf):
@@ -171,24 +192,25 @@ def prepare(script_path, script_argv, load_weights=True, return_gt=False):
   return args, traj_ids, model, feeds
 
 
-def split_argv(argv):
-  """(script path, the script's arguments, batch size) from this module's command line."""
+def split_argv(argv, flag="--batch_size", default=DEFAULT_BATCH,
+               usage="python -m multiverse_b200.multifuture <multifuture_inference.py> <its arguments> "
+                     "[--batch_size N]"):
+  """(script path, the script's arguments, this module's value of `flag`) from this module's command line."""
   if not argv or argv[0].startswith("-"):
-    raise SystemExit("usage: python -m multiverse_b200.multifuture <multifuture_inference.py> <its arguments> "
-                     "[--batch_size N]")
-  rest, batch, i = [], DEFAULT_BATCH, 1
+    raise SystemExit("usage: " + usage)
+  rest, batch, i = [], default, 1
   while i < len(argv):
     a = argv[i]
-    if a == "--batch_size":
+    if a == flag:
       batch, i = int(argv[i + 1]), i + 2
       continue
-    if a.startswith("--batch_size="):
+    if a.startswith(flag + "="):
       batch = int(a.split("=", 1)[1])
     else:
       rest.append(a)
     i += 1
-  if batch < 1:
-    raise SystemExit("--batch_size must be at least 1")
+  if batch is not None and batch < 1:
+    raise SystemExit("%s must be at least 1" % flag)
   return argv[0], rest, batch
 
 
